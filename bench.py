@@ -1,19 +1,25 @@
 #!/usr/bin/env python
-"""bench.py -- throughput of the batched 1-D complex FFT hot path on B200.
+"""bench.py -- throughput of the batched 1-D complex FFT hot path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2|c3|c4|c1] [--impl ours|reference]
+                    [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic input.  The default workload is
-BASELINE.json configs[1]: batched N=2^20 complex-f32 forward FFT, batch 4096, on one B200.  With
+BASELINE.json configs[1]: batched N=2^20 complex-f32 forward FFT, batch 4096, on one H100.  With
 --gpus N>1 (launched by torchrun, one rank per GPU) every rank transforms its own batch of the same
 size (independent transforms, no data-path collective): weak scaling.
 
 Prints ONE JSON line (rank 0).  `value` is whole-job complex samples/s with inputs resident in HBM;
 `e2e` is the same metric through the C-ABI call with HOST (pinned) buffers, copies inside the timed
 region; `roofline` relates the dominant kernel's algorithmic bytes (16 B/sample f32, 32 B/sample
-f64: read once + write once, SURVEY.md 8d) to the measured HBM peak; `cpu_baseline` is the oracle
-(C restatement of the reference CPU algorithm; the Rust reference cannot be built in this image)
-timed on the host cores on a bounded sample.
+f64: read once + write once, SURVEY.md 8d) to the HBM peak (MEASURED_PEAKS.json when present, else the
+H100 SXM data sheet's 3.35 TB/s); `cpu_baseline` is the oracle (C restatement of the reference CPU
+algorithm; the Rust reference needs a Rust toolchain) timed on the host cores on a bounded sample.
+
+--dump-outputs DIR writes, after the timed steps, the output of the last timed step as DIR/y.npy (float32 or
+float64, real and imaginary parts in the last axis).  Outputs above 30 MB are sampled at fixed, seeded positions
+of the flattened output, listed in DIR/y_index.npy.  The input is generated from a fixed hash, so two builds run
+with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -31,7 +37,8 @@ WORKLOADS = {
     # name: (N, per-GPU batch, real, description)
     "c1": (1024, 1, "f32", "single 1024-pt c-f32 forward (BASELINE configs[0], correctness gate)"),
     "c2": (1 << 20, 4096, "f32", "batched N=2^20 c-f32 forward, batch 4096 per GPU (BASELINE configs[1])"),
-    "c3": (1 << 16, 65536, "f64", "batched N=2^16 c-f64 forward, batch 65536 (BASELINE configs[2])"),
+    # 32768 x 2^16 f64 = 32 GiB per buffer: input and output together fill 64 of the H100's 80 GB
+    "c3": (1 << 16, 32768, "f64", "batched N=2^16 c-f64 forward, batch 32768 (BASELINE configs[2])"),
     "c4": (1009, 1 << 20, "f32", "prime N=1009 Bluestein c-f32 forward, batch 2^20 (BASELINE configs[3])"),
     "c5": (1 << 30, 1, "f32", "single distributed N=2^30 c-f32 over all ranks, six-step with NCCL all-to-all "
                               "transposes (BASELINE configs[4])"),
@@ -39,27 +46,33 @@ WORKLOADS = {
 BYTES_PER_SAMPLE = {"f32": 16, "f64": 32}  # algorithmic: read once + write once
 
 
-def measured_traffic(workload):
-    """DRAM bytes per sample of the dominant kernel from the committed ncu capture (profiles/), or None."""
-    try:
-        for name in ("r02_traffic.json", "r01_traffic.json"):
-            path = os.path.join(ROOT, "profiles", name)
-            if os.path.exists(path):
-                with open(path) as f:
-                    d = json.load(f)
-                if workload in d:
-                    return d[workload]
-        return None
-    except Exception:
-        return None
-
-
 def measured_peak():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
+
+
+DUMP_BYTES = 30 << 20   # per dumped array; the sample's index file adds at most as much again (64 MB in all)
+
+
+def dump_outputs(directory, y):
+    """Writes the complex tensor `y` (on the GPU) as directory/y.npy in its real precision, [..., 2] = (re, im).
+    Above DUMP_BYTES a fixed, seeded sample of positions of the flattened tensor is written instead, with the
+    positions (float64, exact below 2^53) in directory/y_index.npy."""
+    import torch
+    os.makedirs(directory, exist_ok=True)
+    flat = y.reshape(-1)
+    per = flat.element_size()
+    if flat.numel() * per <= DUMP_BYTES:
+        np.save(os.path.join(directory, "y.npy"), torch.view_as_real(y).cpu().numpy())
+        return
+    k = DUMP_BYTES // max(per, 8)
+    idx = np.unique(np.random.default_rng(20240611).integers(0, flat.numel(), size=k, dtype=np.int64))
+    got = flat.index_select(0, torch.from_numpy(idx).to(flat.device))
+    np.save(os.path.join(directory, "y.npy"), torch.view_as_real(got).cpu().numpy())
+    np.save(os.path.join(directory, "y_index.npy"), idx.astype(np.float64))
 
 
 class ClockSampler:
@@ -210,17 +223,16 @@ def numa_bind(local_rank):
         return prev, f"not bound ({type(e).__name__})"
 
 
-def run_distributed(args, rank, local_rank, world, barrier, log2n=None, steps=None):
+def run_distributed(args, rank, local_rank, world, barrier, log2n=None, steps=None, dump_dir=None):
     """BASELINE configs[4]: ONE transform of N = 2^30 (or 2^--log2n) samples block-distributed over the ranks.
-    Returns the record (rank 0) or None."""
+    Returns the record (rank 0) or None.  With dump_dir, rank 0 writes its block of the last timed output there."""
     import torch
     import torch.distributed as dist
     import fourier_b200 as fb
     from fourier_b200.distributed import CudaBackend, DistributedFft
     k = log2n or args.log2n
     steps = steps or args.steps
-    # N = n1 * n2: rows of length n2 = 2^16 run on the persistent two-pass kernel (0.60 ms per batch of N/P samples on
-    # 8 GPUs, against 0.87 ms for 2^15-point rows on the two-launch tile kernels: profiles/r02_c5_sweep_8gpu.json)
+    # N = n1 * n2: rows of length n2 = 2^16 run on the persistent two-pass kernel
     k2 = 16 if k >= 26 else k - k // 2
     n1, n2 = 1 << (k - k2), 1 << k2
     n = n1 * n2
@@ -247,6 +259,8 @@ def run_distributed(args, rank, local_rank, world, barrier, log2n=None, steps=No
     ms = torch.tensor([start.elapsed_time(stop)], device="cuda", dtype=torch.float64)
     if world > 1:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, cur)
     n_exchanges = 3 if natural else 2
     wire = plan.wire_bytes_per_exchange(8) * n_exchanges
     be.launches = 0          # one more, untimed transform to count this library's kernel launches per step
@@ -288,7 +302,7 @@ def run_distributed(args, rank, local_rank, world, barrier, log2n=None, steps=No
                    "note": "successive steps transform the previous result (ping-pong buffers)"},
         "nvlink": {"bytes_sent_per_gpu_per_step": wire,
                    "achieved_gbs_per_gpu_per_direction_if_exchanges_were_the_whole_step": wire / (ms_per_step * 1e-3) / 1e9,
-                   "reference_gbs": 770, "reference": "measured peer copy per direction (B200_PROFILING.md)"},
+                   "reference_gbs": 450, "reference": "H100 SXM data sheet: 900 GB/s of NVLink per GPU, 450 per direction"},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                      "traffic": None, "peak_source": peak_src,
                      "note": f"local sweeps only: {sweeps} read+write sweeps of the rank's block per step"},
@@ -296,16 +310,16 @@ def run_distributed(args, rank, local_rank, world, barrier, log2n=None, steps=No
     }
 
 
-# nominal f32 FMA peak of one B200: 148 SMs x 128 lanes x 2 flop x 1.965 GHz; the packed FFMA2 rate measured by
-# tools/ubench.cu (profiles/r01_ubench_fp_pipes.txt) is 113.4 of those 128 lanes per clock and SM
-FP32_PEAK_TFLOPS_NOMINAL = 148 * 128 * 2 * 1.965e9 / 1e12
-FP32_PEAK_TFLOPS_MEASURED = 148 * 113.4 * 2 * 1.965e9 / 1e12
+# f32 FMA peak of one H100 SXM from its data sheet (132 SMs x 128 lanes x 2 flop at boost clock), not measured
+FP32_PEAK_TFLOPS_DATASHEET = 67.0
 C4_FLOP_PER_SAMPLE = 230.0   # SURVEY.md 8(d) / BASELINE.md: two 2048-point FFTs + 3 pointwise passes per 1009 samples
 
 
-def run_batched(args, workload, batch, rank, local_rank, world, barrier, steps, scaling, keep_output=False):
+def run_batched(args, workload, batch, rank, local_rank, world, barrier, steps, scaling, keep_output=False,
+                dump_dir=None):
     """One batched workload on every rank (each its own shard of the global synthetic batch, no collective).
-    Returns (record or None on rank != 0, plan, x, y) -- the buffers only when keep_output."""
+    Returns (record or None on rank != 0, plan, x, y) -- the buffers only when keep_output.  With dump_dir, rank 0
+    writes the output of the last timed step there."""
     import torch
     import torch.distributed as dist
     import fourier_b200 as fb
@@ -335,6 +349,8 @@ def run_batched(args, workload, batch, rank, local_rank, world, barrier, steps, 
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms_total = float(ms.item())
     ms_per_step = ms_total / steps
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, y)
     value = world * batch * n * steps / (ms_total * 1e-3)
 
     rec = None
@@ -355,7 +371,6 @@ def run_batched(args, workload, batch, rank, local_rank, world, barrier, steps, 
         peak, peak_src = measured_peak()
         bps = BYTES_PER_SAMPLE[real]
         achieved = batch * n * bps / (ms_per_step * 1e-3) / 1e9  # per GPU
-        tr = measured_traffic(workload)
         one_kernel = int(launches_per_step) == 1
         rec = {
             "metric": "batched 1D FFT complex-samples/sec", "value": value, "unit": "complex samples/s",
@@ -364,9 +379,8 @@ def run_batched(args, workload, batch, rank, local_rank, world, barrier, steps, 
             "config": workload_config(desc, n, batch, world, real),
             "plan": {"path": info["path_name"], "inner_path": info["inner_path_name"]},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": (tr["dram_bytes_per_sample"] * batch * n) if tr else None,
-                         "traffic_source": tr["source"] if tr else None,
-                         "peak_source": peak_src, "frac_of_nominal_8TBs": achieved / 8000.0,
+                         "traffic": None,
+                         "peak_source": peak_src,
                          "algorithmic_bytes_per_sample": bps,
                          "algorithmic_bytes_per_launch": batch * n * bps,
                          "kernel": (plan.kernel_name() + " -- one launch = one step (whole batch)") if one_kernel
@@ -381,9 +395,8 @@ def run_batched(args, workload, batch, rank, local_rank, world, barrier, steps, 
             tf = C4_FLOP_PER_SAMPLE * (value / world) / 1e12
             rec["roofline"].update({
                 "hbm_frac": achieved / peak, "flop_per_sample_nominal": C4_FLOP_PER_SAMPLE, "achieved_tflops": tf,
-                "fma_frac": tf / FP32_PEAK_TFLOPS_MEASURED, "fma_frac_of_nominal": tf / FP32_PEAK_TFLOPS_NOMINAL,
-                "fma_peak_tflops": FP32_PEAK_TFLOPS_MEASURED,
-                "fma_peak_source": "packed FFMA2 issue rate measured by tools/ubench.cu (113.4 of 128 lanes/clk/SM)"})
+                "fma_frac": tf / FP32_PEAK_TFLOPS_DATASHEET, "fma_peak_tflops": FP32_PEAK_TFLOPS_DATASHEET,
+                "fma_peak_source": "H100 SXM data sheet (67 TFLOP/s FP32), not measured"})
     if keep_output:
         return rec, plan, x, y
     plan.close()
@@ -403,7 +416,7 @@ def run_e2e(args, plan, x, y, n, real, batch, rank, local_rank, world, barrier):
     hx = torch.empty((eb, n), dtype=cdt).pin_memory()
     hy = torch.empty((eb, n), dtype=cdt).pin_memory()
     hx.copy_(x[:eb])
-    e2e_steps = max(2, min(args.steps, 5))
+    e2e_steps = args.steps
     for _ in range(2):
         plan.transform(hx, hy, fb.Transform.Fft)  # warm-up (allocates staging)
     barrier()
@@ -476,6 +489,8 @@ def main():
                          "(c3,c4,c5,latency; 'none'); default: all that apply to this GPU count when the "
                          "workload is the default c2 at its full batch")
     ap.add_argument("--verify", type=int, default=4, help="transforms checked against the oracle")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the output of the last timed step as DIR/y.npy (sampled above 30 MB)")
     ap.add_argument("--log2n", type=int, default=30, help="c5 only: log2 of the distributed transform length")
     ap.add_argument("--transposed-output", action="store_true",
                     help="c5 only: leave the result transposed (2 exchanges instead of 3)")
@@ -516,7 +531,7 @@ def main():
         torch.cuda.synchronize()
 
     if args.workload == "c5":
-        rec = run_distributed(args, rank, local_rank, world, barrier)
+        rec = run_distributed(args, rank, local_rank, world, barrier, dump_dir=args.dump_outputs)
         if rank == 0:
             print(json.dumps(rec))
         if world > 1:
@@ -526,7 +541,8 @@ def main():
     if args.workload == "c3" and not args.batch:
         batch = max(1, batch // world)   # BASELINE configs[2]: the batch of 65536 is sharded over the GPUs
     out, plan, x, y = run_batched(args, args.workload, batch, rank, local_rank, world, barrier, args.steps,
-                                  "strong" if args.workload == "c3" else "weak", keep_output=True)
+                                  "strong" if args.workload == "c3" else "weak", keep_output=True,
+                                  dump_dir=args.dump_outputs)
     e2e = None if args.no_e2e else run_e2e(args, plan, x, y, n, real, batch, rank, local_rank, world, barrier)
     plan.close()
     del x, y
@@ -538,13 +554,13 @@ def main():
     else:
         wanted = [w for w in args.also.split(",") if w and w != "none"]
     also = []
-    sub_steps = max(3, min(args.steps, 10))
+    sub_steps = args.steps
     for w in wanted:
         rec = None
-        if w == "c3":       # configs[2]: batch 65536 sharded over the GPUs (strong scaling)
+        if w == "c3":       # configs[2]: the batch sharded over the GPUs (strong scaling)
             rec, _, _, _ = run_batched(args, "c3", max(1, WORKLOADS["c3"][1] // world), rank, local_rank, world, barrier,
                                        sub_steps, "strong")
-        elif w == "c4" and world == 1:   # configs[3]: 1 x B200
+        elif w == "c4" and world == 1:   # configs[3]: 1 x H100
             rec, _, _, _ = run_batched(args, "c4", WORKLOADS["c4"][1], rank, local_rank, world, barrier, sub_steps, "weak")
         elif w == "c5" and world >= 2:   # configs[4]: one N = 2^30 transform over all ranks
             rec = run_distributed(args, rank, local_rank, world, barrier, log2n=30, steps=sub_steps)

@@ -1,6 +1,6 @@
 """fourier_b200 -- Python mirror of the `fourier` crate's public surface over libfourier.so.
 
-The product is the C-ABI library (include/fourier.h, include/fourier_b200.h; hand-written sm_100a
+The product is the C-ABI library (include/fourier.h, include/fourier_b200.h; hand-written sm_90a
 CUDA).  This module is the thin host-side binding used by the tests and the benchmark; it mirrors the
 reference's operator interface name for name:
 

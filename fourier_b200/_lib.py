@@ -37,7 +37,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python -m fourier_b200.build` "
-            "(nvcc, sm_100a). fourier_b200 has no CPU or PyTorch fallback.")
+            "(nvcc, sm_90a). fourier_b200 has no CPU or PyTorch fallback.")
     L = ctypes.CDLL(LIB_PATH)
     vp, sz, ci = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int
     for t in ("float", "double"):

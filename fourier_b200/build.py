@@ -1,11 +1,11 @@
-"""Builds libfourier.so (hand-written sm_100a CUDA + the C ABI) in-tree with nvcc.
+"""Builds libfourier.so (hand-written sm_90a CUDA + the C ABI) in-tree with nvcc.
 
     python -m fourier_b200.build [--force]
 
 Output: fourier_b200/lib/libfourier.so.0.1.0 with SONAME libfourier.so.0 and the usual symlinks
 (the reference's cdylib is named `fourier` with SONAME libfourier.so.0:
 fourier-ffi/CMakeLists.txt:15-19,55-65).  Objects go to build/ (git-ignored).  nvcc cross-compiles
-without a GPU; the resulting .so travels to the GPU box with the repo snapshot.
+without a GPU.
 """
 import os
 import shutil
@@ -24,9 +24,11 @@ REAL = f"libfourier.so.{VERSION}"
 
 SOURCES = ["plan.cu", "host_math.cu", "stockham_generic.cu", "onchip.cu", "cta_fft.cu", "twopass.cu", "synth.cu", "exchange.cu", "dist_fft.cu", "bigpow2.cu", "capi.cu"]
 
+# H100: the kernels use TMA and mbarrier, so the arch-specific target is required
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
     "-std=c++17", "-O3", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *GENCODE,
     "-Xcompiler", "-fPIC,-fvisibility=hidden",
     "--expt-relaxed-constexpr",
     "-diag-suppress", "20012",
@@ -82,7 +84,7 @@ def build(force=False, verbose=False):
         list(ex.map(run, jobs))
     out = lib_path()
     if force or jobs or _stale(out, objs):
-        run([exe, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-Xlinker", f"-soname={SONAME}",
+        run([exe, "-shared", *GENCODE, "-Xlinker", f"-soname={SONAME}",
              "-o", out] + objs)
         for link in (SONAME, "libfourier.so"):
             lp = os.path.join(LIBDIR, link)

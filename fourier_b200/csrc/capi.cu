@@ -295,6 +295,6 @@ int fourier_b200_twiddle_rows_double(void* data, size_t rows, size_t cols, unsig
 }
 
 const char* fourier_b200_last_error(void) { return fb200::last_error(); }
-const char* fourier_b200_version(void) { return "fourier-b200 0.1.0 (sm_100a)"; }
+const char* fourier_b200_version(void) { return "fourier-b200 0.1.0 (sm_90a)"; }
 
 }  // extern "C"

@@ -30,54 +30,13 @@ template <typename T> using cpx = typename C2<T>::type;
 
 template <typename T> FB_HD cpx<T> mk(T re, T im) { cpx<T> r; r.x = re; r.y = im; return r; }
 
-// On sm_100 a complex<float> is one 64-bit register pair and add / mul / fma exist as packed
-// two-lane instructions (FADD2 / FMUL2 / FFMA2; operands can be a pair, a swapped pair, or one scalar
-// broadcast to both lanes).  Measured on B200 (profiles/r01_ubench_fp_pipes.txt): packed ops keep the
-// 128 lane-ops/clk/SM of the FP32 pipe with HALF the issue slots, and FFMA2 runs at 113 lane-FMAs/clk
-// where scalar 3-register FFMA only reaches 70.  The FFT butterflies are therefore written on pairs.
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 1000)
-#define FB_PACKED_F32 1
-#else
-#define FB_PACKED_F32 0
-#endif
-
-FB_HD float2 cadd(float2 a, float2 b) {
-#if FB_PACKED_F32
-  return __fadd2_rn(a, b);
-#else
-  return make_float2(a.x + b.x, a.y + b.y);
-#endif
-}
-FB_HD float2 csub(float2 a, float2 b) {
-#if FB_PACKED_F32
-  return __fadd2_rn(a, make_float2(-b.x, -b.y));   // folds into a negated FADD2 operand
-#else
-  return make_float2(a.x - b.x, a.y - b.y);
-#endif
-}
-// a * b = a.x * (b.x, b.y) + a.y * (-b.y, b.x)
-FB_HD float2 cmul(float2 a, float2 b) {
-#if FB_PACKED_F32
-  return __ffma2_rn(make_float2(a.x, a.x), b, __fmul2_rn(make_float2(a.y, a.y), make_float2(-b.y, b.x)));
-#else
-  return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x);
-#endif
-}
-// a * conj(b) = a.x * (b.x, -b.y) + a.y * (b.y, b.x)
-FB_HD float2 cmulc(float2 a, float2 b) {
-#if FB_PACKED_F32
-  return __ffma2_rn(make_float2(a.x, a.x), make_float2(b.x, -b.y), __fmul2_rn(make_float2(a.y, a.y), make_float2(b.y, b.x)));
-#else
-  return make_float2(a.x * b.x + a.y * b.y, a.y * b.x - a.x * b.y);
-#endif
-}
-FB_HD float2 cscale(float2 a, float s) {
-#if FB_PACKED_F32
-  return __fmul2_rn(a, make_float2(s, s));
-#else
-  return make_float2(a.x * s, a.y * s);
-#endif
-}
+// complex<float> arithmetic is scalar FP32: Hopper has no packed two-lane FADD2 / FFMA2, and the products below
+// contract into FFMA.
+FB_HD float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+FB_HD float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
+FB_HD float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
+FB_HD float2 cmulc(float2 a, float2 b) { return make_float2(a.x * b.x + a.y * b.y, a.y * b.x - a.x * b.y); }
+FB_HD float2 cscale(float2 a, float s) { return make_float2(a.x * s, a.y * s); }
 
 FB_HD double2 cadd(double2 a, double2 b) { return make_double2(a.x + b.x, a.y + b.y); }
 FB_HD double2 csub(double2 a, double2 b) { return make_double2(a.x - b.x, a.y - b.y); }

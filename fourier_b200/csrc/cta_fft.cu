@@ -78,7 +78,7 @@ cudaError_t upload(DeviceBuffer& buf, const std::vector<cpx<T>>& host) {
 }
 
 int sm_count() {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return sms;

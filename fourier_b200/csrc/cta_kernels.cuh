@@ -150,8 +150,7 @@ template <typename T> struct Args {
 
 // One stage of the group's transforms for thread `tid` of `nthreads`: FWD = direction of this FFT's twiddles,
 // DIR = direction of the user's transform (chirp / W conjugation in CHIRP mode).  `tw` = the stage's twiddle block.
-// Index arithmetic (the first version of this kernel issued more integer than floating-point instructions,
-// profiles/r02_cta_kernel_ncu.txt): with per = len / R the R inputs of butterfly q sit at q + k*per and its outputs
+// Index arithmetic (the first version of this kernel issued more integer than floating-point instructions): with per = len / R the R inputs of butterfly q sit at q + k*per and its outputs
 // at w0 + k*stride, w0 = i*R*stride + j -- both linear in k; the pad term e >> 5 is linear too whenever per
 // (stride) is a multiple of 32, and absent when the buffers are not padded at all (PAD = false: first radix odd,
 // whose stride-1 writes are conflict-free as they are).  The source / destination kind is tested once per

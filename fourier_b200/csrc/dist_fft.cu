@@ -31,8 +31,7 @@ template <typename T> struct RowsExchangeCall {
 };
 
 // Tiles of twice as many transforms where the configuration's pass-2 tile has 16 (f32) / 8 (f64): a warp's store is then
-// one 256-byte run instead of two 128-byte pieces.  Measured (profiles/r02_rows_exchange_knobs.txt, r02_c5_modes_8gpu.json):
-// N = 2^30 on 2 GPUs 12.64 -> 12.27 ms, on 8 GPUs 5.13 -> 5.15 ms (no change), one GPU (three-pass path) no change.
+// one 256-byte run instead of two 128-byte pieces.
 // Paddings are the bank-conflict-free ones (tools/emulate.cu).  FOURIER_B200_DIST_WIDE=0 selects the narrow tiles.
 template <class S, typename T> struct WideShape { using type = S; };
 template <> struct WideShape<twopass::Shape<8, 16, 16, 16, 2>, float> { using type = twopass::Shape<8, 16, 16, 32, 2>; };
@@ -72,7 +71,7 @@ cudaError_t launch_rows_exchange(const RowsExchangeCall<T>& c) {
 }
 
 template <class G, bool WIDE, typename T> cudaError_t dispatch_rows_exchange(const RowsExchangeCall<T>& c) {
-  constexpr int MORE = 2;   // +1 .. 6 % on the three-pass path, neutral on the distributed one (profiles/r02_rows_exchange_knobs.txt)
+  constexpr int MORE = 2;
   if (c.fwd) return c.twiddle ? launch_rows_exchange<G, true, 1, MORE, WIDE>(c) : launch_rows_exchange<G, true, 0, MORE, WIDE>(c);
   return c.twiddle ? launch_rows_exchange<G, false, 2, MORE, WIDE>(c) : launch_rows_exchange<G, false, 0, MORE, WIDE>(c);
 }
@@ -125,9 +124,8 @@ cudaError_t Plan<T>::exec_rows_exchange(const C* in, size_t rows, bool forward, 
   DeviceGuard guard(device_);
   int cb_shift = 0;
   while (((size_t)1 << cb_shift) < n_ / (size_t)nranks) ++cb_shift;
-  // chunks of whole tiles, two of them in flight.  Measured on 2 B200s (N = 2^28, profiles/r02_c5_fused_ab_2gpu.txt):
-  // 16 MB chunks 3.60 ms per transform, 32 MB 3.23, 64 MB 3.07 -- NVLink, not the L2 residency of the intermediate,
-  // bounds this path, and longer kernels overlap better across the two streams.  FOURIER_B200_DIST_CHUNK_MB overrides.
+  // chunks of whole tiles, two of them in flight: NVLink, not the L2 residency of the intermediate, bounds this path,
+  // and longer kernels overlap better across the two streams.  FOURIER_B200_DIST_CHUNK_MB overrides.
   size_t mb = 64;
   if (const char* e = std::getenv("FOURIER_B200_DIST_CHUNK_MB")) mb = (size_t)std::max(1, atoi(e));
   else if (const char* e2 = std::getenv("FOURIER_B200_CHUNK_MB")) mb = (size_t)std::max(1, atoi(e2));

@@ -13,8 +13,8 @@
 //     buffer, releases it (empty[g]) so the next tile's TMA overlaps ALL of the remaining work,
 //     runs stage A, exchanges through a shared buffer (one buffer, taken under a lock: the
 //     exchange is ~10% of a tile), runs stage B and stores straight from registers;
-//   * the intermediate A[k1][n2] lives in a ring of RING transforms (a few tens of MB) that stays
-//     in the 126 MB L2: pass-1 tiles of transform b may only start once pass 2 of transform b-RING
+//   * the intermediate A[k1][n2] lives in a ring of RING transforms (about 32 MB) that stays
+//     in the 50 MB L2: pass-1 tiles of transform b may only start once pass 2 of transform b-RING
 //     has consumed the slot (done2), pass-2 tiles of b once all pass-1 tiles of b are stored (done1).
 //     Every dependency points to an earlier queue position, so the scheme cannot deadlock.
 //
@@ -162,15 +162,15 @@ template <typename T> struct FusedArgs {
 // g % EXB, under a lock when shared); the staging buffer is released as soon as the samples are in registers.
 // The intermediate is stored in 8 x 8 blocks [k1 / 8][n2 / 8][k1 % 8][n2 % 8]: a pass-1 tile writes 256-byte runs (a
 // warp's store = 4 consecutive k1 x 8 columns; row-major A[k1][n2] gave four 64-byte pieces and twice the LSU
-// wavefronts: measured +5 % on B200, profiles/r02_persistent_kernel_variants.txt), and a pass-2 tile (8 rows k1) is
+// wavefronts), and a pass-2 tile (8 rows k1) is
 // still one contiguous bulk copy; its threads pick their samples with the block-fast mapping (tilefft.cuh), under
 // which a warp needs only 8 different stage twiddles (broadcast loads).  The base table of the factored inter-pass
 // twiddle is [tile][p][col] (conflict-free for lanes = 8 columns x 4 p).
 // DIRECT_: no shared-memory staging: the consumers load their samples from global memory straight into registers
 //          (pass 1: the input, which the producer lane has prefetched into L2 one tile period ahead with
 //          cp.async.bulk.prefetch.tensor; pass 2: the L2-resident intermediate, ld.global.cg), one exchange buffer
-//          per group and no lock.  Wins for f64 (four 128-thread groups hide the load latency: +4 %), loses for f32
-//          (two 256-thread groups: -12 %), same profile file.
+//          per group and no lock.  Meant for f64, where four 128-thread groups can hide the load latency; the f32
+//          configurations with two 256-thread groups stage through shared memory.
 // RB_: second radix of the register tile when the tile length L = R_ * RB_ is not a square (L = 128 = 16 x 8,
 //      512 = 32 x 16): N = L^2 = 2^14, 2^18.
 // C1_: columns per pass-1 tile (8, or 16 = two 8 x 8 block columns: then the strided input is read in 128-byte pieces
@@ -440,7 +440,7 @@ fused_twopass_kernel(const __grid_constant__ CUtensorMap in_map, const FusedArgs
         if (it > 0) mbar_wait(&ctl->empty, (it - 1) & 1);
         if constexpr (Cfg::DIRECT) {
           // The group has just started on the previous item, so it will ask for this tile one tile period from now
-          // (~5 us): long enough for HBM -> L2, short enough that the prefetched tiles of all groups (148 x G x 64 KB)
+          // (~5 us): long enough for HBM -> L2, short enough that the prefetched tiles of all groups (132 x G x 64 KB)
           // do not crowd the intermediate out of L2.
           if (wi.pass == 1) {
 #pragma unroll
@@ -527,8 +527,7 @@ fused_twopass_kernel(const __grid_constant__ CUtensorMap in_map, const FusedArgs
       mbar_arrive(&ctl->empty);
       if constexpr (!Cfg::DIRECT && PASS == 2) {
         // The intermediate rows this tile just consumed are dead: drop them from L2 instead of letting the
-        // cache write them back to HBM later (measured: without this ~80% of the intermediate is written
-        // back at RING = 8; the slot is completely rewritten before it is read again).
+        // cache write them back to HBM later (the slot is completely rewritten before it is read again).
         const unsigned char* rows = reinterpret_cast<const unsigned char*>(ring_rows);
         for (uint32_t o = (uint32_t)t * 128u; o < TILE_BYTES; o += (uint32_t)GT * 128u)
           asm volatile("discard.global.L2 [%0], 128;" ::"l"(rows + o) : "memory");

@@ -99,9 +99,8 @@ template <> const OnChipOps<float>* onchip_lookup<float>(size_t l) {
     case 256: return OnChipImpl<float, 16, 16, 16, 8, 3, 8>::ops();
     case 512: return OnChipImpl<float, 16, 32, 32, 8, 2, 8>::ops();
     case 1024:
-      // The fused Bluestein kernel parks the even half in thread-local memory (16 warps per SM, measured
-      // 1.16e11 samples/s at N=1009); FOURIER_B200_BLUESTEIN_LOCAL=0 selects the shared-memory stash
-      // (11 warps per SM, 1.01e11).
+      // The fused Bluestein kernel parks the even half in thread-local memory (16 warps per SM);
+      // FOURIER_B200_BLUESTEIN_LOCAL=0 selects the shared-memory stash (11 warps per SM).
       if (const char* e = std::getenv("FOURIER_B200_BLUESTEIN_LOCAL"); e && atoi(e) == 0)
         return OnChipImpl<float, 32, 32, 32, 8, 2, 11>::ops();
       return OnChipImpl<float, 32, 32, 32, 8, 2, 16, true>::ops();
@@ -125,7 +124,7 @@ cudaError_t upload_vec(DeviceBuffer& buf, const std::vector<U>& host) {
 }
 
 int sm_count() {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return sms;

@@ -383,7 +383,7 @@ cudaError_t Plan<T>::exec_host(const C* in, C* out, size_t batch, int code) {
     if (batch * bytes_per <= kHostZeroCopyBytes && !std::getenv("FOURIER_B200_NO_ZEROCOPY")) {
       // Smallest calls: the two DMA copies cost more than the transform.  The kernels read the input from and write
       // the result to a pinned, device-mapped bounce buffer over PCIe themselves (one launch, one synchronisation;
-      // the CPU copies 2 x <= 64 KB).  Measured: 24 -> ~12 us per 1024-point call (profiles/r02_latency.txt).
+      // the CPU copies 2 x <= 64 KB).
       if (!zc_in_) {
         FB_CHECK(cudaHostAlloc(&zc_in_, kHostZeroCopyBytes, cudaHostAllocMapped));
         FB_CHECK(cudaHostAlloc(&zc_out_, kHostZeroCopyBytes, cudaHostAllocMapped));

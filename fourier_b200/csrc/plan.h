@@ -175,7 +175,7 @@ class Plan {
   const void* fast_ops_ = nullptr;   // TwoPassOps<T> / OnChipOps<T> of the selected kernel family
   size_t chunk_ = 0;                 // transforms per L2-resident chunk (two-pass)
   const void* fused_ops_ = nullptr;  // FusedOps<T>: persistent single-launch variant
-  int ring_ = 0, lag_ = 0, sm_count_ = 148;
+  int ring_ = 0, lag_ = 0, sm_count_ = 132;
   int outer_radix3_ = 0;             // kThreePass: 3 / 9 / 27 = the outer pass is a radix-3 DFT (N = 3^b * 2^k), 0 = power of two
   DeviceBuffer counters_, tbase_, tstep_, trace_;
 

@@ -113,7 +113,7 @@ chirp_out_kernel(const cpx<T>* __restrict__ work, cpx<T>* __restrict__ out,
 
 inline unsigned grid_for(size_t total) {
   size_t blocks = (total + kThreads - 1) / kThreads;
-  const size_t cap = 148u * 32u;  // grid-stride beyond 32 CTAs per SM
+  const size_t cap = 132u * 32u;  // grid-stride beyond 32 CTAs per SM
   if (blocks > cap) blocks = cap;
   if (blocks == 0) blocks = 1;
   return (unsigned)blocks;

@@ -156,7 +156,7 @@ template cudaError_t launch_pack<double>(const cpx<double>*, cpx<double>*, size_
 template <typename T>
 cudaError_t launch_swap_leading(const cpx<T>* in, cpx<T>* out, size_t a, size_t b, size_t inner, cudaStream_t s) {
   size_t blocks = (a * b * inner + 255) / 256;
-  if (blocks > 148u * 32u) blocks = 148u * 32u;
+  if (blocks > 132u * 32u) blocks = 132u * 32u;
   if (blocks == 0) return cudaSuccess;
   swap_leading_kernel<cpx<T>><<<(unsigned)blocks, 256, 0, s>>>(in, out, a, b, inner);
   return cudaGetLastError();
@@ -167,7 +167,7 @@ template <typename T>
 cudaError_t launch_twiddle_rows(cpx<T>* data, size_t rows, size_t cols, unsigned long long row0,
                                 unsigned long long n_total, bool forward, cudaStream_t s) {
   size_t blocks = (rows * cols + 255) / 256;
-  if (blocks > 148u * 32u) blocks = 148u * 32u;
+  if (blocks > 132u * 32u) blocks = 132u * 32u;
   if (blocks == 0) return cudaSuccess;
   if (forward) twiddle_rows_kernel<T, true><<<(unsigned)blocks, 256, 0, s>>>(data, rows, cols, row0, n_total);
   else twiddle_rows_kernel<T, false><<<(unsigned)blocks, 256, 0, s>>>(data, rows, cols, row0, n_total);
@@ -182,7 +182,7 @@ template <typename T>
 cudaError_t launch_fill_input(T* out, unsigned long long first_scalar, size_t count,
                               unsigned long long seed, cudaStream_t s) {
   size_t blocks = (count + 255) / 256;
-  if (blocks > 148u * 16u) blocks = 148u * 16u;
+  if (blocks > 132u * 16u) blocks = 132u * 16u;
   if (blocks == 0) blocks = 1;
   fill_kernel<T><<<(unsigned)blocks, 256, 0, s>>>(out, first_scalar, count, seed);
   return cudaGetLastError();

@@ -75,7 +75,7 @@ template <typename T> struct alignas(2 * sizeof(cpx<T>)) TwPair { cpx<T> a, b; }
 
 // The same table in 8-byte planes, for mappings in which many lanes of a warp read the SAME pair (col fast, block
 // fast): a 16-byte shared-memory load costs a wavefront per quarter-warp even when its lanes hit one address
-// (measured, profiles/r02_lsu_budget.txt: 4 per LDS.128 in pass 1, f64 pairs 8), an 8-byte load of <= 16 distinct
+// (4 per LDS.128 in pass 1, f64 pairs 8), an 8-byte load of <= 16 distinct
 // words costs one in total.  f32: [a (count cpx)][b (count cpx)];  f64: [a.x][a.y][b.x][b.y] (count doubles each).
 template <typename T> struct TwPlanes;
 template <> struct TwPlanes<float> {

@@ -9,7 +9,7 @@
 // registers, transformed by two register radix-R stages with one shared-memory exchange, and written
 // once.  The reference streams the whole array once per radix-4/8 stage -- seven sweeps at N = 2^20
 // (autosort/mod.rs:338-379, SURVEY.md 3.2); here HBM sees one read and one write per sample as long
-// as the intermediate A of a few transforms stays resident in the 126 MB L2, which is what the
+// as the intermediate A of a few transforms stays resident in the 50 MB L2, which is what the
 // chunking in exec_twopass() arranges.  All global accesses are >= 128-byte contiguous pieces:
 //   pass 1 reads  x  as C consecutive columns (C*8 B per row),  writes A[k1][n2] the same way;
 //   pass 2 reads  A  as whole contiguous rows,                  writes X as C consecutive k1.
@@ -103,46 +103,46 @@ template <class Cfg> struct FusedImpl {
 };
 
 template <typename T> const FusedOps<T>* fused_lookup(size_t n);
-// FOURIER_B200_CFG=1 selects the other load strategy (experiments; profiles/r02_persistent_kernel_variants.txt).
+// Ring (intermediates kept in L2) = 32 MB / transform size, lag = ring / 2: the ring must stay well inside the
+// H100's 50 MB L2 next to the prefetched input tiles.  Measured on one H100 SXM (700 W limit, power-capped near
+// 1.3 GHz in that run): N = 2^20 f32 ring 4 against 8 and N = 2^16 f64 ring 32 against 64 gave +20 % and +13 %.
+// FOURIER_B200_CFG=1 selects the other load strategy (experiments).
 template <> const FusedOps<float>* fused_lookup<float>(size_t n) {
   if (n == ((size_t)1 << 20)) {
     // default: two 256-thread groups, TMA staging, one shared exchange buffer taken under a lock
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<float, 32, 8, 2, 8, 2, true>>::ops(8, 4);
-    return FusedImpl<fused::FusedCfg<float, 32, 8, 2, 8, 1>>::ops(8, 4);
+    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<float, 32, 8, 2, 8, 2, true>>::ops(4, 2);
+    return FusedImpl<fused::FusedCfg<float, 32, 8, 2, 8, 1>>::ops(4, 2);
   }
   if (n == ((size_t)1 << 16)) {
-    // 256 x 256 with 16 x 16 register tiles, four 128-thread groups, 64-byte tile rows as at 2^20.  Measured on B200
-    // (profiles/r02_sizes_cta_and_2pow16.txt): TMA staging 56.5 %, direct loads 51.7 % (ring 128; 47 % at ring 64),
-    // two launches per chunk 33.9 % of the measured HBM peak.
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<float, 16, 8, 4, 8, 4, true>>::ops(128, 64);
-    return FusedImpl<fused::FusedCfg<float, 16, 8, 4, 8, 4>>::ops(128, 64);
+    // 256 x 256 with 16 x 16 register tiles, four 128-thread groups, 64-byte tile rows as at 2^20
+    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<float, 16, 8, 4, 8, 4, true>>::ops(64, 32);
+    return FusedImpl<fused::FusedCfg<float, 16, 8, 4, 8, 4>>::ops(64, 32);
   }
   if (n == ((size_t)1 << 18)) {
     // 512 x 512 with 32 x 16 register tiles: three 128-thread groups with TMA staging, or four with direct loads
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<float, 32, 8, 4, 8, 4, true, 16>>::ops(32, 16);
-    return FusedImpl<fused::FusedCfg<float, 32, 8, 3, 8, 3, false, 16>>::ops(32, 16);
+    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<float, 32, 8, 4, 8, 4, true, 16>>::ops(16, 8);
+    return FusedImpl<fused::FusedCfg<float, 32, 8, 3, 8, 3, false, 16>>::ops(16, 8);
   }
   if (n == ((size_t)1 << 14)) {
     // 128 x 128 with 16 x 8 register tiles: eight 64-thread groups
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<float, 16, 8, 8, 8, 8, true, 8>>::ops(512, 256);
-    return FusedImpl<fused::FusedCfg<float, 16, 8, 8, 8, 8, false, 8>>::ops(512, 256);
+    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<float, 16, 8, 8, 8, 8, true, 8>>::ops(256, 128);
+    return FusedImpl<fused::FusedCfg<float, 16, 8, 8, 8, 8, false, 8>>::ops(256, 128);
   }
   // Odd powers of two: N1 x 2 N1 with a different register tile per pass, same threads per FFT in both
-  // (template arguments: <T, RA, C, G, PAD1, EXB, DIRECT, RB, RA2, RB2, E1, E2>).  Ring = 64 MB / transform size.
+  // (template arguments: <T, RA, C, G, PAD1, EXB, DIRECT, RB, RA2, RB2, E1, E2>).
   if (n == ((size_t)1 << 19)) {   // 512 (32 x 16) x 1024 (32 x 32), 16-column pass-1 tiles: two 256-thread groups
-    return FusedImpl<fused::FusedCfg<float, 32, 8, 2, 0, 1, false, 16, 32, 32, 32, 32, 16, true>>::ops(32, 16);   // 39 % (ring 16: 35 %, tile kernels 29 %)
+    return FusedImpl<fused::FusedCfg<float, 32, 8, 2, 0, 1, false, 16, 32, 32, 32, 32, 16, true>>::ops(8, 4);
   }
   if (n == ((size_t)1 << 17)) {   // 256 (16 x 16, 16 per thread) x 512 (32 x 16, 32 per thread): three 128-thread groups
     if (env_int("FOURIER_B200_CFG", 0) == 1)
-      return FusedImpl<fused::FusedCfg<float, 16, 8, 4, 8, 4, true, 16, 32, 16, 16, 32>>::ops(64, 32);
-    return FusedImpl<fused::FusedCfg<float, 16, 8, 3, 8, 3, false, 16, 32, 16, 16, 32>>::ops(64, 32);
+      return FusedImpl<fused::FusedCfg<float, 16, 8, 4, 8, 4, true, 16, 32, 16, 16, 32>>::ops(32, 16);
+    return FusedImpl<fused::FusedCfg<float, 16, 8, 3, 8, 3, false, 16, 32, 16, 16, 32>>::ops(32, 16);
   }
   if (n == ((size_t)1 << 15)) {   // 128 (16 x 8, 16 per thread) x 256 (16 x 16, 32 per thread): six 64-thread groups
     if (env_int("FOURIER_B200_CFG", 0) == 1)
-      return FusedImpl<fused::FusedCfg<float, 16, 8, 8, 8, 8, true, 8, 16, 16, 16, 32>>::ops(256, 128);
-    return FusedImpl<fused::FusedCfg<float, 16, 8, 6, 8, 6, false, 8, 16, 16, 16, 32>>::ops(256, 128);
+      return FusedImpl<fused::FusedCfg<float, 16, 8, 8, 8, 8, true, 8, 16, 16, 16, 32>>::ops(128, 64);
+    return FusedImpl<fused::FusedCfg<float, 16, 8, 6, 8, 6, false, 8, 16, 16, 16, 32>>::ops(128, 64);
   }
-  // (f32 2^12 = 64 x 64 was tried on the persistent kernel: 39.0 % against 41.7 % for the two-launch tile kernels)
   if (n == ((size_t)1 << 13)) {   // 64 (8 x 8, 8 per thread) x 128 (16 x 8, 16 per thread): eight 64-thread groups
     if (env_int("FOURIER_B200_CFG", 0) == 1)
       return FusedImpl<fused::FusedCfg<float, 8, 8, 8, 8, 8, true, 8, 16, 8, 8, 16>>::ops(512, 256);
@@ -152,27 +152,23 @@ template <> const FusedOps<float>* fused_lookup<float>(size_t n) {
 }
 template <> const FusedOps<double>* fused_lookup<double>(size_t n) {
   if (n == ((size_t)1 << 16)) {
-    // Three 128-thread groups with TMA staging, or four loading directly from global memory.  Short runs are a tie
-    // (62.5 % / 59.9 % at batch 2048, 57.9 % / 58.8 % at 16384); at the BASELINE batch of 65536, where the run is
-    // power-capped at ~1760 MHz, staging wins twice out of two A/B pairs: 56.5 / 57.4 % against 54.3 / 54.4 %
-    // (profiles/r02_c3_staged_vs_direct.txt).
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<double, 16, 8, 4, 4, 4, true>>::ops(64, 32);
-    return FusedImpl<fused::FusedCfg<double, 16, 8, 3, 4, 3>>::ops(64, 32);
+    // three 128-thread groups with TMA staging, or four loading directly from global memory
+    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<double, 16, 8, 4, 4, 4, true>>::ops(32, 16);
+    return FusedImpl<fused::FusedCfg<double, 16, 8, 3, 4, 3>>::ops(32, 16);
   }
   if (n == ((size_t)1 << 14)) {
     // 128 x 128 with 16 x 8 register tiles: four 64-thread groups with TMA staging, or eight loading directly
-    // measured: four groups with TMA staging 62.0 %, eight groups loading directly 53.7 %, tile kernels 37.7 %
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<double, 16, 8, 8, 4, 8, true, 8>>::ops(256, 128);
-    return FusedImpl<fused::FusedCfg<double, 16, 8, 4, 4, 4, false, 8>>::ops(256, 128);
+    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<double, 16, 8, 8, 4, 8, true, 8>>::ops(128, 64);
+    return FusedImpl<fused::FusedCfg<double, 16, 8, 4, 4, 4, false, 8>>::ops(128, 64);
   }
   if (n == ((size_t)1 << 12)) {   // 64 x 64 with 8 x 8 register tiles
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<double, 8, 8, 8, 4, 8, false>>::ops(1024, 512);
-    return FusedImpl<fused::FusedCfg<double, 8, 8, 8, 4, 8, true>>::ops(1024, 512);
+    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<double, 8, 8, 8, 4, 8, false>>::ops(512, 256);
+    return FusedImpl<fused::FusedCfg<double, 8, 8, 8, 4, 8, true>>::ops(512, 256);
   }
   if (n == ((size_t)1 << 13)) {   // 64 (8 x 8) x 128 (16 x 8): eight 64-thread groups loading directly
     if (env_int("FOURIER_B200_CFG", 0) == 1)
-      return FusedImpl<fused::FusedCfg<double, 8, 8, 6, 4, 6, false, 8, 16, 8, 8, 16>>::ops(512, 256);
-    return FusedImpl<fused::FusedCfg<double, 8, 8, 8, 4, 8, true, 8, 16, 8, 8, 16>>::ops(512, 256);
+      return FusedImpl<fused::FusedCfg<double, 8, 8, 6, 4, 6, false, 8, 16, 8, 8, 16>>::ops(256, 128);
+    return FusedImpl<fused::FusedCfg<double, 8, 8, 8, 4, 8, true, 8, 16, 8, 8, 16>>::ops(256, 128);
   }
   return nullptr;
 }
@@ -220,7 +216,7 @@ cudaError_t Plan<T>::init_twopass() {
       ring_ = std::max(2, env_int("FOURIER_B200_RING", f->default_ring));
       while (ring_ & (ring_ - 1)) ++ring_;   // the kernel wants a power of two
       lag_ = std::min(ring_ - 1, std::max(1, env_int("FOURIER_B200_LAG", f->default_lag)));
-      int dev = 0, sms = 148;
+      int dev = 0, sms = 132;
       cudaGetDevice(&dev);
       cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
       sm_count_ = sms;

@@ -1,5 +1,5 @@
 """One huge 1-D complex FFT distributed over the GPUs of a box (BASELINE.json configs[4]: N = 2^30 over 8
-B200s): the six-step algorithm with all-to-all transposes between local batched FFTs.
+GPUs): the six-step algorithm with all-to-all transposes between local batched FFTs.
 
 The reference has no counterpart (single-threaded CPU code, SURVEY.md 5); this is the only place of the
 engine where the path has a real exchange step, hence the only place a collective is used.
@@ -249,7 +249,7 @@ class NumpyBackend:
 
 class DistributedFft:
     """Plan for one length-N transform over `world` ranks (N = n1 * n2, both divisible by world).
-    `chunks` pieces per exchange (reduced to a divisor of the rows each rank receives; None = the measured best
+    `chunks` pieces per exchange (reduced to a divisor of the rows each rank receives; None = the default
     of the exchange mode)."""
 
     def __init__(self, n1, n2, rank, world, backend, group=None, chunks=None, exchange="nccl"):
@@ -260,8 +260,7 @@ class DistributedFft:
         self.n1, self.n2, self.n = n1, n2, n1 * n2
         self.rank, self.world, self.backend, self.group = rank, world, backend, group
         self.exchange = exchange if world > 1 else "nccl"
-        # measured (profiles/r01_c5_variants_8gpu.json, r01_c5_breakdown.txt): 8 pieces is the best pipelining of
-        # the NCCL formulation; on the peer-memory path the overlap gains nothing yet (1 = no pipelining)
+        # the NCCL formulation is pipelined in 8 pieces; the peer-memory path is not pipelined (1 piece)
         self.chunks = max(1, int(chunks)) if chunks else (8 if self.exchange == "nccl" else 1)
         self._send = self._recv = None
         self._bufs, self._tables = None, {}

@@ -1,5 +1,5 @@
 /*
- * fourier.h -- drop-in C / C++ interface of the B200 FFT engine (libfourier.so).
+ * fourier.h -- drop-in C / C++ interface of the H100 FFT engine (libfourier.so).
  *
  * This header declares exactly the C ABI that the reference's `fourier-ffi` crate exports
  * (reference: fourier-ffi/include/fourier.h:30-58, implemented by fourier-ffi/src/lib.rs:14-106)

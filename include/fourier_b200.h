@@ -6,7 +6,7 @@
  *
  * Why they exist: the reference's hot path is Fft::transform_in_place on ONE transform
  * (fourier-algorithms/src/fft.rs:48); a GPU needs many independent transforms per call to fill
- * 148 SMs and HBM, and callers that already hold data on the device must not pay PCIe.  A batch
+ * 132 SMs and HBM, and callers that already hold data on the device must not pay PCIe.  A batch
  * is `batch` contiguous transforms of size() samples each: transform b occupies samples
  * [b*size, (b+1)*size).  Every transform of a batch is independent, exactly as if the reference's
  * transform() were called in a loop (fourier-bench/benches/fft_bench.rs:36).

@@ -18,7 +18,7 @@ def test_emulated_kernels_match_f64_fft(tmp_path):
     exe = tmp_path / "emulate"
     csrc = os.path.join(ROOT, "fourier_b200", "csrc")
     subprocess.run([nvcc, "-std=c++17", "-O1", "--expt-relaxed-constexpr", "-gencode",
-                    "arch=compute_100a,code=sm_100a", "-I", csrc, os.path.join(ROOT, "tools", "emulate.cu"),
+                    "arch=compute_90a,code=sm_90a", "-I", csrc, os.path.join(ROOT, "tools", "emulate.cu"),
                     os.path.join(csrc, "host_math.cu"), "-o", str(exe)], check=True, capture_output=True)
     r = subprocess.run([str(exe)], capture_output=True, text=True)
     print(r.stdout)

@@ -1,7 +1,7 @@
 // emulate.cu -- runs the fused kernels' device code on the CPU, thread by thread and phase by phase
 // (the code in tilefft.cuh / twopass_kernels.cuh is __host__ __device__), and checks the result
 // against a double-precision FFT.  There is no GPU in the build container, so this is how index maps,
-// twiddle tables and shared-memory layouts are verified before a kernel ever runs on the B200.
+// twiddle tables and shared-memory layouts are verified before a kernel ever runs on the GPU.
 // It also reports shared-memory bank conflicts of the exchange (64-bit/128-bit access model).
 // Build: nvcc -std=c++17 -O1 --expt-relaxed-constexpr -I fourier_b200/csrc tools/emulate.cu \
 //             fourier_b200/csrc/plan.cu ... (host only, never run on the device)
