@@ -4,19 +4,24 @@
 //   * one CTA per SM: G consumer groups, each processing one TileFFT tile in registers at a time, and
 //     one producer warp (a first version let thread 0 of each group produce: the ~3000 cycles of
 //     queue/TMA work per tile then sat on the critical path of its group's first barrier);
-//   * the producer claims items of a global work queue (atomic counter) whose order interleaves
-//     pass-1 tiles of transform s with pass-2 tiles of transform s-LAG, waits for the tile's
-//     dependencies, and brings the tile into the target group's shared-memory staging buffer with TMA: a 2-D tensor-map box for the
+//   * the producer waits until its group has emptied the staging buffer, then claims an item of a global
+//     work queue (atomic counter) whose order interleaves pass-1 tiles of transform s with pass-2 tiles
+//     of transform s-LAG, waits for the tile's dependencies, and brings the tile into the group's
+//     shared-memory staging buffer with TMA: a 2-D tensor-map box for the
 //     strided column tiles of pass 1 (cp.async.bulk.tensor), plain bulk copies for the contiguous
 //     row tiles of pass 2 (cp.async.bulk) -- completion is signalled on an mbarrier (full[g]);
 //   * a consumer group waits on full[g], pulls its 32 (16) samples per thread out of the staging
 //     buffer, releases it (empty[g]) so the next tile's TMA overlaps ALL of the remaining work,
 //     runs stage A, exchanges through a shared buffer (one buffer, taken under a lock: the
 //     exchange is ~10% of a tile), runs stage B and stores straight from registers;
-//   * the intermediate A[k1][n2] lives in a ring of RING transforms (about 32 MB) that stays
-//     in the 50 MB L2: pass-1 tiles of transform b may only start once pass 2 of transform b-RING
-//     has consumed the slot (done2), pass-2 tiles of b once all pass-1 tiles of b are stored (done1).
-//     Every dependency points to an earlier queue position, so the scheme cannot deadlock.
+//   * the intermediate A[k1][n2] lives in a ring of RING transforms (any RING >= 2; slot = b % RING)
+//     that stays in the 50 MB L2: pass-1 tiles of transform b may only start once pass 2 of transform
+//     b-RING has consumed the slot (done2), pass-2 tiles of b once all pass-1 tiles of b are stored (done1).
+//     The scheme cannot deadlock: every dependency points to an earlier queue position; the tile a group
+//     computes in registers waits on nothing; and a producer claims only into an empty staging buffer, so
+//     the earliest claimed but unfinished item depends only on finished items and has a buffer to land in.
+//     A group holds at most two claimed items (registers, staging), so about 2 x G x SMs queue positions
+//     are in flight, and the ring must cover that window for the dependency waits to stay short.
 //
 // HBM therefore sees each sample exactly twice (one read, one write); there are no launch gaps or
 // partial waves, and memory latency is hidden by the TMA prefetch instead of by occupancy.
@@ -156,6 +161,7 @@ template <typename T> struct FusedArgs {
   T scale;
   int do_scale;
   long long* trace;           // optional phase timestamps of CTA 0 (debugging / DESIGN.md timeline), else nullptr
+  uint32_t trace_from;        // first tile of each warp the trace records (kTraceTiles from there)
 };
 
 // Configuration: N = N1 * N2 (two register-tile lengths, see RB_ / RA2_ ... below), tiles of C = 8 FFTs, G consumer groups per CTA, EXB exchange buffers (group g uses
@@ -255,7 +261,7 @@ __device__ __forceinline__ void issue_tile(const WorkItem& wi, const CUtensorMap
   using V = cpx<typename Cfg::T>;
   constexpr int C = Cfg::C;
   WorkItem d = wi;
-  d.slot = wi.b & (a.ring - 1);               // ring is a power of two
+  d.slot = wi.b % a.ring;
   ctl->desc = d;
   if (wi.pass < 0) { mbar_arrive(&ctl->full); return; }
   if constexpr (Cfg::DIRECT) {
@@ -358,14 +364,16 @@ template <class Cfg, bool FWD> struct FusedMath {
 constexpr int kTraceTiles = 64, kTracePhases = 8;
 #define FB_TRACE(phase)                                                                                   \
   do {                                                                                                    \
-    if (a.trace && blockIdx.x == 0 && (t & 31) == 0 && k < kTraceTiles)                                   \
-      a.trace[(((long)g * (GT / 32) + (t >> 5)) * kTraceTiles + k) * kTracePhases + (phase)] = clock64(); \
+    if (a.trace && blockIdx.x == 0 && (t & 31) == 0 && k - a.trace_from < kTraceTiles)                    \
+      a.trace[(((long)g * (GT / 32) + (t >> 5)) * kTraceTiles + (k - a.trace_from)) * kTracePhases + (phase)] = \
+          clock64();                                                                                      \
   } while (0)
 
 #define FB_PTRACE(phase)                                                                                  \
   do {                                                                                                    \
-    if (a.trace && blockIdx.x == 0 && it < kTraceTiles)                                                   \
-      a.trace[(((long)(Cfg::CONSUMERS / 32) + g) * kTraceTiles + it) * kTracePhases + (phase)] = clock64(); \
+    if (a.trace && blockIdx.x == 0 && it - a.trace_from < kTraceTiles)                                    \
+      a.trace[(((long)(Cfg::CONSUMERS / 32) + g) * kTraceTiles + (it - a.trace_from)) * kTracePhases + (phase)] = \
+          clock64();                                                                                      \
   } while (0)
 
 template <class Cfg, bool FWD>
@@ -420,35 +428,36 @@ fused_twopass_kernel(const __grid_constant__ CUtensorMap in_map, const FusedArgs
     const int pw = (tid - Cfg::CONSUMERS) >> 5;
     if ((tid & 31) != 0) return;
     if (pw < G) {
-      // ---- producer of group pw: claim a queue item (one ahead, so the atomic's latency is hidden), wait for
-      // its dependencies (blocking is fine here: nothing a consumer needs is held back by it), wait until
-      // the group has emptied its staging buffer, refill it by TMA.
+      // ---- producer of group pw: wait until the group has emptied its staging buffer, only then claim a queue
+      // item, wait for its dependencies (blocking is fine here: nothing a consumer needs is held back by it),
+      // refill the staging buffer by TMA.  Claiming just in time keeps a group at two claimed but unfinished
+      // items (one in registers, one in staging or in flight): every item claimed ahead of that widens the
+      // window of queue positions in flight, and with it the ring the dependency waits need to stay short.
       const int g = pw;
       GroupCtl* ctl = &ctl_all[g];
       V* stage_g = reinterpret_cast<V*>(staging + (size_t)g * Cfg::BUF_BYTES);
       V* tab_g = tabs + (size_t)g * 2 * Cfg::TAB_ELEMS;
       uint32_t n_p1 = 0;
-      unsigned w_next = atomicAdd(queue, 1u);
       for (uint32_t it = 0;; ++it) {
-        const WorkItem wi = decode_work((long)w_next, a.batch, a.lag, T1, T2);
-        if (wi.pass >= 0) w_next = atomicAdd(queue, 1u);
         FB_PTRACE(0);
+        if (it > 0) mbar_wait(&ctl->empty, (it - 1) & 1);
+        FB_PTRACE(2);
+        const WorkItem wi = decode_work((long)atomicAdd(queue, 1u), a.batch, a.lag, T1, T2);
         unsigned target;
         const unsigned* dep = dep_counter<Cfg>(wi, a, &target);
         if (dep) { spin_until_ge(dep, target); fence_proxy_async(); }
         FB_PTRACE(1);
-        if (it > 0) mbar_wait(&ctl->empty, (it - 1) & 1);
         if constexpr (Cfg::DIRECT) {
-          // The group has just started on the previous item, so it will ask for this tile one tile period from now
-          // (~5 us): long enough for HBM -> L2, short enough that the prefetched tiles of all groups (132 x G x 64 KB)
-          // do not crowd the intermediate out of L2.
+          // The group started on the previous item when `empty` landed, so it will ask for this tile at most one tile
+          // period from now (less by the dependency wait above): long enough for HBM -> L2 in the steady state,
+          // short enough that the prefetched tiles of all groups (132 x G x 64 KB) do not crowd the intermediate
+          // out of L2.
           if (wi.pass == 1) {
 #pragma unroll
             for (int r0 = 0; r0 < (int)Cfg::N1; r0 += Cfg::BOX_ROWS)
               tma_prefetch_2d(&in_map, wi.tile * Cfg::C1 * 2, (int)((long)wi.b * Cfg::N1 + r0));
           }
         }
-        FB_PTRACE(2);
         issue_tile<Cfg>(wi, &in_map, a, stage_g, tab_g + (size_t)(n_p1 & 1) * Cfg::TAB_ELEMS, ctl);
         FB_PTRACE(3);
         n_p1 += wi.pass == 1;
@@ -510,7 +519,8 @@ fused_twopass_kernel(const __grid_constant__ CUtensorMap in_map, const FusedArgs
     const WorkItem wi = ctl->desc;
     if (wi.pass < 0) break;
     FB_TRACE(1);
-    if (a.trace && blockIdx.x == 0 && t == 0 && k < kTraceTiles) a.trace[((long)g * (GT / 32) * kTraceTiles + k) * kTracePhases + 7] = wi.pass;
+    if (a.trace && blockIdx.x == 0 && t == 0 && k - a.trace_from < kTraceTiles)
+      a.trace[((long)g * (GT / 32) * kTraceTiles + (k - a.trace_from)) * kTracePhases + 7] = wi.pass;
     const V* ring_rows = a.scratch + (size_t)wi.slot * N + (size_t)wi.tile * C * N2;   // pass 2: the tile's rows
 
     // One tile, from its samples to its stores; the whole group takes the same branch (wi is the group's item), so

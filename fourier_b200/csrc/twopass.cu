@@ -104,8 +104,9 @@ template <class Cfg> struct FusedImpl {
 
 template <typename T> const FusedOps<T>* fused_lookup(size_t n);
 // Ring (intermediates kept in L2) = 32 MB / transform size, lag = ring / 2: the ring must stay well inside the
-// H100's 50 MB L2 next to the prefetched input tiles.  Measured on one H100 SXM (700 W limit, power-capped near
-// 1.3 GHz in that run): N = 2^20 f32 ring 4 against 8 and N = 2^16 f64 ring 32 against 64 gave +20 % and +13 %.
+// H100's 50 MB L2 next to the prefetched input tiles.  The ring may have any size >= 2.  Measured on one H100 SXM
+// (700 W limit, power-capped near 1.3 GHz in that run): N = 2^20 f32 ring 4 against 8 and N = 2^16 f64 ring 32
+// against 64 gave +20 % and +13 %.
 // FOURIER_B200_CFG=1 selects the other load strategy (experiments).
 template <> const FusedOps<float>* fused_lookup<float>(size_t n) {
   if (n == ((size_t)1 << 20)) {
@@ -214,7 +215,6 @@ cudaError_t Plan<T>::init_twopass() {
       FB_CHECK((upload_vec<T, cpx<T>>(tstep_, ts)));
       fused_ops_ = f;
       ring_ = std::max(2, env_int("FOURIER_B200_RING", f->default_ring));
-      while (ring_ & (ring_ - 1)) ++ring_;   // the kernel wants a power of two
       lag_ = std::min(ring_ - 1, std::max(1, env_int("FOURIER_B200_LAG", f->default_lag)));
       int dev = 0, sms = 132;
       cudaGetDevice(&dev);
@@ -236,7 +236,7 @@ cudaError_t Plan<T>::exec_twopass(const C* in, C* out, size_t batch, int code, c
   if (fused_ops_ && batch <= (size_t)1 << 24) {
     const auto* f = static_cast<const FusedOps<T>*>(fused_ops_);
     int ring = ring_;
-    while (ring > 2 && (size_t)ring / 2 >= batch) ring /= 2;
+    while (ring > 2 && (size_t)ring / 2 >= batch) ring = std::max(2, ring / 2);
     const int lag = std::min(lag_, ring - 1);
     FB_CHECK(work_.reserve((size_t)ring * n_ * sizeof(C)));
     const size_t cbytes = (1 + 2 * batch) * sizeof(unsigned);
@@ -249,7 +249,10 @@ cudaError_t Plan<T>::exec_twopass(const C* in, C* out, size_t batch, int code, c
     a.tbase = (const C*)tbase_.data(); a.tstep = (const C*)tstep_.data();
     a.counters = (unsigned*)counters_.data();
     a.trace = nullptr;
+    a.trace_from = 0;
     if (std::getenv("FOURIER_B200_TRACE")) {
+      // FOURIER_B200_TRACE_FROM: skip that many tiles per warp, to record a window of the steady state
+      a.trace_from = (uint32_t)std::max(0, env_int("FOURIER_B200_TRACE_FROM", 0));
       const size_t tbytes = sizeof(long long) * 64 * fused::kTraceTiles * fused::kTracePhases;
       FB_CHECK(trace_.reserve(tbytes));
       FB_CHECK(cudaMemsetAsync(trace_.data(), 0, tbytes, s));
