@@ -148,6 +148,16 @@ __host__ __device__ inline WorkItem decode_work(long w, int batch, int lag, int 
   return it;
 }
 
+// Ring and lag of one launch.  A batch that fills only part of the plan's ring gets a smaller ring: it is halved
+// while half of it still holds the whole batch (so a shrunk ring never wraps), down to 2 slots, and the lag stays
+// below the ring.
+struct RingLag { int ring, lag; };
+__host__ __device__ inline RingLag launch_ring(int ring, int lag, long batch) {
+  while (ring > 2 && (long)(ring / 2) >= batch) ring = ring / 2 > 2 ? ring / 2 : 2;
+  RingLag r = {ring, lag < ring - 1 ? lag : ring - 1};
+  return r;
+}
+
 template <typename T> struct FusedArgs {
   const cpx<T>* in;
   cpx<T>* out;
@@ -245,13 +255,25 @@ struct GroupCtl {            // per-group control block in shared memory
   uint64_t full;             // TMA for the group's next tile has landed
   uint64_t empty;            // every thread of the group is done with the staging buffer
   WorkItem desc;             // the tile the staging buffer holds / will hold
-  int loaded;                // warps of the group that have pulled their samples out of staging (this tile)
+  unsigned loaded;           // warps of the group that are done with the ring rows of the current pass-2 tile
   unsigned stored_warps;     // warps of the group that have issued the stores of the current pass-1 tile
   unsigned stored_seq;       // pass-1 tiles of this group whose stores have all been issued
   unsigned finished;         // the group has left its tile loop
   unsigned acked;            // pass-1 tiles of this group the signaller has published (back-pressure)
   int store_b[kStoreRing];   // transform index of pass-1 tile number n at [n % kStoreRing]
 };
+
+// Direct loads: a pass-2 tile reports its ring slot as consumed (done2) once every warp of the group has loaded and
+// discarded the slot's rows.  Each warp's discards are ordered before its lane 0's acq_rel count in shared memory
+// (__syncwarp), and the last warp of the group publishes with a gpu-scope release: a pass-1 tile of b + RING that sees
+// done2[b] complete stores into the slot only after all of them.  Called by every thread of the group.
+__device__ __forceinline__ void report_consumed(GroupCtl* ctl, unsigned* done2_b, int warps) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0 && atom_add_acq_rel_cta_shared(&ctl->loaded, 1u) == (unsigned)warps - 1) {
+    ctl->loaded = 0;
+    red_release_add(done2_b, 1u);
+  }
+}
 
 // Issues the loads of one work item into the group's staging buffer (one thread of the group).
 template <class Cfg>
@@ -543,17 +565,16 @@ fused_twopass_kernel(const __grid_constant__ CUtensorMap in_map, const FusedArgs
           asm volatile("discard.global.L2 [%0], 128;" ::"l"(rows + o) : "memory");
         // the last warp of the group to have pulled its samples reports the ring slot as consumed by this
         // tile -- promptly and from the consumer side (a lazy report by the producer could deadlock it
-        // against its own dependency wait)
-        if ((t & 31) == 0 && atomicAdd(&ctl->loaded, 1) == GT / 32 - 1) { ctl->loaded = 0; atomicAdd(&done2[wi.b], 1u); }
+        // against its own dependency wait).  Each warp issues its discards before its count (__syncwarp), but the
+        // report stays relaxed: report_consumed() here (gpu-scope release) made the f32 2^20 kernel 4.3 % slower,
+        // a release after stage A 7.3 % (DESIGN.md 4.2).  So only timing orders these discards before the stores of
+        // the pass-1 tile of b + RING, which sees done2, loads its input and computes a whole tile first.
+        __syncwarp();
+        if ((t & 31) == 0 && atomicAdd(&ctl->loaded, 1u) == GT / 32 - 1) { ctl->loaded = 0; atomicAdd(&done2[wi.b], 1u); }
       }
       FB_TRACE(2);
 
       P::stage_a(f, t, PASS == 1 ? twa1 : twa2);
-      if constexpr (Cfg::DIRECT && PASS == 2) {
-        // same report with direct loads: stage A has consumed every register the warp loaded, so its global loads
-        // have completed
-        if ((t & 31) == 0 && atomicAdd(&ctl->loaded, 1) == GT / 32 - 1) { ctl->loaded = 0; atomicAdd(&done2[wi.b], 1u); }
-      }
 
       // ---- exchange through the shared buffer (under the CTA-wide lock when the groups share one) --------------
       if (kLocked && t == 0) {
@@ -563,10 +584,13 @@ fused_twopass_kernel(const __grid_constant__ CUtensorMap in_map, const FusedArgs
       FB_TRACE(3);
       group_sync(bar_id, GT);
       if constexpr (Cfg::DIRECT && PASS == 2) {
-        // every warp of the group is past stage A, i.e. all loads of the tile have completed: drop its rows from L2
+        // every warp of the group is past stage A, i.e. all loads of the tile have completed: drop its rows from L2,
+        // then report the slot as consumed (not before: a pass-1 tile of b + RING may store into these rows as soon
+        // as done2 is complete, and a discard landing after those stores would throw them away)
         const unsigned char* rows = reinterpret_cast<const unsigned char*>(ring_rows);
         for (uint32_t o = (uint32_t)t * 128u; o < TILE_BYTES; o += (uint32_t)GT * 128u)
           asm volatile("discard.global.L2 [%0], 128;" ::"l"(rows + o) : "memory");
+        report_consumed(ctl, &done2[wi.b], GT / 32);
       }
       P::scatter(f, t, exch);
       FB_TRACE(4);

@@ -133,7 +133,7 @@ const char* Plan<T>::kernel_name() const {
   switch (path_) {
     case Path::kTrivial: return "scale_copy_kernel";
     case Path::kOnChip: return "onchip::onchip_fft_kernel";
-    case Path::kTwoPass: return fused_ops_ ? "fused::fused_twopass_kernel" : "twopass::tile_kernel (pass 1 + pass 2)";
+    case Path::kTwoPass: return fused_ops_ ? kernel_desc_.c_str() : "twopass::tile_kernel (pass 1 + pass 2)";
     case Path::kGlobalStages: return "stockham_stage_kernel (one launch per radix stage)";
     case Path::kBluestein: return "chirp / pointwise kernels around the inner plan's kernels";
     case Path::kBluesteinFused: return cta_chirp_ ? "cta::cta_fft_kernel (chirp mode)" : "onchip::bluestein_fused_kernel";

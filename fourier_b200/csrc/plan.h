@@ -135,7 +135,10 @@ class Plan {
   // Number of kernel launches the last exec_* call issued (bench.py reports it).
   unsigned long long launches() const { return launches_; }
 
-  // Name of the kernel that moves (nearly) all of this plan's bytes -- what a profiler will list first.
+  // Name of the kernel that moves (nearly) all of this plan's bytes -- what a profiler will list first.  For the
+  // persistent two-pass kernel it is followed by the configuration the plan chose, e.g.
+  // "fused::fused_twopass_kernel [1024x1024, 2 groups x 256, TMA staging, ring 4, lag 2]" (the ring and lag of a full
+  // batch; exec_twopass shrinks the ring for a small one).
   const char* kernel_name() const;
 
  private:
@@ -176,6 +179,7 @@ class Plan {
   size_t chunk_ = 0;                 // transforms per L2-resident chunk (two-pass)
   const void* fused_ops_ = nullptr;  // FusedOps<T>: persistent single-launch variant
   int ring_ = 0, lag_ = 0, sm_count_ = 132;
+  std::string kernel_desc_;          // kernel_name() of the persistent kernel: tile lengths, groups, loads, ring, lag
   int outer_radix3_ = 0;             // kThreePass: 3 / 9 / 27 = the outer pass is a radix-3 DFT (N = 3^b * 2^k), 0 = power of two
   DeviceBuffer counters_, tbase_, tstep_, trace_;
 

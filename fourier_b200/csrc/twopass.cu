@@ -17,6 +17,7 @@
 #include <cstdlib>
 
 #include "plan.h"
+#include "fused_configs.cuh"
 #include "fused_kernels.cuh"
 #include "twopass_kernels.cuh"
 
@@ -61,6 +62,8 @@ template <typename T> struct FusedOps {
   int ra, rb, ra2, rb2, tile_c;   // register tiles of pass 1 (ra x rb) and pass 2 (ra2 x rb2); columns per pass-1 tile
   size_t smem_bytes;
   int default_ring, default_lag;
+  int groups, group_threads;   // consumer groups per CTA and threads per group
+  bool direct;                 // consumers load from global memory (else TMA staging through shared memory)
   bool base_pcol;   // layout of the factored base table this configuration reads (tables.cuh)
   cudaError_t (*prepare)();
   cudaError_t (*launch)(const fused::FusedArgs<T>&, bool fwd, int grid, cudaStream_t);
@@ -97,79 +100,41 @@ template <class Cfg> struct FusedImpl {
   }
   static const FusedOps<T>* ops(int ring, int lag) {
     static const FusedOps<T> o = {(size_t)Cfg::N1, (size_t)Cfg::N2, Cfg::RA, Cfg::RB, Cfg::RA2, Cfg::RB2, Cfg::C1, Cfg::SMEM_BYTES, ring, lag,
-                                  true, &prepare, &launch};
+                                  Cfg::G, Cfg::GT, Cfg::DIRECT, true, &prepare, &launch};
     return &o;
   }
 };
 
+// The configuration of N = 2^LOG2N (fused_configs.cuh); FOURIER_B200_CFG=1 selects the other load strategy (experiments).
+template <typename T, int LOG2N> const FusedOps<T>* fused_pick() {
+  using D = fused::FusedConfig<T, LOG2N>;
+  using A = fused::FusedConfig<T, LOG2N, true>;
+  if constexpr (A::HAS) {
+    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<typename A::Cfg>::ops(A::RING, A::LAG);
+  }
+  return FusedImpl<typename D::Cfg>::ops(D::RING, D::LAG);
+}
+
 template <typename T> const FusedOps<T>* fused_lookup(size_t n);
-// Ring (intermediates kept in L2) = 32 MB / transform size, lag = ring / 2: the ring must stay well inside the
-// H100's 50 MB L2 next to the prefetched input tiles.  The ring may have any size >= 2.  Measured on one H100 SXM
-// (700 W limit, power-capped near 1.3 GHz in that run): N = 2^20 f32 ring 4 against 8 and N = 2^16 f64 ring 32
-// against 64 gave +20 % and +13 %.
-// FOURIER_B200_CFG=1 selects the other load strategy (experiments).
 template <> const FusedOps<float>* fused_lookup<float>(size_t n) {
-  if (n == ((size_t)1 << 20)) {
-    // default: two 256-thread groups, TMA staging, one shared exchange buffer taken under a lock
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<float, 32, 8, 2, 8, 2, true>>::ops(4, 2);
-    return FusedImpl<fused::FusedCfg<float, 32, 8, 2, 8, 1>>::ops(4, 2);
-  }
-  if (n == ((size_t)1 << 16)) {
-    // 256 x 256 with 16 x 16 register tiles, four 128-thread groups, 64-byte tile rows as at 2^20
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<float, 16, 8, 4, 8, 4, true>>::ops(64, 32);
-    return FusedImpl<fused::FusedCfg<float, 16, 8, 4, 8, 4>>::ops(64, 32);
-  }
-  if (n == ((size_t)1 << 18)) {
-    // 512 x 512 with 32 x 16 register tiles: three 128-thread groups with TMA staging, or four with direct loads
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<float, 32, 8, 4, 8, 4, true, 16>>::ops(16, 8);
-    return FusedImpl<fused::FusedCfg<float, 32, 8, 3, 8, 3, false, 16>>::ops(16, 8);
-  }
-  if (n == ((size_t)1 << 14)) {
-    // 128 x 128 with 16 x 8 register tiles: eight 64-thread groups
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<float, 16, 8, 8, 8, 8, true, 8>>::ops(256, 128);
-    return FusedImpl<fused::FusedCfg<float, 16, 8, 8, 8, 8, false, 8>>::ops(256, 128);
-  }
-  // Odd powers of two: N1 x 2 N1 with a different register tile per pass, same threads per FFT in both
-  // (template arguments: <T, RA, C, G, PAD1, EXB, DIRECT, RB, RA2, RB2, E1, E2>).
-  if (n == ((size_t)1 << 19)) {   // 512 (32 x 16) x 1024 (32 x 32), 16-column pass-1 tiles: two 256-thread groups
-    return FusedImpl<fused::FusedCfg<float, 32, 8, 2, 0, 1, false, 16, 32, 32, 32, 32, 16, true>>::ops(8, 4);
-  }
-  if (n == ((size_t)1 << 17)) {   // 256 (16 x 16, 16 per thread) x 512 (32 x 16, 32 per thread): three 128-thread groups
-    if (env_int("FOURIER_B200_CFG", 0) == 1)
-      return FusedImpl<fused::FusedCfg<float, 16, 8, 4, 8, 4, true, 16, 32, 16, 16, 32>>::ops(32, 16);
-    return FusedImpl<fused::FusedCfg<float, 16, 8, 3, 8, 3, false, 16, 32, 16, 16, 32>>::ops(32, 16);
-  }
-  if (n == ((size_t)1 << 15)) {   // 128 (16 x 8, 16 per thread) x 256 (16 x 16, 32 per thread): six 64-thread groups
-    if (env_int("FOURIER_B200_CFG", 0) == 1)
-      return FusedImpl<fused::FusedCfg<float, 16, 8, 8, 8, 8, true, 8, 16, 16, 16, 32>>::ops(128, 64);
-    return FusedImpl<fused::FusedCfg<float, 16, 8, 6, 8, 6, false, 8, 16, 16, 16, 32>>::ops(128, 64);
-  }
-  if (n == ((size_t)1 << 13)) {   // 64 (8 x 8, 8 per thread) x 128 (16 x 8, 16 per thread): eight 64-thread groups
-    if (env_int("FOURIER_B200_CFG", 0) == 1)
-      return FusedImpl<fused::FusedCfg<float, 8, 8, 8, 8, 8, true, 8, 16, 8, 8, 16>>::ops(512, 256);
-    return FusedImpl<fused::FusedCfg<float, 8, 8, 8, 8, 8, false, 8, 16, 8, 8, 16>>::ops(512, 256);
+  switch (n) {
+    case (size_t)1 << 13: return fused_pick<float, 13>();
+    case (size_t)1 << 14: return fused_pick<float, 14>();
+    case (size_t)1 << 15: return fused_pick<float, 15>();
+    case (size_t)1 << 16: return fused_pick<float, 16>();
+    case (size_t)1 << 17: return fused_pick<float, 17>();
+    case (size_t)1 << 18: return fused_pick<float, 18>();
+    case (size_t)1 << 19: return fused_pick<float, 19>();
+    case (size_t)1 << 20: return fused_pick<float, 20>();
   }
   return nullptr;
 }
 template <> const FusedOps<double>* fused_lookup<double>(size_t n) {
-  if (n == ((size_t)1 << 16)) {
-    // three 128-thread groups with TMA staging, or four loading directly from global memory
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<double, 16, 8, 4, 4, 4, true>>::ops(32, 16);
-    return FusedImpl<fused::FusedCfg<double, 16, 8, 3, 4, 3>>::ops(32, 16);
-  }
-  if (n == ((size_t)1 << 14)) {
-    // 128 x 128 with 16 x 8 register tiles: four 64-thread groups with TMA staging, or eight loading directly
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<double, 16, 8, 8, 4, 8, true, 8>>::ops(128, 64);
-    return FusedImpl<fused::FusedCfg<double, 16, 8, 4, 4, 4, false, 8>>::ops(128, 64);
-  }
-  if (n == ((size_t)1 << 12)) {   // 64 x 64 with 8 x 8 register tiles
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<fused::FusedCfg<double, 8, 8, 8, 4, 8, false>>::ops(512, 256);
-    return FusedImpl<fused::FusedCfg<double, 8, 8, 8, 4, 8, true>>::ops(512, 256);
-  }
-  if (n == ((size_t)1 << 13)) {   // 64 (8 x 8) x 128 (16 x 8): eight 64-thread groups loading directly
-    if (env_int("FOURIER_B200_CFG", 0) == 1)
-      return FusedImpl<fused::FusedCfg<double, 8, 8, 6, 4, 6, false, 8, 16, 8, 8, 16>>::ops(256, 128);
-    return FusedImpl<fused::FusedCfg<double, 8, 8, 8, 4, 8, true, 8, 16, 8, 8, 16>>::ops(256, 128);
+  switch (n) {
+    case (size_t)1 << 12: return fused_pick<double, 12>();
+    case (size_t)1 << 13: return fused_pick<double, 13>();
+    case (size_t)1 << 14: return fused_pick<double, 14>();
+    case (size_t)1 << 16: return fused_pick<double, 16>();
   }
   return nullptr;
 }
@@ -216,6 +181,10 @@ cudaError_t Plan<T>::init_twopass() {
       fused_ops_ = f;
       ring_ = std::max(2, env_int("FOURIER_B200_RING", f->default_ring));
       lag_ = std::min(ring_ - 1, std::max(1, env_int("FOURIER_B200_LAG", f->default_lag)));
+      char desc[160];
+      snprintf(desc, sizeof desc, "fused::fused_twopass_kernel [%zux%zu, %d groups x %d, %s, ring %d, lag %d]", f->n1,
+               f->n2, f->groups, f->group_threads, f->direct ? "direct loads" : "TMA staging", ring_, lag_);
+      kernel_desc_ = desc;
       int dev = 0, sms = 132;
       cudaGetDevice(&dev);
       cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -235,9 +204,8 @@ cudaError_t Plan<T>::exec_twopass(const C* in, C* out, size_t batch, int code, c
   else if (do_scale) scale = (T)1 / std::sqrt((T)n_);
   if (fused_ops_ && batch <= (size_t)1 << 24) {
     const auto* f = static_cast<const FusedOps<T>*>(fused_ops_);
-    int ring = ring_;
-    while (ring > 2 && (size_t)ring / 2 >= batch) ring = std::max(2, ring / 2);
-    const int lag = std::min(lag_, ring - 1);
+    const fused::RingLag rl = fused::launch_ring(ring_, lag_, (long)batch);
+    const int ring = rl.ring, lag = rl.lag;
     FB_CHECK(work_.reserve((size_t)ring * n_ * sizeof(C)));
     const size_t cbytes = (1 + 2 * batch) * sizeof(unsigned);
     FB_CHECK(counters_.reserve(cbytes));

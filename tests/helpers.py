@@ -58,6 +58,53 @@ def sweep_input(max_size, dtype, forward, seed=0xDEADBEEF):
     return z.astype(dtype)
 
 
+def poisoned_like(x):
+    """An output buffer like `x` (numpy array or torch tensor) filled with NaN, so that a sample the transform never
+    stores cannot pass for a result left behind by an earlier call in a reused allocation."""
+    if isinstance(x, np.ndarray):
+        return np.full_like(x, np.nan)
+    import torch
+    return torch.full_like(x, complex(float("nan"), float("nan")))
+
+
+def truth_ld(x, code):
+    """Reference in long double: numpy's FFT on clongdouble (computed natively, not through f64), with the Transform
+    scaling definitions applied in long double.  An input exact in f32 or f64 converts exactly, so for f64 data this
+    is more precise than the kernels, which truth_f64 is not."""
+    x = np.asarray(x).astype(np.clongdouble)
+    if code in (0, 3):
+        y = np.fft.fft(x, axis=-1)
+    else:
+        y = np.fft.ifft(x, axis=-1) * np.longdouble(x.shape[-1])
+    assert y.dtype == np.clongdouble
+    return scale_ld(y, code)
+
+
+def scale_ld(y, code):
+    """Applies the scale of Transform `code` in long double to the unscaled forward (codes 0, 3) or unscaled inverse
+    (codes 1, 2, 4) transform `y`."""
+    n = np.longdouble(y.shape[-1])
+    if code == 1:
+        return y / n
+    if code in (3, 4):
+        return y / np.sqrt(n)
+    return y
+
+
+def per_transform_err(got, ref):
+    """max_k |got[b,k] - ref[b,k]| / max_k |ref[b,k]| for every transform b of a batch (last axis = transform), in the
+    precision of `ref`: one bad transform cannot hide behind the others.  NaN (an unstored sample) counts as infinite."""
+    got = np.asarray(got).reshape(-1, np.shape(ref)[-1])
+    ref = np.asarray(ref).reshape(got.shape)
+    err = np.empty(got.shape[0])
+    rows = max(1, (1 << 20) // got.shape[1])   # bounds the long-double temporaries
+    for b0 in range(0, got.shape[0], rows):
+        g, r = got[b0:b0 + rows], ref[b0:b0 + rows]
+        e = np.abs(g.astype(r.dtype) - r).max(axis=1) / np.maximum(np.abs(r).max(axis=1), 1e-300)
+        err[b0:b0 + rows] = e
+    return np.where(np.isnan(err), np.inf, err)
+
+
 def truth_f64(x, code):
     """Independent reference: numpy pocketfft in f64, with the Transform scaling definitions
     (fourier-algorithms/src/fft.rs:5-16, autosort/mod.rs:381-385)."""

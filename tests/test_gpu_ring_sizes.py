@@ -1,17 +1,19 @@
 """The persistent two-pass kernel keeps its intermediate in a ring of RING transforms (slot = b % RING).  Any RING >= 2
 works, not only powers of two, including a ring shrunk before the launch for a small batch.  Ring size and lag only
-change the schedule, not the per-tile arithmetic, so the result must equal the default plan's bit for bit."""
+change the schedule, not the per-tile arithmetic, so the result must equal the default plan's bit for bit, and every
+transform must match the long-double reference within the bounds of tools/emulate.cu."""
 import numpy as np
 import pytest
 import torch
 
 import fourier_b200 as fb
 from oracle import oracle as O
+from helpers import per_transform_err, poisoned_like, truth_ld
 
 pytestmark = pytest.mark.gpu
 
 NP = {"f32": np.complex64, "f64": np.complex128}
-TOL = {"f32": 1e-5, "f64": 1e-12}
+TOL = {"f32": 2e-6, "f64": 5e-15}
 
 
 def create(real, n):
@@ -34,13 +36,13 @@ def test_ring_of_any_size(monkeypatch, real, n, ring, lag, batch):
     assert p.info()["path_name"] == ref.info()["path_name"]
     x = O.fill_input(batch, n, NP[real], first_transform=3)
     xd = torch.from_numpy(x).cuda()
-    got, want = torch.empty_like(xd), torch.empty_like(xd)
+    got, want = poisoned_like(xd), poisoned_like(xd)
     p.transform(xd, got, fb.Transform.Fft)
     ref.transform(xd, want, fb.Transform.Fft)
     torch.cuda.synchronize()
     got, want = got.cpu().numpy(), want.cpu().numpy()
     assert np.array_equal(got.view(np.uint8), want.view(np.uint8))
-    truth = O.transform(x[-1], O.FFT)
-    assert float(np.abs(got[-1] - truth).max() / np.abs(truth).max()) < TOL[real]
+    err = per_transform_err(got, truth_ld(x, int(fb.Transform.Fft)))
+    assert (err < TOL[real]).all(), f"transforms {np.nonzero(~(err < TOL[real]))[0].tolist()} of {batch}: {err}"
     p.close()
     ref.close()

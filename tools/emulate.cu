@@ -13,6 +13,7 @@
 
 #include "cta_kernels.cuh"
 #include "dist_kernels.cuh"
+#include "fused_configs.cuh"
 #include "fused_kernels.cuh"
 #include "onchip_kernels.cuh"
 #include "outer_kernels.cuh"
@@ -379,41 +380,79 @@ static int check_fused(const char* name, double tol) {
 }
 
 // ---- work queue of the fused kernel: order and dependency properties ---------------------------------------------
-static int check_queue() {
-  int bad = 0;
-  const int t1 = 128, t2 = 128;
-  for (int batch : {1, 2, 3, 5, 8, 17, 64}) {
-    for (int lag : {1, 2, 3, 4, 7}) {
-      for (int ring : {lag + 1, 2 * lag + 2}) {
-        const long total = (long)batch * (t1 + t2);
-        std::vector<long> pos1((size_t)batch * t1, -1), pos2((size_t)batch * t2, -1);
-        bool ok = true;
-        for (long w = 0; w < total; ++w) {
-          const fused::WorkItem it = fused::decode_work(w, batch, lag, t1, t2);
-          if (it.pass == 1 && it.b >= 0 && it.b < batch && it.tile >= 0 && it.tile < t1 && pos1[(size_t)it.b * t1 + it.tile] < 0)
-            pos1[(size_t)it.b * t1 + it.tile] = w;
-          else if (it.pass == 2 && it.b >= 0 && it.b < batch && it.tile >= 0 && it.tile < t2 && pos2[(size_t)it.b * t2 + it.tile] < 0)
-            pos2[(size_t)it.b * t2 + it.tile] = w;
-          else ok = false;   // out of range or duplicate
-        }
-        ok = ok && fused::decode_work(total, batch, lag, t1, t2).pass < 0;   // exhausted marker
-        for (int b = 0; b < batch && ok; ++b) {
-          long last1 = 0, first2 = total, last2 = 0, first1 = total;
-          for (int t = 0; t < t1; ++t) { last1 = std::max(last1, pos1[(size_t)b * t1 + t]); first1 = std::min(first1, pos1[(size_t)b * t1 + t]); }
-          for (int t = 0; t < t2; ++t) { first2 = std::min(first2, pos2[(size_t)b * t2 + t]); last2 = std::max(last2, pos2[(size_t)b * t2 + t]); }
-          if (first1 < 0 || first2 < 0) ok = false;                     // every tile appears
-          if (!(last1 < first2)) ok = false;                            // pass 2 of b only depends on earlier items
-          if (b + ring < batch) {                                       // slot reuse: pass 1 of b+ring after pass 2 of b
-            long f = total;
-            for (int t = 0; t < t1; ++t) f = std::min(f, pos1[(size_t)(b + ring) * t1 + t]);
-            if (!(last2 < f)) ok = false;
-          }
-        }
-        if (!ok) { printf("queue order FAILED batch=%d lag=%d ring=%d\n", batch, lag, ring); ++bad; }
-      }
+// One queue (T1 pass-1 and T2 pass-2 tiles per transform, `batch` transforms, ring / lag as launched): every tile
+// appears exactly once; pass 2 of b comes after all pass-1 tiles of b; pass 1 of b + ring comes after all pass-2
+// tiles of b (the slot is free); and in the steady state both gaps of DESIGN.md 4.2 hold exactly.  `gaps` counts the
+// steady-state gaps checked.
+static bool check_queue_order(int t1, int t2, int batch, int ring, int lag, long* gaps) {
+  const long total = (long)batch * (t1 + t2);
+  std::vector<long> pos1((size_t)batch * t1, -1), pos2((size_t)batch * t2, -1);
+  for (long w = 0; w < total; ++w) {
+    const fused::WorkItem it = fused::decode_work(w, batch, lag, t1, t2);
+    if (it.pass == 1 && it.b >= 0 && it.b < batch && it.tile >= 0 && it.tile < t1 && pos1[(size_t)it.b * t1 + it.tile] < 0)
+      pos1[(size_t)it.b * t1 + it.tile] = w;
+    else if (it.pass == 2 && it.b >= 0 && it.b < batch && it.tile >= 0 && it.tile < t2 && pos2[(size_t)it.b * t2 + it.tile] < 0)
+      pos2[(size_t)it.b * t2 + it.tile] = w;
+    else return false;   // out of range or duplicate (so, with `total` items, some tile is missing)
+  }
+  if (fused::decode_work(total, batch, lag, t1, t2).pass >= 0) return false;   // exhausted marker
+  std::vector<long> first1(batch), last1(batch), first2(batch), last2(batch);
+  for (int b = 0; b < batch; ++b) {
+    first1[b] = *std::min_element(pos1.begin() + (size_t)b * t1, pos1.begin() + (size_t)(b + 1) * t1);
+    last1[b] = *std::max_element(pos1.begin() + (size_t)b * t1, pos1.begin() + (size_t)(b + 1) * t1);
+    first2[b] = *std::min_element(pos2.begin() + (size_t)b * t2, pos2.begin() + (size_t)(b + 1) * t2);
+    last2[b] = *std::max_element(pos2.begin() + (size_t)b * t2, pos2.begin() + (size_t)(b + 1) * t2);
+  }
+  for (int b = 0; b < batch; ++b) {
+    if (!(last1[b] < first2[b])) return false;                          // pass 2 of b only depends on earlier items
+    if (b >= ring && !(last2[b - ring] < first1[b])) return false;      // slot reuse: pass 1 of b after pass 2 of b-ring
+    if (b >= lag && b + lag < batch) {                                  // steady state: pass-2 gap
+      if (first2[b] - last1[b] != (long)lag * (t1 + t2) + 1) return false;
+      ++*gaps;
+    }
+    if (b >= ring) {                                                    // steady state: slot-reuse gap
+      if (first1[b] - last2[b - ring] != (long)(ring - lag - 1) * (t1 + t2) + 1) return false;
+      ++*gaps;
     }
   }
-  printf("fused work queue: permutation / dependency-order properties %s\n", bad ? "FAILED" : "OK");
+  return true;
+}
+
+// The queue of one persistent configuration (fused_configs.cuh: the library's table): its (T1, T2) at its default
+// ring / lag and at rings 2, 3, 5 and 24 with every lag, over a range of batches, and the ring / lag the launch
+// actually uses (fused::launch_ring, the rule the library runs) for every batch 1 .. 3 x ring.
+template <class Conf>
+static int check_queue(const char* name) {
+  using Cfg = typename Conf::Cfg;
+  constexpr int t1 = Cfg::T1, t2 = Cfg::T2;
+  const int ring0 = Conf::RING, lag0 = Conf::LAG;
+  int layouts = 0, bad = 0;
+  long gaps = 0;
+  auto one = [&](int batch, int ring, int lag) {
+    ++layouts;
+    if (!check_queue_order(t1, t2, batch, ring, lag, &gaps)) {
+      printf("  queue order FAILED %s T1=%d T2=%d batch=%d ring=%d lag=%d\n", name, t1, t2, batch, ring, lag);
+      ++bad;
+    }
+  };
+  std::vector<std::pair<int, int>> rings = {{ring0, lag0}};
+  for (int ring : {2, 3, 5, 24})
+    for (int lag = 1; lag < ring; ++lag) rings.push_back({ring, lag});
+  for (auto rl : rings)
+    for (int batch : {1, 2, 3, rl.second, rl.second + 1, rl.first, rl.first + 1, 2 * rl.first + rl.second + 3})
+      one(batch, rl.first, rl.second);
+  int shrunk = 0;
+  for (int batch = 1; batch <= 3 * ring0; ++batch) {
+    const fused::RingLag rl = fused::launch_ring(ring0, lag0, batch);
+    const bool ok = rl.ring >= 2 && rl.ring <= ring0 && rl.lag >= 1 && rl.lag < rl.ring &&
+                    (rl.ring == ring0 || rl.ring >= batch);   // a shrunk ring holds the whole batch
+    if (!ok) { printf("  ring shrink FAILED %s batch=%d: ring %d lag %d\n", name, batch, rl.ring, rl.lag); ++bad; }
+    shrunk += rl.ring < ring0;
+    one(batch, rl.ring, rl.lag);
+  }
+  printf("fused work queue %s (T1 %d, T2 %d; ring %d, lag %d; rings 2, 3, 5, 24; launch rings of batches 1..%d, %d "
+         "shrunk): %d layouts, %ld steady-state gaps, permutation / dependency-order / gap properties %s\n",
+         name, t1, t2, ring0, lag0, 3 * ring0, shrunk, layouts, gaps, bad ? "FAILED" : "OK");
   return bad;
 }
 
@@ -776,7 +815,18 @@ int main() {
   bad += check_fused<fused::FusedCfg<double, 16, 8, 4, 4, 4, false, 8>>("fused f64 2^14", 5e-15);
   bad += check_fused<fused::FusedCfg<float, 16, 8, 4, FB_PAD16, 4, true>>("fused f32 2^16", 2e-6);
   bad += check_fused<fused::FusedCfg<float, 16, 8, 4, FB_PAD16, 4>>("fused f32 2^16", 2e-6);
-  bad += check_queue();
+  bad += check_queue<fused::FusedConfig<float, 13>>("f32 2^13");
+  bad += check_queue<fused::FusedConfig<float, 14>>("f32 2^14");
+  bad += check_queue<fused::FusedConfig<float, 15>>("f32 2^15");
+  bad += check_queue<fused::FusedConfig<float, 16>>("f32 2^16");
+  bad += check_queue<fused::FusedConfig<float, 17>>("f32 2^17");
+  bad += check_queue<fused::FusedConfig<float, 18>>("f32 2^18");
+  bad += check_queue<fused::FusedConfig<float, 19>>("f32 2^19");
+  bad += check_queue<fused::FusedConfig<float, 20>>("f32 2^20");
+  bad += check_queue<fused::FusedConfig<double, 12>>("f64 2^12");
+  bad += check_queue<fused::FusedConfig<double, 13>>("f64 2^13");
+  bad += check_queue<fused::FusedConfig<double, 14>>("f64 2^14");
+  bad += check_queue<fused::FusedConfig<double, 16>>("f64 2^16");
   printf(bad ? "EMULATION FAILED (%d)\n" : "EMULATION OK\n", bad);
   return bad ? 1 : 0;
 }
