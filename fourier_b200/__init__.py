@@ -11,6 +11,8 @@ reference's operator interface name for name:
                                                             transform, fft_in_place, ifft_in_place, fft, ifft
     fourier::create_fft_f32 / create_fft_f64              create_fft_f32 / create_fft_f64
       fourier/src/lib.rs:31-60
+    (no counterpart)                                      RealFft, create_rfft_f32 / create_rfft_f64:
+                                                            batched rfft / irfft of real rows
 
 Buffers are numpy arrays (host memory: staged over PCIe by the library) or torch CUDA tensors
 (device memory: transformed in HBM on torch's current stream).  A leading batch dimension is
@@ -23,7 +25,8 @@ import numpy as np
 
 from . import _lib
 
-__all__ = ["Transform", "Fft", "create_fft_f32", "create_fft_f64", "set_device", "fill_input", "lib_path"]
+__all__ = ["Transform", "Fft", "create_fft_f32", "create_fft_f64", "RealFft", "create_rfft_f32", "create_rfft_f64",
+           "set_device", "fill_input", "lib_path"]
 
 
 class Transform(enum.IntEnum):
@@ -193,6 +196,114 @@ def create_fft_f32(size, general=False):
 def create_fft_f64(size, general=False):
     """fourier::create_fft_f64 (fourier/src/lib.rs:49-60)."""
     return Fft(size, "f64", general=general)
+
+
+class RealFft:
+    """A plan for real-input transforms of one length N (numpy's rfft / irfft, batched): reals of shape (..., N) and
+    spectra of shape (..., N//2+1), with equal leading dimensions.  Out of place only."""
+
+    def __init__(self, size, real):
+        if real not in ("f32", "f64"):
+            raise ValueError("real must be 'f32' or 'f64'")
+        self.real = real
+        self._t = "float" if real == "f32" else "double"
+        self._np = {"real": np.dtype(np.float32 if real == "f32" else np.float64),
+                    "spec": np.dtype(np.complex64 if real == "f32" else np.complex128)}
+        self._plan = getattr(_lib.load(), f"fourier_b200_rfft_create_{self._t}")(int(size))
+        if not self._plan:
+            raise RuntimeError(f"fourier_b200_rfft_create_{self._t}({size}) returned NULL: {_lib.last_error()}")
+        self._size = int(size)
+        self._device = self.info()["device"]
+
+    def close(self):
+        p, self._plan = getattr(self, "_plan", None), None
+        if p:
+            getattr(_lib.load(), f"fourier_b200_rfft_destroy_{self._t}")(p)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def size(self):
+        return self._size
+
+    def info(self):
+        i = _lib.PlanInfo()
+        getattr(_lib.load(), f"fourier_b200_rfft_info_{self._t}")(self._plan, ctypes.byref(i))
+        d = {f: getattr(i, f) for f, _ in i._fields_}
+        d["path_name"] = _lib.load().fourier_b200_path_name(i.path).decode()
+        d["inner_path_name"] = _lib.load().fourier_b200_path_name(i.inner_path).decode()
+        return d
+
+    def kernel_name(self):
+        """The real kernel of the plan, and for the half-length and full-length paths the inner plan's kernel."""
+        return getattr(_lib.load(), f"fourier_b200_rfft_kernel_{self._t}")(self._plan).decode()
+
+    def _describe(self, x, kind):
+        """kind 'real' (last dimension N) or 'spec' (N//2+1) -> (pointer, leading shape, is_device, stream)"""
+        last = self._size if kind == "real" else self._size // 2 + 1
+        if _is_torch(x):
+            import torch
+            want = {("real", "f32"): torch.float32, ("real", "f64"): torch.float64,
+                    ("spec", "f32"): torch.complex64, ("spec", "f64"): torch.complex128}[(kind, self.real)]
+            if x.dtype != want:
+                raise TypeError(f"expected {want}, got {x.dtype}")
+            if not x.is_contiguous():
+                raise ValueError("buffers must be contiguous")
+            if x.dim() == 0 or x.shape[-1] != last:
+                raise ValueError(f"last dimension must be {last}")
+            if x.is_cuda:
+                if x.device.index != self._device:
+                    raise ValueError(f"plan lives on cuda:{self._device}, buffer on {x.device}")
+                return x.data_ptr(), tuple(x.shape[:-1]), True, torch.cuda.current_stream(x.device).cuda_stream
+            return x.data_ptr(), tuple(x.shape[:-1]), False, None
+        if not isinstance(x, np.ndarray):
+            raise TypeError("buffers must be numpy arrays or torch tensors")
+        if x.dtype != self._np[kind]:
+            raise TypeError(f"expected {self._np[kind]}, got {x.dtype}")
+        if not x.flags.c_contiguous:
+            raise ValueError("buffers must be C-contiguous")
+        if x.ndim == 0 or x.shape[-1] != last:
+            raise ValueError(f"last dimension must be {last}")
+        return x.ctypes.data, tuple(x.shape[:-1]), False, None
+
+    def _run(self, direction, src, dst, transform):
+        code = int(Transform(transform))
+        kinds = ("real", "spec") if direction == "forward" else ("spec", "real")
+        pi, li, di, si = self._describe(src, kinds[0])
+        po, lo, do_, _ = self._describe(dst, kinds[1])
+        if li != lo:
+            raise ValueError(f"leading dimensions differ: {li} and {lo}")
+        if di != do_:
+            raise ValueError("input and output must both be host or both be device buffers")
+        batch = int(np.prod(li, dtype=np.int64))
+        L = _lib.load()
+        if di:
+            rc = getattr(L, f"fourier_b200_rfft_{direction}_async_{self._t}")(self._plan, pi, po, batch, code, si)
+        else:
+            rc = getattr(L, f"fourier_b200_rfft_{direction}_{self._t}")(self._plan, pi, po, batch, code)
+        if rc != 0:
+            raise RuntimeError(f"real {direction} transform failed (cuda error {rc}): {_lib.last_error()}")
+
+    def rfft(self, input, output, transform=Transform.Fft):
+        """output[..., :N//2+1] = numpy.fft.rfft(input) (Fft) or that times 1/sqrt(N) (SqrtScaledFft)."""
+        self._run("forward", input, output, transform)
+
+    def irfft(self, input, output, transform=Transform.Ifft):
+        """output = numpy.fft.irfft(input, n=N) (Ifft), N times that (UnscaledIfft) or sqrt(N) times (SqrtScaledIfft)."""
+        self._run("inverse", input, output, transform)
+
+
+def create_rfft_f32(size):
+    """Real-input transforms of length `size` in single precision."""
+    return RealFft(size, "f32")
+
+
+def create_rfft_f64(size):
+    """Real-input transforms of length `size` in double precision."""
+    return RealFft(size, "f64")
 
 
 def set_device(device):

@@ -27,7 +27,9 @@ EXTENSION_SYMBOLS = (
      "fourier_b200_path_name", "fourier_b200_last_error", "fourier_b200_version"]
     + [f"fourier_b200_{op}_{t}" for t in ("float", "double")
        for op in ("transform_batch", "transform_batch_async", "plan_info", "create_general", "fill_input",
-                  "transpose", "pack", "exchange", "fft_rows_exchange", "swap_leading", "twiddle_rows", "plan_kernel")])
+                  "transpose", "pack", "exchange", "fft_rows_exchange", "swap_leading", "twiddle_rows", "plan_kernel")]
+    + [f"fourier_b200_rfft_{op}_{t}" for t in ("float", "double")
+       for op in ("create", "destroy", "forward", "forward_async", "inverse", "inverse_async", "info", "kernel")])
 
 
 def load():
@@ -66,6 +68,16 @@ def load():
                                                                     ctypes.c_ulonglong, ctypes.c_ulonglong, vp]
         getattr(L, f"fourier_b200_swap_leading_{t}").argtypes = [vp, vp, sz, sz, sz, vp]
         getattr(L, f"fourier_b200_twiddle_rows_{t}").argtypes = [vp, sz, sz, ctypes.c_ulonglong, ctypes.c_ulonglong, ci, vp]
+        getattr(L, f"fourier_b200_rfft_create_{t}").restype = vp
+        getattr(L, f"fourier_b200_rfft_create_{t}").argtypes = [sz]
+        getattr(L, f"fourier_b200_rfft_destroy_{t}").restype = None
+        getattr(L, f"fourier_b200_rfft_destroy_{t}").argtypes = [vp]
+        for d in ("forward", "inverse"):
+            getattr(L, f"fourier_b200_rfft_{d}_{t}").argtypes = [vp, vp, vp, sz, ci]
+            getattr(L, f"fourier_b200_rfft_{d}_async_{t}").argtypes = [vp, vp, vp, sz, ci, vp]
+        getattr(L, f"fourier_b200_rfft_info_{t}").argtypes = [vp, ctypes.POINTER(PlanInfo)]
+        getattr(L, f"fourier_b200_rfft_kernel_{t}").restype = ctypes.c_char_p
+        getattr(L, f"fourier_b200_rfft_kernel_{t}").argtypes = [vp]
     L.fourier_b200_peer_alloc.argtypes = [sz, ctypes.POINTER(vp), ctypes.c_char_p]
     L.fourier_b200_peer_open.argtypes = [ctypes.c_char_p, ctypes.POINTER(vp)]
     L.fourier_b200_peer_close.argtypes = [vp]

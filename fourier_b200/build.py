@@ -22,7 +22,7 @@ VERSION = "0.1.0"
 SONAME = "libfourier.so.0"
 REAL = f"libfourier.so.{VERSION}"
 
-SOURCES = ["plan.cu", "host_math.cu", "stockham_generic.cu", "onchip.cu", "cta_fft.cu", "twopass.cu", "synth.cu", "exchange.cu", "dist_fft.cu", "bigpow2.cu", "capi.cu"]
+SOURCES = ["plan.cu", "host_math.cu", "stockham_generic.cu", "onchip.cu", "cta_fft.cu", "twopass.cu", "synth.cu", "exchange.cu", "dist_fft.cu", "bigpow2.cu", "real.cu", "capi.cu"]
 
 # H100: the kernels use TMA and mbarrier, so the arch-specific target is required
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]

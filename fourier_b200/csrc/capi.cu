@@ -1,6 +1,6 @@
 // capi.cu -- the C ABI of libfourier.so: the eight reference symbols (include/fourier.h, replacing
 // fourier-ffi/src/lib.rs:14-106) and the additive batched / device-pointer entry points
-// (include/fourier_b200.h).  No torch types, plain pointers and sizes only.
+// (include/fourier_b200.h), real-input transforms included.  No torch types, plain pointers and sizes only.
 //
 // Error convention of the reference symbols (fourier-ffi/src/lib.rs): create returns NULL when the
 // constructor fails; transform_* / destroy swallow every failure (catch_unwind) and return nothing.
@@ -15,6 +15,7 @@
 #include "plan.h"
 
 using fb200::Plan;
+using fb200::RealPlan;
 
 namespace {
 
@@ -121,6 +122,71 @@ template <typename T>
 int plan_info(const void* plan, fourier_b200_plan_info* out) {
   if (!plan || !out) return (int)cudaErrorInvalidValue;
   const auto* p = static_cast<const Plan<T>*>(plan);
+  const fb200::PlanInfo i = p->info();
+  out->size = i.size; out->path = i.path; out->inner_size = i.inner_size; out->inner_path = i.inner_path;
+  out->n1 = i.n1; out->n2 = i.n2; out->precision_bytes = i.precision_bytes; out->device = i.device;
+  out->table_bytes = i.table_bytes; out->last_launches = p->launches();
+  return 0;
+}
+
+template <typename T>
+void* create_real_plan(size_t size) {
+  const int dev = resolve_device();
+  if (dev < 0) {
+    fb200::set_last_error("no usable CUDA device (libfourier.so has no CPU fallback)");
+    return nullptr;
+  }
+  try {
+    return RealPlan<T>::create(size, dev);
+  } catch (...) {
+    fb200::set_last_error("plan construction threw");
+    return nullptr;
+  }
+}
+
+// Real transforms are out of place: the byte ranges [in, in + in_bytes) and [out, out + out_bytes) must not meet.
+bool disjoint(const void* in, size_t in_bytes, const void* out, size_t out_bytes) {
+  const uintptr_t a = (uintptr_t)in, b = (uintptr_t)out;
+  if (a < b + out_bytes && b < a + in_bytes) {
+    fb200::set_last_error("input and output overlap (real transforms are out of place only)");
+    return false;
+  }
+  return true;
+}
+
+// async: device pointers on `stream`, not synchronised; otherwise host or device pointers, synchronised.
+template <typename T>
+int rfft_exec(void* plan, bool forward, const void* in, void* out, size_t batch, int code, bool async, void* stream) {
+  if (!plan || !in || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  try {
+    if (cudaError_t e = p->check_code(forward, code)) return (int)e;
+    if (batch == 0) return (int)p->exec_device(forward, in, out, 0, code, nullptr);
+    if (!disjoint(in, batch * p->row_bytes(forward, true), out, batch * p->row_bytes(forward, false)))
+      return (int)cudaErrorInvalidValue;
+    if (!async) {
+      const bool din = is_device_pointer(in), dout = is_device_pointer(out);
+      if (din != dout) {
+        fb200::set_last_error("input and output must both be host or both be device memory");
+        return (int)cudaErrorInvalidValue;
+      }
+      if (!din) return (int)p->exec_host(forward, in, out, batch, code);
+    }
+    if (!device_pointers_aligned(in, out)) return (int)cudaErrorMisalignedAddress;
+    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
+    cudaError_t e = p->exec_device(forward, in, out, batch, code, s);
+    if (e != cudaSuccess || async) return (int)e;
+    return (int)cudaStreamSynchronize(s);
+  } catch (...) {
+    fb200::set_last_error("real transform threw");
+    return (int)cudaErrorUnknown;
+  }
+}
+
+template <typename T>
+int rfft_info(const void* plan, fourier_b200_plan_info* out) {
+  if (!plan || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
+  const auto* p = static_cast<const RealPlan<T>*>(plan);
   const fb200::PlanInfo i = p->info();
   out->size = i.size; out->path = i.path; out->inner_size = i.inner_size; out->inner_path = i.inner_path;
   out->n1 = i.n1; out->n2 = i.n2; out->precision_bytes = i.precision_bytes; out->device = i.device;
@@ -292,6 +358,60 @@ int fourier_b200_twiddle_rows_float(void* data, size_t rows, size_t cols, unsign
 int fourier_b200_twiddle_rows_double(void* data, size_t rows, size_t cols, unsigned long long row0,
                                      unsigned long long n_total, int forward, void* stream) {
   return (int)fb200::launch_twiddle_rows<double>((double2*)data, rows, cols, row0, n_total, forward != 0, (cudaStream_t)stream);
+}
+
+// ---- real-input transforms ------------------------------------------------------------------------------
+fourier_b200_rfft_float* fourier_b200_rfft_create_float(size_t n) {
+  return static_cast<fourier_b200_rfft_float*>(create_real_plan<float>(n));
+}
+fourier_b200_rfft_double* fourier_b200_rfft_create_double(size_t n) {
+  return static_cast<fourier_b200_rfft_double*>(create_real_plan<double>(n));
+}
+void fourier_b200_rfft_destroy_float(fourier_b200_rfft_float* plan) {
+  try { delete reinterpret_cast<RealPlan<float>*>(plan); } catch (...) {}
+}
+void fourier_b200_rfft_destroy_double(fourier_b200_rfft_double* plan) {
+  try { delete reinterpret_cast<RealPlan<double>*>(plan); } catch (...) {}
+}
+int fourier_b200_rfft_forward_float(fourier_b200_rfft_float* plan, const float* in, void* out, size_t batch, int t) {
+  return rfft_exec<float>(plan, true, in, out, batch, t, false, nullptr);
+}
+int fourier_b200_rfft_forward_double(fourier_b200_rfft_double* plan, const double* in, void* out, size_t batch, int t) {
+  return rfft_exec<double>(plan, true, in, out, batch, t, false, nullptr);
+}
+int fourier_b200_rfft_forward_async_float(fourier_b200_rfft_float* plan, const float* in, void* out, size_t batch, int t,
+                                          void* stream) {
+  return rfft_exec<float>(plan, true, in, out, batch, t, true, stream);
+}
+int fourier_b200_rfft_forward_async_double(fourier_b200_rfft_double* plan, const double* in, void* out, size_t batch,
+                                           int t, void* stream) {
+  return rfft_exec<double>(plan, true, in, out, batch, t, true, stream);
+}
+int fourier_b200_rfft_inverse_float(fourier_b200_rfft_float* plan, const void* in, float* out, size_t batch, int t) {
+  return rfft_exec<float>(plan, false, in, out, batch, t, false, nullptr);
+}
+int fourier_b200_rfft_inverse_double(fourier_b200_rfft_double* plan, const void* in, double* out, size_t batch, int t) {
+  return rfft_exec<double>(plan, false, in, out, batch, t, false, nullptr);
+}
+int fourier_b200_rfft_inverse_async_float(fourier_b200_rfft_float* plan, const void* in, float* out, size_t batch, int t,
+                                          void* stream) {
+  return rfft_exec<float>(plan, false, in, out, batch, t, true, stream);
+}
+int fourier_b200_rfft_inverse_async_double(fourier_b200_rfft_double* plan, const void* in, double* out, size_t batch,
+                                           int t, void* stream) {
+  return rfft_exec<double>(plan, false, in, out, batch, t, true, stream);
+}
+int fourier_b200_rfft_info_float(const fourier_b200_rfft_float* plan, fourier_b200_plan_info* out) {
+  return rfft_info<float>(plan, out);
+}
+int fourier_b200_rfft_info_double(const fourier_b200_rfft_double* plan, fourier_b200_plan_info* out) {
+  return rfft_info<double>(plan, out);
+}
+const char* fourier_b200_rfft_kernel_float(const fourier_b200_rfft_float* plan) {
+  return plan ? reinterpret_cast<const RealPlan<float>*>(plan)->kernel_name() : "";
+}
+const char* fourier_b200_rfft_kernel_double(const fourier_b200_rfft_double* plan) {
+  return plan ? reinterpret_cast<const RealPlan<double>*>(plan)->kernel_name() : "";
 }
 
 const char* fourier_b200_last_error(void) { return fb200::last_error(); }

@@ -1,5 +1,6 @@
 // onchip.cu -- plans and launchers for the transforms that fit on chip (onchip_kernels.cuh):
-// batched power-of-two FFTs up to 1024 points and the fused Bluestein kernel for N <= 1024.
+// batched power-of-two FFTs up to 1024 points, the fused Bluestein kernel for N <= 1024 and the fused
+// real-input kernels for N = 2L (real.cu drives them).
 // Reference counterparts: Autosort for small sizes (autosort/mod.rs:141-166) and
 // Bluesteins::transform_in_place / apply (bluesteins.rs:193-259).
 #include <algorithm>
@@ -34,6 +35,7 @@ template <typename T> struct OnChipOps {
   cudaError_t (*bluestein)(const cpx<T>*, cpx<T>*, const void* twa, const cpx<T>* chirp, const cpx<T>* wm,
                            const cpx<T>* wce, const cpx<T>* wco, size_t n, size_t batch, T scale, int sms,
                            cudaStream_t);
+  const RealOnChipOps<T>* real;   // real-input transforms of length 2L on the same tiles
 };
 
 template <typename T, int RA, int RB, int E, int WARPS, int MINB, int BWARPS, bool LOCAL_STASH = false>
@@ -84,8 +86,31 @@ struct OnChipImpl {
       return cudaErrorNotSupported;
     }
   }
+  static cudaError_t real_prepare() {
+    cudaError_t e;
+    if ((e = cudaFuncSetAttribute(onchip::onchip_real_kernel<Cfg<true>, MINB>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_fft))) return e;
+    return cudaFuncSetAttribute(onchip::onchip_real_kernel<Cfg<false>, MINB>,
+                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_fft);
+  }
+  static cudaError_t real(const void* in, void* out, const void* twa, const cpx<T>* tab, size_t batch, bool fwd, T h,
+                          int sms, cudaStream_t s) {
+    const size_t groups = (batch + Cfg<true>::C - 1) / Cfg<true>::C;
+    const unsigned grid = (unsigned)std::min<size_t>(groups, (size_t)sms * MINB * 4);
+    if (fwd) {
+      const typename onchip::RealBody<Cfg<true>>::Args a = {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab,
+                                                            (long)batch, h};
+      onchip::onchip_real_kernel<Cfg<true>, MINB><<<grid, Cfg<true>::THREADS, smem_fft, s>>>(a);
+    } else {
+      const typename onchip::RealBody<Cfg<false>>::Args a = {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab,
+                                                             (long)batch, h};
+      onchip::onchip_real_kernel<Cfg<false>, MINB><<<grid, Cfg<false>::THREADS, smem_fft, s>>>(a);
+    }
+    return cudaGetLastError();
+  }
   static const OnChipOps<T>* ops() {
-    static const OnChipOps<T> o = {RA, RB, &prepare, &fft, kHasBluestein ? &bluestein : nullptr};
+    static const RealOnChipOps<T> r = {RA, RB, &real_prepare, &real};
+    static const OnChipOps<T> o = {RA, RB, &prepare, &fft, kHasBluestein ? &bluestein : nullptr, &r};
     return &o;
   }
 };
@@ -201,6 +226,14 @@ cudaError_t Plan<T>::exec_bluestein_fused(const C* in, C* out, size_t batch, int
   return cudaSuccess;
 }
 
+template <typename T>
+const RealOnChipOps<T>* real_onchip_lookup(size_t m) {
+  const OnChipOps<T>* ops = onchip_lookup<T>(m);
+  return ops ? ops->real : nullptr;
+}
+
+template const RealOnChipOps<float>* real_onchip_lookup<float>(size_t);
+template const RealOnChipOps<double>* real_onchip_lookup<double>(size_t);
 template cudaError_t Plan<float>::init_onchip();
 template cudaError_t Plan<double>::init_onchip();
 template cudaError_t Plan<float>::exec_onchip(const C*, C*, size_t, int, cudaStream_t);

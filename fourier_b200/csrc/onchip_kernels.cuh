@@ -4,6 +4,7 @@
 //
 //   * onchip_fft_kernel:      batched power-of-two FFT, N = L in {64 .. 1024}: global -> registers ->
 //                             one warp-private shared-memory exchange -> registers -> global.
+//   * onchip_real_kernel:     real-input transforms of length 2L (forward and inverse) on the same tiles.
 //   * bluestein_fused_kernel: the whole chirp-z transform of the reference (bluesteins.rs:218-259) for
 //                             N <= L, M = 2L, in one kernel and without touching HBM in between.
 //
@@ -16,6 +17,7 @@
 // multiplies, so only the forward tile is instantiated.
 #pragma once
 
+#include "real_kernels.cuh"
 #include "tilefft.cuh"
 
 namespace fb200 {
@@ -95,6 +97,102 @@ onchip_fft_kernel(const typename FftBody<Cfg>::Args a) {
     Body::phase1(f, a, grp, threadIdx.x, exch, twa);
     __syncwarp();
     Body::phase2(f, a, grp, threadIdx.x, exch);
+    __syncwarp();
+  }
+}
+
+// ---- fused real-input transforms, N = 2L (real_kernels.cuh) ----------------------------------------------------
+// Forward: the 2L reals of a row are loaded as L complex values with FftBody's loads and run through the tile; the
+// spectrum Z is parked in natural order in the FFT's own block of the exchange buffer, and each lane untangles the
+// pairs (k, L-k), k = u + TP*j, into the L+1 bins of the row (lane u = 0 also the self-paired k = L/2).
+// Inverse: the lane that owns stage-A position n forms Z'[n] from X[n] and X[L-n] in registers; the tile's own store
+// writes z' as interleaved reals.  One launch, one trip through HBM.
+template <class Cfg> struct RealBody {
+  using Tile = typename Cfg::Tile;
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  using Fft = FftBody<Cfg>;
+  static constexpr int L = Cfg::L, TP = Tile::TP, RA = Tile::RA, RB = Tile::RB, E = Tile::E;
+  struct Args { const V* in; V* out; const TwPair<T>* twa; const V* tab; long batch; T h; };
+
+  // the FFT `col` of the CTA keeps Z in natural order at smem[col * SC + k], k < L (inside its exchange block)
+  static FB_HD int park(int t) { return Tile::template col_of<true>(t) * Cfg::Lay::SC; }
+
+  static FB_HD void fwd_phase1(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    const typename Fft::Args fa = {a.in, nullptr, twa, a.batch, (T)1, 0};
+    Fft::phase1(f, fa, grp, t, smem, twa);
+  }
+  static FB_HD void fwd_gather(Tile& f, int t, const V* smem) {
+    f.template gather<true, typename Cfg::Lay>(t, smem);
+    f.stage_b();
+  }
+  static FB_HD void fwd_park(const Tile& f, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    V* z = smem + park(t);
+    static_for<0, Tile::NB>([&](auto Cc) FB_LAMBDA {
+      constexpr int c = decltype(Cc)::value;
+      static_for<0, RB>([&](auto Rr) FB_LAMBDA {
+        constexpr int r = decltype(Rr)::value;
+        z[(u + TP * c) + RA * r] = f.v[c * RB + bitrev(r, ilog2(RB))];
+      });
+    });
+  }
+  static FB_HD void fwd_store(const Args& a, long grp, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const long b = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (b >= a.batch) return;
+    const V* z = smem + park(t);
+    V* x = a.out + b * (L + 1);
+#pragma unroll
+    for (int j = 0; j < E / 2; ++j) real::untangle(z, x, (long)L, (long)(u + TP * j), a.tab, a.h);
+    if (u == 0) real::untangle(z, x, (long)L, (long)(L / 2), a.tab, a.h);
+  }
+
+  static FB_HD void inv_phase1(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    const int u = Tile::template u_of<true>(t);
+    long b = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (b >= a.batch) b = a.batch - 1;
+    const V* x = a.in + b * (L + 1);
+#pragma unroll
+    for (int q = 0; q < Tile::NA; ++q)
+#pragma unroll
+      for (int i = 0; i < RA; ++i) f.v[q * RA + i] = real::tangle_one(x, (long)L, (long)(u + TP * q + RB * i), a.tab, a.h);
+    f.template stage_a<true>(t, twa);
+    f.template scatter<true, typename Cfg::Lay>(t, smem);
+  }
+  static FB_HD void inv_phase2(Tile& f, const Args& a, long grp, int t, const V* smem) {
+    const typename Fft::Args fa = {nullptr, a.out, nullptr, a.batch, (T)1, 0};
+    Fft::phase2(f, fa, grp, t, smem);
+  }
+};
+
+template <class Cfg, int MINB>
+__global__ void __launch_bounds__(Cfg::THREADS, MINB)
+onchip_real_kernel(const typename RealBody<Cfg>::Args a) {
+  using Body = RealBody<Cfg>;
+  using V = typename Cfg::Tile::V;
+  using T = decltype(V::x);
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  V* exch = reinterpret_cast<V*>(smem_raw);
+  TwPair<T>* twa = reinterpret_cast<TwPair<T>*>(smem_raw + Cfg::EX_BYTES);
+  for (int i = threadIdx.x; i < (Cfg::Tile::RA / 2) * Cfg::Tile::RB; i += Cfg::THREADS) twa[i] = a.twa[i];
+  __syncthreads();
+  const long groups = (a.batch + Cfg::C - 1) / Cfg::C;
+  typename Cfg::Tile f;
+  for (long grp = blockIdx.x; grp < groups; grp += gridDim.x) {
+    if constexpr (Cfg::Tile::FWD) {
+      Body::fwd_phase1(f, a, grp, threadIdx.x, exch, twa);
+      __syncwarp();
+      Body::fwd_gather(f, threadIdx.x, exch);
+      __syncwarp();
+      Body::fwd_park(f, threadIdx.x, exch);
+      __syncwarp();
+      Body::fwd_store(a, grp, threadIdx.x, exch);
+    } else {
+      Body::inv_phase1(f, a, grp, threadIdx.x, exch, twa);
+      __syncwarp();
+      Body::inv_phase2(f, a, grp, threadIdx.x, exch);
+    }
     __syncwarp();
   }
 }

@@ -42,6 +42,9 @@ const char* path_name(Path p) {
     case Path::kBluesteinFused: return "bluestein_fused";
     case Path::kCta: return "onchip_cta";
     case Path::kThreePass: return "threepass";
+    case Path::kRealFused: return "real_fused";
+    case Path::kRealHalf: return "real_half";
+    case Path::kRealFull: return "real_full";
   }
   return "?";
 }
@@ -97,8 +100,6 @@ template <typename T> T scale_for(int code, size_t n) {
   }
 }
 
-constexpr size_t kScratchTargetBytes = (size_t)512 << 20;  // per scratch buffer on the general path
-constexpr size_t kHostChunkBytes = (size_t)64 << 20;       // host-pointer pipeline granule
 constexpr size_t kHostSmallBytes = (size_t)1 << 20;        // below this a host call takes the single-stream latency path
 constexpr size_t kHostZeroCopyBytes = (size_t)64 << 10;    // below this the kernel reads / writes mapped host memory itself
 

@@ -30,9 +30,16 @@ enum class Path : int {
   kCta = 6,             // whole transforms in shared memory, one CTA per group of transforms, all Stockham stages
                         // in one kernel ({2,3}-smooth N, pow2 N between the on-chip and two-pass kernels)
   kThreePass = 7,       // pow2 N above the two-pass kernels: outer column pass + two-pass rows storing transposed
+  // real-input plans (RealPlan, real.cu)
+  kRealFused = 8,       // N = 2M, M an on-chip size class: one fused on-chip kernel
+  kRealHalf = 9,        // other even N: complex plan of length N/2 + one untangle / tangle kernel
+  kRealFull = 10,       // odd N: complex plan of length N between two O(N) kernels
 };
 
 const char* path_name(Path p);
+
+constexpr size_t kScratchTargetBytes = (size_t)512 << 20;  // per scratch buffer on the general and real paths
+constexpr size_t kHostChunkBytes = (size_t)64 << 20;       // host-pointer pipeline granule
 
 constexpr int kMaxPeers = 16;   // ranks of one box (peer-memory exchange, exchange.cu / dist_fft.cu)
 
@@ -201,6 +208,68 @@ class Plan {
   cudaError_t host_resources();   // streams and events of the host-pointer path, created once
   void* zc_in_ = nullptr;         // pinned, device-mapped bounce buffers of the smallest host calls (64 KB each)
   void* zc_out_ = nullptr;
+};
+
+// onchip.cu: the fused real-input kernels of the on-chip size class of L (onchip_lookup), N = 2L; nullptr when L has
+// none.  run(): `in` / `out` are the reals (L complex values per row) and the spectrum (L+1 per row), swapped for the
+// inverse; tab = w_N^k, k <= L/2; h = scale / 2 (forward) or scale (inverse).
+template <typename T> struct RealOnChipOps {
+  int ra, rb;
+  cudaError_t (*prepare)();
+  cudaError_t (*run)(const void* in, void* out, const void* twa, const cpx<T>* tab, size_t batch, bool fwd, T h,
+                     int sms, cudaStream_t);
+};
+template <typename T> const RealOnChipOps<T>* real_onchip_lookup(size_t l);
+
+// Batched real-input transform of length N (real.cu, DESIGN.md §4.10).  Forward: `batch` rows of N reals -> rows of
+// N/2+1 complex bins (numpy's rfft layout); inverse: the other way round (numpy's irfft).  Out of place only.
+template <typename T>
+class RealPlan {
+ public:
+  using C = cpx<T>;
+
+  // nullptr (and last_error set) when the plan cannot be built; size 0 is refused
+  static RealPlan* create(size_t n, int device, bool allow_fast_paths = true);
+  ~RealPlan();
+
+  size_t size() const { return n_; }
+  Path path() const { return path_; }
+  PlanInfo info() const;
+
+  // Device pointers, enqueued on `stream`, not synchronised.  `forward` selects the direction; a code of the other
+  // direction is refused.
+  cudaError_t exec_device(bool forward, const void* in, void* out, size_t batch, int code, cudaStream_t stream);
+  // Host pointers: staged through the plan's device buffers in chunks, the same device code; returns when `out` is done.
+  cudaError_t exec_host(bool forward, const void* in, void* out, size_t batch, int code);
+
+  unsigned long long launches() const { return launches_; }
+  const char* kernel_name() const { return kernel_desc_.c_str(); }
+
+  // cudaErrorInvalidValue (and last_error set) for an unknown code or one of the other direction
+  cudaError_t check_code(bool forward, int code) const;
+
+  // bytes of one input / output row
+  size_t row_bytes(bool forward, bool input) const {
+    const size_t real = n_ * sizeof(T), spec = (n_ / 2 + 1) * sizeof(C);
+    return forward == input ? real : spec;
+  }
+
+ private:
+  RealPlan() = default;
+  cudaError_t init(size_t n, int device, bool allow_fast_paths);
+
+  size_t n_ = 0, m_ = 0;        // m_ = N/2 (even N)
+  int device_ = 0;
+  Path path_ = Path::kRealFull;
+  unsigned long long launches_ = 0;
+  int sm_count_ = 132;
+  const RealOnChipOps<T>* fused_ = nullptr;
+  std::unique_ptr<Plan<T>> inner_;   // length N/2 (kRealHalf) or N (kRealFull)
+  DeviceBuffer tab_, twa_;           // w_N^k, k <= N/4 (even N); stage twiddles of the fused kernel
+  DeviceBuffer work_;                // one chunk of inner-plan rows
+  DeviceBuffer stage_in_, stage_out_;
+  cudaStream_t host_stream_ = nullptr;
+  std::string kernel_desc_;
 };
 
 // thread-local error text for the C ABI

@@ -1,0 +1,278 @@
+// real.cu -- real-input transforms (DESIGN.md §4.10): plan construction, path selection, and the O(N) kernels
+// around the inner complex plan.
+//
+//   kRealFused  N = 2M, M an on-chip size class: onchip_real_kernel (onchip_kernels.cuh), one launch.
+//   kRealHalf   other even N: the reals as M = N/2 complex values through a complex plan of length M, and one
+//               untangle (forward) / tangle (inverse) kernel over a plan-owned scratch chunk.
+//   kRealFull   odd N: widen to complex, complex plan of length N, first (N+1)/2 bins; the inverse extends the bins
+//               to a Hermitian spectrum, runs the complex inverse and keeps the real parts.  Correctness path only.
+#include <algorithm>
+#include <cmath>
+#include <exception>
+#include <new>
+#include <string>
+#include <vector>
+
+#include "plan.h"
+#include "real_kernels.cuh"
+#include "tables.cuh"  // make_twa
+
+namespace fb200 {
+
+#define FB_CHECK(expr)                                                                       \
+  do {                                                                                       \
+    cudaError_t _e = (expr);                                                                 \
+    if (_e != cudaSuccess) {                                                                 \
+      set_last_error(std::string(#expr) + ": " + cudaGetErrorString(_e));                    \
+      return _e;                                                                             \
+    }                                                                                        \
+  } while (0)
+
+namespace {
+
+constexpr int kThreads = 256;
+
+inline unsigned grid_for(size_t total) {
+  size_t blocks = (total + kThreads - 1) / kThreads;
+  const size_t cap = 132u * 32u;
+  return (unsigned)std::max<size_t>(1, std::min(blocks, cap));
+}
+
+// One thread per pair (k, M-k), k <= M/2, of one row: consecutive threads read Z[k] ascending and Z[M-k] descending.
+template <typename T, bool FWD>
+__global__ void __launch_bounds__(kThreads)
+untangle_kernel(const cpx<T>* __restrict__ in, cpx<T>* __restrict__ out, const cpx<T>* __restrict__ tab, long m,
+                long batch, T h) {
+  const long pairs = m / 2 + 1, total = pairs * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / pairs, k = g - b * pairs;
+    if (FWD) real::untangle(in + b * m, out + b * (m + 1), m, k, tab, h);
+    else real::tangle(in + b * (m + 1), out + b * m, m, k, tab, h);
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+widen_kernel(const T* __restrict__ in, cpx<T>* __restrict__ out, size_t count) {
+  for (size_t g = blockIdx.x * (size_t)blockDim.x + threadIdx.x; g < count; g += (size_t)gridDim.x * blockDim.x)
+    out[g] = mk<T>(in[g], (T)0);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+copy_bins_kernel(const cpx<T>* __restrict__ y, cpx<T>* __restrict__ x, long n, long batch) {
+  const long bins = n / 2 + 1, total = bins * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / bins, k = g - b * bins;
+    real::copy_bin(y + b * n, x + b * bins, k);
+  }
+}
+
+// grid.y runs over rows, grid.x along a row
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+hermitian_kernel(const cpx<T>* __restrict__ x, cpx<T>* __restrict__ y, long n, long batch) {
+  const long bins = n / 2 + 1;
+  for (long b = blockIdx.y; b < batch; b += gridDim.y)
+    for (long k = blockIdx.x * (long)blockDim.x + threadIdx.x; k < n; k += (long)gridDim.x * blockDim.x)
+      y[b * n + k] = real::hermitian(x + b * bins, n, k);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+real_part_kernel(const cpx<T>* __restrict__ y, T* __restrict__ out, size_t count) {
+  for (size_t g = blockIdx.x * (size_t)blockDim.x + threadIdx.x; g < count; g += (size_t)gridDim.x * blockDim.x)
+    out[g] = y[g].x;
+}
+
+template <typename T> T scale_of(int code, size_t n) {
+  if (code == kIfft) return (T)1 / (T)n;
+  if (code == kSqrtScaledFft || code == kSqrtScaledIfft) return (T)1 / std::sqrt((T)n);
+  return (T)1;
+}
+
+template <typename T, typename U>
+cudaError_t upload_vec(DeviceBuffer& buf, const std::vector<U>& host) {
+  cudaError_t e = buf.reserve(std::max<size_t>(host.size(), 1) * sizeof(U));
+  if (e != cudaSuccess || host.empty()) return e;
+  return cudaMemcpy(buf.data(), host.data(), host.size() * sizeof(U), cudaMemcpyHostToDevice);
+}
+
+}  // namespace
+
+template <typename T>
+RealPlan<T>* RealPlan<T>::create(size_t n, int device, bool allow_fast_paths) {
+  if (n == 0) {
+    set_last_error("size 0 is not a valid transform length");
+    return nullptr;
+  }
+  RealPlan<T>* p = new (std::nothrow) RealPlan<T>();
+  if (!p) return nullptr;
+  cudaError_t e = cudaErrorUnknown;
+  try {
+    e = p->init(n, device, allow_fast_paths);
+  } catch (const std::exception& ex) {
+    set_last_error(std::string("plan construction threw: ") + ex.what());
+  }
+  if (e != cudaSuccess) {
+    delete p;
+    return nullptr;
+  }
+  return p;
+}
+
+template <typename T>
+RealPlan<T>::~RealPlan() {
+  DeviceGuard g(device_);
+  if (host_stream_) cudaStreamDestroy(host_stream_);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::init(size_t n, int device, bool allow_fast_paths) {
+  n_ = n;
+  device_ = device;
+  DeviceGuard g(device_);
+  if (!g.ok) { set_last_error("cudaSetDevice failed"); return cudaErrorInvalidDevice; }
+  if (n % 2 != 0) {
+    inner_.reset(Plan<T>::create(n, device, allow_fast_paths));
+    if (!inner_) return cudaErrorUnknown;
+    path_ = Path::kRealFull;
+    kernel_desc_ = std::string("real::widen_kernel / real::hermitian_kernel + ") + inner_->kernel_name();
+    return cudaSuccess;
+  }
+  m_ = n / 2;
+  std::vector<C> tab(m_ / 2 + 1);
+  for (size_t k = 0; k < tab.size(); ++k) {
+    double re, im;
+    host_twiddle(k, n, &re, &im);
+    tab[k] = mk<T>((T)re, (T)im);
+  }
+  FB_CHECK((upload_vec<T, C>(tab_, tab)));
+  if (allow_fast_paths && (fused_ = real_onchip_lookup<T>(m_)) != nullptr) {
+    FB_CHECK(fused_->prepare());
+    FB_CHECK((upload_vec<T, TwPair<T>>(twa_, twopass::make_twa<T>(fused_->ra, fused_->rb))));
+    if (cudaDeviceGetAttribute(&sm_count_, cudaDevAttrMultiProcessorCount, device_) != cudaSuccess) sm_count_ = 132;
+    path_ = Path::kRealFused;
+    kernel_desc_ = "onchip::onchip_real_kernel";
+    return cudaSuccess;
+  }
+  inner_.reset(Plan<T>::create(m_, device, allow_fast_paths));
+  if (!inner_) return cudaErrorUnknown;
+  path_ = Path::kRealHalf;
+  kernel_desc_ = std::string("real::untangle_kernel / real::tangle_kernel + ") + inner_->kernel_name();
+  return cudaSuccess;
+}
+
+template <typename T>
+PlanInfo RealPlan<T>::info() const {
+  PlanInfo i;
+  if (inner_) i = inner_->info();
+  i.inner_size = inner_ ? inner_->size() : 0;
+  i.inner_path = inner_ ? (int)inner_->path() : 0;
+  i.size = n_;
+  i.path = (int)path_;
+  i.precision_bytes = (int)sizeof(T);
+  i.device = device_;
+  i.table_bytes = tab_.bytes() + twa_.bytes() + (inner_ ? inner_->info().table_bytes : 0);
+  return i;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::check_code(bool forward, int code) const {
+  if (code < 0 || code > 4) { set_last_error("unknown transform code"); return cudaErrorInvalidValue; }
+  if (transform_is_forward(code) != forward) {
+    set_last_error(forward ? "the forward real transform takes Fft or SqrtScaledFft"
+                           : "the inverse real transform takes Ifft, UnscaledIfft or SqrtScaledIfft");
+    return cudaErrorInvalidValue;
+  }
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::exec_device(bool forward, const void* in, void* out, size_t batch, int code,
+                                     cudaStream_t s) {
+  launches_ = 0;
+  if (cudaError_t e = check_code(forward, code)) return e;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  const T scale = scale_of<T>(code, n_);
+  if (path_ == Path::kRealFused) {
+    FB_CHECK(fused_->run(in, out, twa_.data(), (const C*)tab_.data(), batch, forward, forward ? scale / 2 : scale,
+                         sm_count_, s));
+    launches_ = 1;
+    return cudaSuccess;
+  }
+  const size_t len = inner_->size(), bins = n_ / 2 + 1;
+  const size_t chunk = std::min(batch, std::max<size_t>(1, kScratchTargetBytes / (len * sizeof(C))));
+  FB_CHECK(work_.reserve(chunk * len * sizeof(C)));
+  C* work = (C*)work_.data();
+  for (size_t b0 = 0; b0 < batch; b0 += chunk) {
+    const size_t nb = std::min(chunk, batch - b0);
+    if (path_ == Path::kRealHalf) {
+      if (forward) {
+        FB_CHECK(inner_->exec_device((const C*)in + b0 * m_, work, nb, kFft, s));
+        launches_ += inner_->launches();
+        untangle_kernel<T, true><<<grid_for((m_ / 2 + 1) * nb), kThreads, 0, s>>>(
+            work, (C*)out + b0 * bins, (const C*)tab_.data(), (long)m_, (long)nb, scale / 2);
+        FB_CHECK(cudaGetLastError());
+      } else {
+        untangle_kernel<T, false><<<grid_for((m_ / 2 + 1) * nb), kThreads, 0, s>>>(
+            (const C*)in + b0 * bins, work, (const C*)tab_.data(), (long)m_, (long)nb, scale);
+        FB_CHECK(cudaGetLastError());
+        FB_CHECK(inner_->exec_device(work, (C*)out + b0 * m_, nb, kUnscaledIfft, s));
+        launches_ += inner_->launches();
+      }
+      launches_ += 1;
+    } else {
+      if (forward) {
+        widen_kernel<T><<<grid_for(nb * n_), kThreads, 0, s>>>((const T*)in + b0 * n_, work, nb * n_);
+        FB_CHECK(cudaGetLastError());
+        FB_CHECK(inner_->exec_device(work, work, nb, code, s));
+        launches_ += inner_->launches();
+        copy_bins_kernel<T><<<grid_for(nb * bins), kThreads, 0, s>>>(work, (C*)out + b0 * bins, (long)n_, (long)nb);
+        FB_CHECK(cudaGetLastError());
+      } else {
+        const dim3 grid(grid_for(n_), (unsigned)std::min<size_t>(nb, 65535));
+        hermitian_kernel<T><<<grid, kThreads, 0, s>>>((const C*)in + b0 * bins, work, (long)n_, (long)nb);
+        FB_CHECK(cudaGetLastError());
+        FB_CHECK(inner_->exec_device(work, work, nb, code, s));
+        launches_ += inner_->launches();
+        real_part_kernel<T><<<grid_for(nb * n_), kThreads, 0, s>>>(work, (T*)out + b0 * n_, nb * n_);
+        FB_CHECK(cudaGetLastError());
+      }
+      launches_ += 2;
+    }
+  }
+  return cudaSuccess;
+}
+
+// Host pointers: chunks of rows go H2D into stage_in_, through exec_device into stage_out_, and D2H, one chunk at a
+// time on the plan's own stream (no pipelining: the results are those of the device path, bit for bit).
+template <typename T>
+cudaError_t RealPlan<T>::exec_host(bool forward, const void* in, void* out, size_t batch, int code) {
+  launches_ = 0;
+  if (cudaError_t e = check_code(forward, code)) return e;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
+  const size_t ib = row_bytes(forward, true), ob = row_bytes(forward, false);
+  const size_t rows = std::min(batch, std::max<size_t>(1, kHostChunkBytes / std::max(ib, ob)));
+  FB_CHECK(stage_in_.reserve(rows * ib));
+  FB_CHECK(stage_out_.reserve(rows * ob));
+  unsigned long long total = 0;
+  for (size_t b0 = 0; b0 < batch; b0 += rows) {
+    const size_t nb = std::min(rows, batch - b0);
+    FB_CHECK(cudaMemcpyAsync(stage_in_.data(), (const char*)in + b0 * ib, nb * ib, cudaMemcpyHostToDevice, host_stream_));
+    FB_CHECK(exec_device(forward, stage_in_.data(), stage_out_.data(), nb, code, host_stream_));
+    total += launches_;
+    FB_CHECK(cudaMemcpyAsync((char*)out + b0 * ob, stage_out_.data(), nb * ob, cudaMemcpyDeviceToHost, host_stream_));
+    FB_CHECK(cudaStreamSynchronize(host_stream_));
+  }
+  launches_ = total;
+  return cudaSuccess;
+}
+
+template class RealPlan<float>;
+template class RealPlan<double>;
+
+}  // namespace fb200

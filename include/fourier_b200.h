@@ -58,10 +58,12 @@ int fourier_b200_transform_batch_async_double(FB200_PLAN_D *plan, const void *in
 /* Plan introspection (Fft::size, fourier-algorithms/src/fft.rs:45, and the chosen strategy). */
 struct fourier_b200_plan_info {
   size_t size;        /* transform length N */
-  int path;           /* 0 trivial, 1 onchip, 2 twopass, 3 global_stages, 4 bluestein, 5 bluestein_fused, 6 onchip_cta, 7 threepass */
-  size_t inner_size;  /* Bluestein inner length next_pow2(2N-1) (bluesteins.rs:110), else 0 */
+  int path;           /* 0 trivial, 1 onchip, 2 twopass, 3 global_stages, 4 bluestein, 5 bluestein_fused, 6 onchip_cta, 7 threepass;
+                         real plans: 8 real_fused, 9 real_half, 10 real_full */
+  size_t inner_size;  /* Bluestein inner length next_pow2(2N-1) (bluesteins.rs:110); real plans: length of the inner
+                         complex plan (N/2 for real_half, N for real_full, 0 for real_fused); else 0 */
   int inner_path;
-  size_t n1, n2;      /* two-pass split N = n1*n2, else 0 */
+  size_t n1, n2;      /* two-pass split N = n1*n2 (real plans: that of the inner plan), else 0 */
   int precision_bytes;
   int device;
   size_t table_bytes; /* twiddle / chirp tables resident in HBM */
@@ -144,6 +146,50 @@ int fourier_b200_twiddle_rows_float(void *data_dev, size_t rows, size_t cols, un
                                     unsigned long long n_total, int forward, void *cuda_stream);
 int fourier_b200_twiddle_rows_double(void *data_dev, size_t rows, size_t cols, unsigned long long row0,
                                      unsigned long long n_total, int forward, void *cuda_stream);
+
+/* ---- Real-input transforms (numpy's rfft / irfft) ----
+ * A plan for real length N >= 1.  Forward: `batch` rows of N reals -> `batch` rows of N/2+1 complex bins, row b
+ * starting at complex element b*(N/2+1); transform Fft (0) or SqrtScaledFft (3, times 1/sqrt(N)).  Inverse: the
+ * other way round; Ifft (1) is numpy.fft.irfft(X, n=N), UnscaledIfft (2) N times that, SqrtScaledIfft (4) sqrt(N)
+ * times that.  Scales are relative to N.  The inverse ignores the imaginary part of bin 0 and, for even N, of bin
+ * N/2; the forward writes them as exactly +0.  A code of the other direction, or an unknown one, is refused with
+ * cudaErrorInvalidValue.  Out of place only: overlapping `in` and `out` are refused with cudaErrorInvalidValue.
+ * batch == 0 succeeds and launches nothing.  create returns NULL for N = 0 and without a usable device.
+ * Alignment: device base pointers must be 16-byte aligned (cudaErrorMisalignedAddress otherwise).  Spectrum rows
+ * need not be: for f32 with N a multiple of 4 (every power of two), N/2+1 is odd and every odd row starts 8 bytes
+ * off a 16-byte boundary; the kernels move the spectrum one complex value (8 bytes) at a time.
+ * The synchronous calls take host or device memory (both alike) and return when `out` is complete; host memory
+ * is staged through the plan's device buffers in chunks and gives the same bits.  The _async calls take device
+ * memory, are enqueued on `cuda_stream` and not synchronised.  Threading as for complex plans: Send, not Sync,
+ * one stream at a time. */
+struct fourier_b200_rfft_float;
+struct fourier_b200_rfft_double;
+struct fourier_b200_rfft_float *fourier_b200_rfft_create_float(size_t n);
+struct fourier_b200_rfft_double *fourier_b200_rfft_create_double(size_t n);
+void fourier_b200_rfft_destroy_float(struct fourier_b200_rfft_float *plan);
+void fourier_b200_rfft_destroy_double(struct fourier_b200_rfft_double *plan);
+int fourier_b200_rfft_forward_float(struct fourier_b200_rfft_float *plan, const float *in, void *out, size_t batch,
+                                    int transform);
+int fourier_b200_rfft_forward_double(struct fourier_b200_rfft_double *plan, const double *in, void *out,
+                                     size_t batch, int transform);
+int fourier_b200_rfft_forward_async_float(struct fourier_b200_rfft_float *plan, const float *in_dev, void *out_dev,
+                                          size_t batch, int transform, void *cuda_stream);
+int fourier_b200_rfft_forward_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev,
+                                           void *out_dev, size_t batch, int transform, void *cuda_stream);
+int fourier_b200_rfft_inverse_float(struct fourier_b200_rfft_float *plan, const void *in, float *out, size_t batch,
+                                    int transform);
+int fourier_b200_rfft_inverse_double(struct fourier_b200_rfft_double *plan, const void *in, double *out,
+                                     size_t batch, int transform);
+int fourier_b200_rfft_inverse_async_float(struct fourier_b200_rfft_float *plan, const void *in_dev, float *out_dev,
+                                          size_t batch, int transform, void *cuda_stream);
+int fourier_b200_rfft_inverse_async_double(struct fourier_b200_rfft_double *plan, const void *in_dev,
+                                           double *out_dev, size_t batch, int transform, void *cuda_stream);
+/* path 8 / 9 / 10; inner_size, inner_path, n1, n2 describe the inner complex plan; last_launches counts every
+ * kernel of the last call */
+int fourier_b200_rfft_info_float(const struct fourier_b200_rfft_float *plan, struct fourier_b200_plan_info *out);
+int fourier_b200_rfft_info_double(const struct fourier_b200_rfft_double *plan, struct fourier_b200_plan_info *out);
+const char *fourier_b200_rfft_kernel_float(const struct fourier_b200_rfft_float *plan);
+const char *fourier_b200_rfft_kernel_double(const struct fourier_b200_rfft_double *plan);
 
 const char *fourier_b200_last_error(void);
 const char *fourier_b200_version(void);
