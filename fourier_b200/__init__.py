@@ -13,6 +13,8 @@ reference's operator interface name for name:
       fourier/src/lib.rs:31-60
     (no counterpart)                                      RealFft, create_rfft_f32 / create_rfft_f64:
                                                             batched rfft / irfft of real rows
+    (no counterpart)                                      RealFft.convolve: y = irfft(rfft(x) * H) of real
+                                                            rows, one or several spectra H, one call
 
 Buffers are numpy arrays (host memory: staged over PCIe by the library) or torch CUDA tensors
 (device memory: transformed in HBM on torch's current stream).  A leading batch dimension is
@@ -200,7 +202,8 @@ def create_fft_f64(size, general=False):
 
 class RealFft:
     """A plan for real-input transforms of one length N (numpy's rfft / irfft, batched): reals of shape (..., N) and
-    spectra of shape (..., N//2+1), with equal leading dimensions.  Out of place only."""
+    spectra of shape (..., N//2+1), with equal leading dimensions.  rfft / irfft are out of place only; convolve
+    (irfft(rfft(x) * H) in one call) may run in place."""
 
     def __init__(self, size, real):
         if real not in ("f32", "f64"):
@@ -286,6 +289,36 @@ class RealFft:
             rc = getattr(L, f"fourier_b200_rfft_{direction}_{self._t}")(self._plan, pi, po, batch, code)
         if rc != 0:
             raise RuntimeError(f"real {direction} transform failed (cuda error {rc}): {_lib.last_error()}")
+
+    def convolve(self, input, spectrum, output):
+        """output = numpy.fft.irfft(numpy.fft.rfft(input) * spectrum, n=N): circular convolution of every row of
+        `input` (shape (..., N)) with the filter whose rfft is `spectrum` (shape (..., N//2+1), this plan's rfft
+        layout).  The spectrum's leading shape must equal a trailing part of the input's leading shape and is
+        broadcast over the rest: () means one filter for all rows, (C,) one per channel for input (B, C, N), the
+        input's whole leading shape one per row.  `output` has the input's shape and may be `input`
+        itself.  Correlation: pass conj(H), resolved (spectrum.conj().resolve_conj() for torch)."""
+        for x in (input, spectrum, output):
+            if _is_torch(x) and (x.is_conj() or x.is_neg()):
+                raise ValueError("torch tensors with the conj or neg bit set hold unconjugated data: "
+                                 "pass x.resolve_conj() (and resolve_neg()) instead")
+        pi, li, di, si = self._describe(input, "real")
+        ps, ls, ds, _ = self._describe(spectrum, "spec")
+        po, lo, do_, _ = self._describe(output, "real")
+        if li != lo:
+            raise ValueError(f"input and output shapes differ: {li} and {lo}")
+        if len(ls) > len(li) or tuple(li[len(li) - len(ls):]) != ls:
+            raise ValueError(f"spectrum leading shape {ls} is not a trailing part of the input's {li}")
+        if not (di == ds == do_):
+            raise ValueError("input, spectrum and output must all be host or all be device buffers")
+        batch = int(np.prod(li, dtype=np.int64))
+        rows = int(np.prod(ls, dtype=np.int64))
+        L = _lib.load()
+        if di:
+            rc = getattr(L, f"fourier_b200_convolve_real_async_{self._t}")(self._plan, pi, ps, rows, po, batch, si)
+        else:
+            rc = getattr(L, f"fourier_b200_convolve_real_{self._t}")(self._plan, pi, ps, rows, po, batch)
+        if rc != 0:
+            raise RuntimeError(f"real convolution failed (cuda error {rc}): {_lib.last_error()}")
 
     def rfft(self, input, output, transform=Transform.Fft):
         """output[..., :N//2+1] = numpy.fft.rfft(input) (Fft) or that times 1/sqrt(N) (SqrtScaledFft)."""

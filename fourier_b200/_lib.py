@@ -29,7 +29,8 @@ EXTENSION_SYMBOLS = (
        for op in ("transform_batch", "transform_batch_async", "plan_info", "create_general", "fill_input",
                   "transpose", "pack", "exchange", "fft_rows_exchange", "swap_leading", "twiddle_rows", "plan_kernel")]
     + [f"fourier_b200_rfft_{op}_{t}" for t in ("float", "double")
-       for op in ("create", "destroy", "forward", "forward_async", "inverse", "inverse_async", "info", "kernel")])
+       for op in ("create", "destroy", "forward", "forward_async", "inverse", "inverse_async", "info", "kernel")]
+    + [f"fourier_b200_convolve_real_{op}{t}" for t in ("float", "double") for op in ("", "async_")])
 
 
 def load():
@@ -78,6 +79,8 @@ def load():
         getattr(L, f"fourier_b200_rfft_info_{t}").argtypes = [vp, ctypes.POINTER(PlanInfo)]
         getattr(L, f"fourier_b200_rfft_kernel_{t}").restype = ctypes.c_char_p
         getattr(L, f"fourier_b200_rfft_kernel_{t}").argtypes = [vp]
+        getattr(L, f"fourier_b200_convolve_real_{t}").argtypes = [vp, vp, vp, sz, vp, sz]
+        getattr(L, f"fourier_b200_convolve_real_async_{t}").argtypes = [vp, vp, vp, sz, vp, sz, vp]
     L.fourier_b200_peer_alloc.argtypes = [sz, ctypes.POINTER(vp), ctypes.c_char_p]
     L.fourier_b200_peer_open.argtypes = [ctypes.c_char_p, ctypes.POINTER(vp)]
     L.fourier_b200_peer_close.argtypes = [vp]

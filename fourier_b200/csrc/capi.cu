@@ -144,10 +144,15 @@ void* create_real_plan(size_t size) {
   }
 }
 
+// the byte ranges [a, a + a_bytes) and [b, b + b_bytes) share a byte
+bool ranges_meet(const void* a, size_t a_bytes, const void* b, size_t b_bytes) {
+  const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+  return x < y + b_bytes && y < x + a_bytes;
+}
+
 // Real transforms are out of place: the byte ranges [in, in + in_bytes) and [out, out + out_bytes) must not meet.
 bool disjoint(const void* in, size_t in_bytes, const void* out, size_t out_bytes) {
-  const uintptr_t a = (uintptr_t)in, b = (uintptr_t)out;
-  if (a < b + out_bytes && b < a + in_bytes) {
+  if (ranges_meet(in, in_bytes, out, out_bytes)) {
     fb200::set_last_error("input and output overlap (real transforms are out of place only)");
     return false;
   }
@@ -179,6 +184,46 @@ int rfft_exec(void* plan, bool forward, const void* in, void* out, size_t batch,
     return (int)cudaStreamSynchronize(s);
   } catch (...) {
     fb200::set_last_error("real transform threw");
+    return (int)cudaErrorUnknown;
+  }
+}
+
+// Convolution of real rows: in == out allowed, otherwise in, out and spectrum as for rfft_exec.
+template <typename T>
+int convolve_exec(void* plan, const T* in, const void* spectrum, size_t rows, T* out, size_t batch, bool async,
+                  void* stream) {
+  if (!plan || !in || !out || !spectrum) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
+  if (rows == 0) { fb200::set_last_error("spectrum_rows must be at least 1"); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  using C = typename RealPlan<T>::C;
+  const C* spec = static_cast<const C*>(spectrum);
+  try {
+    if (batch == 0) return (int)p->convolve_device(in, spec, rows, out, 0, nullptr);
+    const size_t bytes = batch * p->size() * sizeof(T);
+    if (in != out && ranges_meet(in, bytes, out, bytes)) {
+      fb200::set_last_error("input and output overlap (they must be the same buffer or disjoint)");
+      return (int)cudaErrorInvalidValue;
+    }
+    if (ranges_meet(spectrum, p->spec_bytes(rows), out, bytes)) {
+      fb200::set_last_error("spectrum and output overlap");
+      return (int)cudaErrorInvalidValue;
+    }
+    if (!async) {
+      const bool din = is_device_pointer(in), dspec = is_device_pointer(spectrum), dout = is_device_pointer(out);
+      if (din != dout || dspec != dout) {
+        fb200::set_last_error("input, spectrum and output must all be host or all be device memory");
+        return (int)cudaErrorInvalidValue;
+      }
+      if (!din) return (int)p->convolve_host(in, spec, rows, out, batch);
+    }
+    if (!device_pointers_aligned(in, out) || !device_pointers_aligned(spectrum, spectrum))
+      return (int)cudaErrorMisalignedAddress;
+    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
+    cudaError_t e = p->convolve_device(in, spec, rows, out, batch, s);
+    if (e != cudaSuccess || async) return (int)e;
+    return (int)cudaStreamSynchronize(s);
+  } catch (...) {
+    fb200::set_last_error("convolution threw");
     return (int)cudaErrorUnknown;
   }
 }
@@ -412,6 +457,24 @@ const char* fourier_b200_rfft_kernel_float(const fourier_b200_rfft_float* plan) 
 }
 const char* fourier_b200_rfft_kernel_double(const fourier_b200_rfft_double* plan) {
   return plan ? reinterpret_cast<const RealPlan<double>*>(plan)->kernel_name() : "";
+}
+
+int fourier_b200_convolve_real_float(fourier_b200_rfft_float* plan, const float* in, const void* spectrum,
+                                     size_t spectrum_rows, float* out, size_t batch) {
+  return convolve_exec<float>(plan, in, spectrum, spectrum_rows, out, batch, false, nullptr);
+}
+int fourier_b200_convolve_real_double(fourier_b200_rfft_double* plan, const double* in, const void* spectrum,
+                                      size_t spectrum_rows, double* out, size_t batch) {
+  return convolve_exec<double>(plan, in, spectrum, spectrum_rows, out, batch, false, nullptr);
+}
+int fourier_b200_convolve_real_async_float(fourier_b200_rfft_float* plan, const float* in_dev, const void* spectrum_dev,
+                                           size_t spectrum_rows, float* out_dev, size_t batch, void* stream) {
+  return convolve_exec<float>(plan, in_dev, spectrum_dev, spectrum_rows, out_dev, batch, true, stream);
+}
+int fourier_b200_convolve_real_async_double(fourier_b200_rfft_double* plan, const double* in_dev,
+                                            const void* spectrum_dev, size_t spectrum_rows, double* out_dev,
+                                            size_t batch, void* stream) {
+  return convolve_exec<double>(plan, in_dev, spectrum_dev, spectrum_rows, out_dev, batch, true, stream);
 }
 
 const char* fourier_b200_last_error(void) { return fb200::last_error(); }

@@ -90,8 +90,19 @@ struct OnChipImpl {
     cudaError_t e;
     if ((e = cudaFuncSetAttribute(onchip::onchip_real_kernel<Cfg<true>, MINB>,
                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_fft))) return e;
-    return cudaFuncSetAttribute(onchip::onchip_real_kernel<Cfg<false>, MINB>,
+    if ((e = cudaFuncSetAttribute(onchip::onchip_real_kernel<Cfg<false>, MINB>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_fft))) return e;
+    return cudaFuncSetAttribute(onchip::onchip_conv_kernel<Cfg<true>, MINB>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_fft);
+  }
+  static cudaError_t conv(const void* in, void* out, const void* twa, const cpx<T>* tab, const cpx<T>* spec,
+                          size_t rows, size_t row0, size_t batch, T h, int sms, cudaStream_t s) {
+    const size_t groups = (batch + Cfg<true>::C - 1) / Cfg<true>::C;
+    const unsigned grid = (unsigned)std::min<size_t>(groups, (size_t)sms * MINB * 4);
+    const typename onchip::ConvBody<Cfg<true>>::Args a = {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab,
+                                                          spec, (long)rows, (long)row0, (long)batch, h};
+    onchip::onchip_conv_kernel<Cfg<true>, MINB><<<grid, Cfg<true>::THREADS, smem_fft, s>>>(a);
+    return cudaGetLastError();
   }
   static cudaError_t real(const void* in, void* out, const void* twa, const cpx<T>* tab, size_t batch, bool fwd, T h,
                           int sms, cudaStream_t s) {
@@ -109,7 +120,7 @@ struct OnChipImpl {
     return cudaGetLastError();
   }
   static const OnChipOps<T>* ops() {
-    static const RealOnChipOps<T> r = {RA, RB, &real_prepare, &real};
+    static const RealOnChipOps<T> r = {RA, RB, &real_prepare, &real, &conv};
     static const OnChipOps<T> o = {RA, RB, &prepare, &fft, kHasBluestein ? &bluestein : nullptr, &r};
     return &o;
   }

@@ -5,6 +5,7 @@
 //   * onchip_fft_kernel:      batched power-of-two FFT, N = L in {64 .. 1024}: global -> registers ->
 //                             one warp-private shared-memory exchange -> registers -> global.
 //   * onchip_real_kernel:     real-input transforms of length 2L (forward and inverse) on the same tiles.
+//   * onchip_conv_kernel:     y = irfft(rfft(x) . H) of real rows of length 2L, both transforms in one kernel.
 //   * bluestein_fused_kernel: the whole chirp-z transform of the reference (bluesteins.rs:218-259) for
 //                             N <= L, M = 2L, in one kernel and without touching HBM in between.
 //
@@ -193,6 +194,95 @@ onchip_real_kernel(const typename RealBody<Cfg>::Args a) {
       __syncwarp();
       Body::inv_phase2(f, a, grp, threadIdx.x, exch);
     }
+    __syncwarp();
+  }
+}
+
+// ---- fused convolution of real rows, y = irfft(rfft(x) . H), N = 2L (real_kernels.cuh, DESIGN.md §4.11) ----------
+// The forward phase is RealBody's: Z parked in natural order in the FFT's own exchange block.  Each lane then runs
+// real::conv_pair on the pairs it owns (k = u + TP*j, lane u = 0 also k = L/2), in place on the park.  The inverse
+// FFT of Z' runs on the same forward tile as conj(FFT(conj Z')), as bluestein_fused_kernel does: the stage-A reads
+// conjugate, and so does the store.  Row b uses spectrum row (row0 + b) mod rows.
+template <class Cfg> struct ConvBody {
+  using Tile = typename Cfg::Tile;   // FWD = true
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  using Fft = FftBody<Cfg>;
+  using Real = RealBody<Cfg>;
+  static constexpr int L = Cfg::L, TP = Tile::TP, RA = Tile::RA, RB = Tile::RB, E = Tile::E;
+  struct Args { const V* in; V* out; const TwPair<T>* twa; const V* tab; const V* spec; long rows, row0, batch; T h; };
+
+  static FB_HD void fwd_phase1(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    const typename Fft::Args fa = {a.in, nullptr, twa, a.batch, (T)1, 0};
+    Fft::phase1(f, fa, grp, t, smem, twa);
+  }
+  // untangle . H . tangle of the lane's pairs, written back into the park
+  static FB_HD void pairs(const Args& a, long grp, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const long b = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (b >= a.batch) return;
+    V* z = smem + Real::park(t);
+    const V* hs = a.spec + ((a.row0 + b) % a.rows) * (L + 1);
+#pragma unroll 4
+    for (int j = 0; j < E / 2; ++j) real::conv_pair(z, hs, (long)L, (long)(u + TP * j), a.tab, a.h);
+    if (u == 0) real::conv_pair(z, hs, (long)L, (long)(L / 2), a.tab, a.h);
+  }
+  // conj Z' from the park in stage-A input order, stage A; the scatter (which overwrites the park) comes after a
+  // __syncwarp
+  static FB_HD void inv_stage_a(Tile& f, int t, const V* smem, const TwPair<T>* twa) {
+    const int u = Tile::template u_of<true>(t);
+    const V* z = smem + Real::park(t);
+#pragma unroll
+    for (int q = 0; q < Tile::NA; ++q)
+#pragma unroll
+      for (int i = 0; i < RA; ++i) f.v[q * RA + i] = cconj(z[u + TP * q + RB * i]);
+    f.template stage_a<true>(t, twa);
+  }
+  static FB_HD void inv_scatter(const Tile& f, int t, V* smem) { f.template scatter<true, typename Cfg::Lay>(t, smem); }
+  static FB_HD void inv_store(Tile& f, const Args& a, long grp, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    f.template gather<true, typename Cfg::Lay>(t, smem);
+    f.stage_b();
+    const long b = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (b >= a.batch) return;
+    V* p = a.out + b * L;
+    static_for<0, Tile::NB>([&](auto Cc) FB_LAMBDA {
+      constexpr int c = decltype(Cc)::value;
+      static_for<0, RB>([&](auto Rr) FB_LAMBDA {
+        constexpr int r = decltype(Rr)::value;
+        p[(u + TP * c) + RA * r] = cconj(f.v[c * RB + bitrev(r, ilog2(RB))]);
+      });
+    });
+  }
+};
+
+template <class Cfg, int MINB>
+__global__ void __launch_bounds__(Cfg::THREADS, MINB)
+onchip_conv_kernel(const typename ConvBody<Cfg>::Args a) {
+  using Body = ConvBody<Cfg>;
+  using V = typename Cfg::Tile::V;
+  using T = decltype(V::x);
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  V* exch = reinterpret_cast<V*>(smem_raw);
+  TwPair<T>* twa = reinterpret_cast<TwPair<T>*>(smem_raw + Cfg::EX_BYTES);
+  for (int i = threadIdx.x; i < (Cfg::Tile::RA / 2) * Cfg::Tile::RB; i += Cfg::THREADS) twa[i] = a.twa[i];
+  __syncthreads();
+  const long groups = (a.batch + Cfg::C - 1) / Cfg::C;
+  typename Cfg::Tile f;
+  for (long grp = blockIdx.x; grp < groups; grp += gridDim.x) {
+    Body::fwd_phase1(f, a, grp, threadIdx.x, exch, twa);
+    __syncwarp();
+    Body::Real::fwd_gather(f, threadIdx.x, exch);
+    __syncwarp();
+    Body::Real::fwd_park(f, threadIdx.x, exch);
+    __syncwarp();
+    Body::pairs(a, grp, threadIdx.x, exch);
+    __syncwarp();
+    Body::inv_stage_a(f, threadIdx.x, exch, twa);
+    __syncwarp();
+    Body::inv_scatter(f, threadIdx.x, exch);
+    __syncwarp();
+    Body::inv_store(f, a, grp, threadIdx.x, exch);
     __syncwarp();
   }
 }

@@ -212,17 +212,22 @@ class Plan {
 
 // onchip.cu: the fused real-input kernels of the on-chip size class of L (onchip_lookup), N = 2L; nullptr when L has
 // none.  run(): `in` / `out` are the reals (L complex values per row) and the spectrum (L+1 per row), swapped for the
-// inverse; tab = w_N^k, k <= L/2; h = scale / 2 (forward) or scale (inverse).
+// inverse; tab = w_N^k, k <= L/2; h = scale / 2 (forward) or scale (inverse).  conv(): y = irfft(rfft(x) . H) of
+// real rows, in == out allowed; spec holds `rows` spectrum rows of L+1 bins, row b of the batch uses spectrum row
+// (row0 + b) mod rows; h = 1 / (2N).
 template <typename T> struct RealOnChipOps {
   int ra, rb;
   cudaError_t (*prepare)();
   cudaError_t (*run)(const void* in, void* out, const void* twa, const cpx<T>* tab, size_t batch, bool fwd, T h,
                      int sms, cudaStream_t);
+  cudaError_t (*conv)(const void* in, void* out, const void* twa, const cpx<T>* tab, const cpx<T>* spec, size_t rows,
+                      size_t row0, size_t batch, T h, int sms, cudaStream_t);
 };
 template <typename T> const RealOnChipOps<T>* real_onchip_lookup(size_t l);
 
 // Batched real-input transform of length N (real.cu, DESIGN.md §4.10).  Forward: `batch` rows of N reals -> rows of
 // N/2+1 complex bins (numpy's rfft layout); inverse: the other way round (numpy's irfft).  Out of place only.
+// convolve_*: both in one call with a pointwise multiply between them (DESIGN.md §4.11), in place allowed.
 template <typename T>
 class RealPlan {
  public:
@@ -242,6 +247,17 @@ class RealPlan {
   // Host pointers: staged through the plan's device buffers in chunks, the same device code; returns when `out` is done.
   cudaError_t exec_host(bool forward, const void* in, void* out, size_t batch, int code);
 
+  // Circular convolution (DESIGN.md §4.11): out[b] = irfft(rfft(in[b]) . spec[b mod rows], n = N) for `batch` rows of
+  // N reals; `spec` holds rows >= 1 spectra of N/2+1 bins in the rfft layout.  in == out allowed.  Device pointers,
+  // enqueued on `stream`, not synchronised.
+  cudaError_t convolve_device(const T* in, const C* spec, size_t rows, T* out, size_t batch, cudaStream_t stream) {
+    launches_ = 0;
+    return convolve_rows(in, spec, rows, 0, out, batch, stream);
+  }
+  // Host pointers: the spectra are staged once, the rows in chunks as in exec_host; returns when `out` is done.
+  cudaError_t convolve_host(const T* in, const C* spec, size_t rows, T* out, size_t batch);
+  size_t spec_bytes(size_t rows) const { return rows * (n_ / 2 + 1) * sizeof(C); }
+
   unsigned long long launches() const { return launches_; }
   const char* kernel_name() const { return kernel_desc_.c_str(); }
 
@@ -257,6 +273,8 @@ class RealPlan {
  private:
   RealPlan() = default;
   cudaError_t init(size_t n, int device, bool allow_fast_paths);
+  // convolve_device with row b using spectrum row (row0 + b) mod rows; adds its kernels to launches_
+  cudaError_t convolve_rows(const T* in, const C* spec, size_t rows, size_t row0, T* out, size_t batch, cudaStream_t s);
 
   size_t n_ = 0, m_ = 0;        // m_ = N/2 (even N)
   int device_ = 0;
@@ -268,6 +286,7 @@ class RealPlan {
   DeviceBuffer tab_, twa_;           // w_N^k, k <= N/4 (even N); stage twiddles of the fused kernel
   DeviceBuffer work_;                // one chunk of inner-plan rows
   DeviceBuffer stage_in_, stage_out_;
+  DeviceBuffer stage_spec_;          // the spectra of convolve_host
   cudaStream_t host_stream_ = nullptr;
   std::string kernel_desc_;
 };

@@ -6,6 +6,8 @@
 //               untangle (forward) / tangle (inverse) kernel over a plan-owned scratch chunk.
 //   kRealFull   odd N: widen to complex, complex plan of length N, first (N+1)/2 bins; the inverse extends the bins
 //               to a Hermitian spectrum, runs the complex inverse and keeps the real parts.  Correctness path only.
+// Convolution of real rows (DESIGN.md §4.11) runs on the same three paths: onchip_conv_kernel; the inner FFT,
+// conv_pair_kernel and the inner inverse, in place in `out`; widen, FFT, hermitian_mul_kernel, inverse, real part.
 #include <algorithm>
 #include <cmath>
 #include <exception>
@@ -51,6 +53,19 @@ untangle_kernel(const cpx<T>* __restrict__ in, cpx<T>* __restrict__ out, const c
   }
 }
 
+// One thread per pair (k, M-k), k <= M/2, of one row, in place on z (M complex values per row); row b uses spectrum
+// row (row0 + b) mod rows.
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+conv_pair_kernel(cpx<T>* __restrict__ z, const cpx<T>* __restrict__ spec, const cpx<T>* __restrict__ tab, long m,
+                 long batch, long rows, long row0, T h) {
+  const long pairs = m / 2 + 1, total = pairs * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / pairs, k = g - b * pairs;
+    real::conv_pair(z + b * m, spec + ((row0 + b) % rows) * (m + 1), m, k, tab, h);
+  }
+}
+
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
 widen_kernel(const T* __restrict__ in, cpx<T>* __restrict__ out, size_t count) {
@@ -76,6 +91,19 @@ hermitian_kernel(const cpx<T>* __restrict__ x, cpx<T>* __restrict__ y, long n, l
   for (long b = blockIdx.y; b < batch; b += gridDim.y)
     for (long k = blockIdx.x * (long)blockDim.x + threadIdx.x; k < n; k += (long)gridDim.x * blockDim.x)
       y[b * n + k] = real::hermitian(x + b * bins, n, k);
+}
+
+// y[k] *= s * (Hermitian extension of the spectrum row (row0 + b) mod rows)[k]; grid as hermitian_kernel
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+hermitian_mul_kernel(cpx<T>* __restrict__ y, const cpx<T>* __restrict__ spec, long n, long batch, long rows, long row0,
+                     T s) {
+  const long bins = n / 2 + 1;
+  for (long b = blockIdx.y; b < batch; b += gridDim.y) {
+    const cpx<T>* hs = spec + ((row0 + b) % rows) * bins;
+    for (long k = blockIdx.x * (long)blockDim.x + threadIdx.x; k < n; k += (long)gridDim.x * blockDim.x)
+      y[b * n + k] = cscale(cmul(y[b * n + k], real::hermitian(hs, n, k)), s);
+  }
 }
 
 template <typename T>
@@ -269,6 +297,77 @@ cudaError_t RealPlan<T>::exec_host(bool forward, const void* in, void* out, size
     FB_CHECK(cudaStreamSynchronize(host_stream_));
   }
   launches_ = total;
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::convolve_rows(const T* in, const C* spec, size_t rows, size_t row0, T* out, size_t batch,
+                                       cudaStream_t s) {
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  row0 %= rows;
+  if (path_ == Path::kRealFused) {
+    FB_CHECK(fused_->conv(in, out, twa_.data(), (const C*)tab_.data(), spec, rows, row0, batch, (T)1 / (T)(2 * n_),
+                          sm_count_, s));
+    launches_ += 1;
+    return cudaSuccess;
+  }
+  if (path_ == Path::kRealHalf) {
+    // z = x as M complex values per row: the forward, the pair step and the inverse all run in `out`
+    FB_CHECK(inner_->exec_device((const C*)in, (C*)out, batch, kFft, s));
+    launches_ += inner_->launches();
+    conv_pair_kernel<T><<<grid_for((m_ / 2 + 1) * batch), kThreads, 0, s>>>(
+        (C*)out, spec, (const C*)tab_.data(), (long)m_, (long)batch, (long)rows, (long)row0, (T)1 / (T)(2 * n_));
+    FB_CHECK(cudaGetLastError());
+    launches_ += 1;
+    FB_CHECK(inner_->exec_device((C*)out, (C*)out, batch, kUnscaledIfft, s));
+    launches_ += inner_->launches();
+    return cudaSuccess;
+  }
+  const size_t chunk = std::min(batch, std::max<size_t>(1, kScratchTargetBytes / (n_ * sizeof(C))));
+  FB_CHECK(work_.reserve(chunk * n_ * sizeof(C)));
+  C* work = (C*)work_.data();
+  for (size_t b0 = 0; b0 < batch; b0 += chunk) {
+    const size_t nb = std::min(chunk, batch - b0);
+    widen_kernel<T><<<grid_for(nb * n_), kThreads, 0, s>>>(in + b0 * n_, work, nb * n_);
+    FB_CHECK(cudaGetLastError());
+    FB_CHECK(inner_->exec_device(work, work, nb, kFft, s));
+    launches_ += inner_->launches();
+    const dim3 grid(grid_for(n_), (unsigned)std::min<size_t>(nb, 65535));
+    hermitian_mul_kernel<T><<<grid, kThreads, 0, s>>>(work, spec, (long)n_, (long)nb, (long)rows,
+                                                      (long)((row0 + b0) % rows), (T)1 / (T)n_);
+    FB_CHECK(cudaGetLastError());
+    FB_CHECK(inner_->exec_device(work, work, nb, kUnscaledIfft, s));
+    launches_ += inner_->launches();
+    real_part_kernel<T><<<grid_for(nb * n_), kThreads, 0, s>>>(work, out + b0 * n_, nb * n_);
+    FB_CHECK(cudaGetLastError());
+    launches_ += 3;
+  }
+  return cudaSuccess;
+}
+
+// Host pointers: the spectra go H2D once into stage_spec_; chunks of rows then go through convolve_rows as in
+// exec_host, each chunk starting at its own spectrum row, so the bits are those of one device call.
+template <typename T>
+cudaError_t RealPlan<T>::convolve_host(const T* in, const C* spec, size_t rows, T* out, size_t batch) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
+  const size_t rb = n_ * sizeof(T);
+  const size_t nrows = std::min(batch, std::max<size_t>(1, kHostChunkBytes / rb));
+  FB_CHECK(stage_spec_.reserve(spec_bytes(rows)));
+  FB_CHECK(stage_in_.reserve(nrows * rb));
+  FB_CHECK(stage_out_.reserve(nrows * rb));
+  FB_CHECK(cudaMemcpyAsync(stage_spec_.data(), spec, spec_bytes(rows), cudaMemcpyHostToDevice, host_stream_));
+  for (size_t b0 = 0; b0 < batch; b0 += nrows) {
+    const size_t nb = std::min(nrows, batch - b0);
+    FB_CHECK(cudaMemcpyAsync(stage_in_.data(), (const char*)in + b0 * rb, nb * rb, cudaMemcpyHostToDevice, host_stream_));
+    FB_CHECK(convolve_rows((const T*)stage_in_.data(), (const C*)stage_spec_.data(), rows, b0, (T*)stage_out_.data(), nb,
+                           host_stream_));
+    FB_CHECK(cudaMemcpyAsync((char*)out + b0 * rb, stage_out_.data(), nb * rb, cudaMemcpyDeviceToHost, host_stream_));
+    FB_CHECK(cudaStreamSynchronize(host_stream_));
+  }
   return cudaSuccess;
 }
 

@@ -191,6 +191,32 @@ int fourier_b200_rfft_info_double(const struct fourier_b200_rfft_double *plan, s
 const char *fourier_b200_rfft_kernel_float(const struct fourier_b200_rfft_float *plan);
 const char *fourier_b200_rfft_kernel_double(const struct fourier_b200_rfft_double *plan);
 
+/* ---- Convolution of real rows, y = irfft(rfft(x) . H) ----
+ * On a real plan of length N: out[b] = numpy.fft.irfft(numpy.fft.rfft(in[b]) * H[b mod F], n=N) for `batch` rows of
+ * N reals, where `spectrum` holds F = spectrum_rows >= 1 rows of N/2+1 complex bins in exactly the layout the plan's
+ * rfft writes (row f starting at complex element f*(N/2+1)).  With H = rfft(h) this is the circular convolution
+ * out[b][n] = sum_m in[b][m] h[(n-m) mod N]; F = 1 applies one filter to every row, F = C one filter per channel of
+ * rows ordered (batch, channel), F = batch one per row.  Correlation is the same call with conj(H).  The imaginary
+ * parts of the products at bin 0 and, for even N, bin N/2 are ignored, as irfft ignores them.  Linear convolution:
+ * zero-pad x and h to N >= len(x) + len(h) - 1.  One launch on the real_fused path, 2 x (inner plan) + 1 on
+ * real_half, 3 + 2 x (inner plan) per scratch chunk on real_full; last_launches of the info call reports it.
+ * `in` and `out` must be the same buffer (in place) or disjoint, and `spectrum` must not overlap `out`
+ * (cudaErrorInvalidValue otherwise); a NULL argument or spectrum_rows == 0 is refused with cudaErrorInvalidValue.
+ * batch == 0 succeeds and launches nothing.  Device pointers must be 16-byte aligned (cudaErrorMisalignedAddress).
+ * The synchronous calls take all three buffers as host memory or all three as device memory (a mix is refused with
+ * cudaErrorInvalidValue) and return when `out` is complete; host memory gives the same bits.  The _async calls take
+ * device memory, are enqueued on `cuda_stream` and not synchronised.  Threading as for the plan: Send, not Sync. */
+int fourier_b200_convolve_real_float(struct fourier_b200_rfft_float *plan, const float *in, const void *spectrum,
+                                     size_t spectrum_rows, float *out, size_t batch);
+int fourier_b200_convolve_real_double(struct fourier_b200_rfft_double *plan, const double *in, const void *spectrum,
+                                      size_t spectrum_rows, double *out, size_t batch);
+int fourier_b200_convolve_real_async_float(struct fourier_b200_rfft_float *plan, const float *in_dev,
+                                           const void *spectrum_dev, size_t spectrum_rows, float *out_dev,
+                                           size_t batch, void *cuda_stream);
+int fourier_b200_convolve_real_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev,
+                                            const void *spectrum_dev, size_t spectrum_rows, double *out_dev,
+                                            size_t batch, void *cuda_stream);
+
 const char *fourier_b200_last_error(void);
 const char *fourier_b200_version(void);
 
