@@ -17,15 +17,6 @@
 
 namespace fb200 {
 
-#define FB_CHECK(expr)                                                                       \
-  do {                                                                                       \
-    cudaError_t _e = (expr);                                                                 \
-    if (_e != cudaSuccess) {                                                                 \
-      set_last_error(std::string(#expr) + ": " + cudaGetErrorString(_e));                    \
-      return _e;                                                                             \
-    }                                                                                        \
-  } while (0)
-
 namespace {
 
 template <typename T> struct ColumnOps {
@@ -140,7 +131,7 @@ cudaError_t Plan<T>::init_bigpow2() {
   if (!inner_ || inner_->path() != Path::kTwoPass) { inner_.reset(); return cudaErrorNotSupported; }
   n1_ = (size_t)1 << a;
   n2_ = (size_t)1 << (k - a);
-  FB_CHECK((twopass::upload_vec<T, TwPair<T>>(tw_a_, twopass::make_twa<T>(col->ra, col->rb))));
+  FB_CHECK(upload(tw_a_, twopass::make_twa<T>(col->ra, col->rb)));
   fast_ops_ = col;
   return cudaSuccess;
 }
@@ -149,9 +140,7 @@ template <typename T>
 cudaError_t Plan<T>::exec_bigpow2(const C* in, C* out, size_t batch, int code, cudaStream_t s) {
   const auto* col = static_cast<const ColumnOps<T>*>(fast_ops_);   // nullptr with an outer radix-3 pass
   const bool fwd = transform_is_forward(code);
-  T scale = (T)1;
-  if (code == kIfft) scale = (T)1 / (T)n_;
-  else if (code == kSqrtScaledFft || code == kSqrtScaledIfft) scale = (T)1 / std::sqrt((T)n_);
+  const T scale = scale_for<T>(code, n_);
   // the intermediate A[ka][nb] of a few transforms at a time (at most 2 GB of scratch, at least one transform)
   const size_t chunk = std::min(batch, std::max<size_t>(1, ((size_t)2 << 30) / (n_ * sizeof(C))));
   // the row kernel works on whole tiles of up to 32 rows: 3 / 9 / 27 rows per transform are padded up (the padding rows

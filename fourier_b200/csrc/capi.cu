@@ -10,6 +10,7 @@
 #pragma GCC visibility pop
 
 #include <cstdint>
+#include <initializer_list>
 #include <new>
 
 #include "plan.h"
@@ -38,6 +39,19 @@ bool is_device_pointer(const void* p) {
   return attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged;
 }
 
+// Where the buffers of a synchronous call live: 1 all in device memory, 0 all in host memory, -1 a mix, which is
+// refused (last_error set to `mix`).
+int residence(std::initializer_list<const void*> bufs,
+              const char* mix = "input and output must both be host or both be device memory") {
+  const bool dev = is_device_pointer(*bufs.begin());
+  for (auto p = bufs.begin() + 1; p != bufs.end(); ++p)
+    if (is_device_pointer(*p) != dev) {
+      fb200::set_last_error(mix);
+      return -1;
+    }
+  return dev ? 1 : 0;
+}
+
 // The kernels read and write device buffers with 16-byte vector accesses (cpx<double> as double2, f32 pairs as
 // float4, TMA tensor maps on the input): a misaligned device pointer would fault and poison the CUDA context, so it
 // is refused up front.  (cudaMalloc and torch allocations are 256/512-byte aligned; a slice starting at an odd f32
@@ -50,51 +64,39 @@ bool device_pointers_aligned(const void* in, const void* out) {
   return true;
 }
 
-template <typename T>
-void* create_plan(size_t size, bool fast) {
+// Plan<T> or RealPlan<T> on the calling thread's device
+template <class P>
+void* create(size_t size, bool fast) {
   const int dev = resolve_device();
   if (dev < 0) {
     fb200::set_last_error("no usable CUDA device (libfourier.so has no CPU fallback)");
     return nullptr;
   }
   try {
-    return Plan<T>::create(size, dev, fast);
+    return P::create(size, dev, fast);
   } catch (...) {
     fb200::set_last_error("plan construction threw");
     return nullptr;
   }
 }
 
+// async: device pointers on `stream`, not synchronised; otherwise host or device pointers, synchronised.
 template <typename T>
-int transform_batch(const void* plan, const void* in, void* out, size_t batch, int code) {
+int fft_exec(const void* plan, const void* in, void* out, size_t batch, int code, bool async, void* stream) {
   if (!plan || !in || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
   auto* p = const_cast<Plan<T>*>(static_cast<const Plan<T>*>(plan));
   using C = typename Plan<T>::C;
   try {
-    const bool din = is_device_pointer(in), dout = is_device_pointer(out);
-    if (din != dout) {
-      fb200::set_last_error("input and output must both be host or both be device memory");
-      return (int)cudaErrorInvalidValue;
+    if (!async) {
+      const int dev = residence({in, out});
+      if (dev < 0) return (int)cudaErrorInvalidValue;
+      if (!dev) return (int)p->exec_host((const C*)in, (C*)out, batch, code);
     }
-    if (!din) return (int)p->exec_host((const C*)in, (C*)out, batch, code);
     if (!device_pointers_aligned(in, out)) return (int)cudaErrorMisalignedAddress;
-    cudaError_t e = p->exec_device((const C*)in, (C*)out, batch, code, cudaStreamPerThread);
-    if (e != cudaSuccess) return (int)e;
-    return (int)cudaStreamSynchronize(cudaStreamPerThread);
-  } catch (...) {
-    fb200::set_last_error("transform threw");
-    return (int)cudaErrorUnknown;
-  }
-}
-
-template <typename T>
-int transform_async(const void* plan, const void* in, void* out, size_t batch, int code, void* stream) {
-  if (!plan || !in || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
-  auto* p = const_cast<Plan<T>*>(static_cast<const Plan<T>*>(plan));
-  using C = typename Plan<T>::C;
-  try {
-    if (!device_pointers_aligned(in, out)) return (int)cudaErrorMisalignedAddress;
-    return (int)p->exec_device((const C*)in, (C*)out, batch, code, (cudaStream_t)stream);
+    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
+    cudaError_t e = p->exec_device((const C*)in, (C*)out, batch, code, s);
+    if (e != cudaSuccess || async) return (int)e;
+    return (int)cudaStreamSynchronize(s);
   } catch (...) {
     fb200::set_last_error("transform threw");
     return (int)cudaErrorUnknown;
@@ -118,30 +120,16 @@ int rows_exchange(const void* plan, const void* in, size_t rows, int forward, vo
   }
 }
 
-template <typename T>
+// Plan<T> or RealPlan<T>
+template <class P>
 int plan_info(const void* plan, fourier_b200_plan_info* out) {
-  if (!plan || !out) return (int)cudaErrorInvalidValue;
-  const auto* p = static_cast<const Plan<T>*>(plan);
+  if (!plan || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
+  const auto* p = static_cast<const P*>(plan);
   const fb200::PlanInfo i = p->info();
   out->size = i.size; out->path = i.path; out->inner_size = i.inner_size; out->inner_path = i.inner_path;
   out->n1 = i.n1; out->n2 = i.n2; out->precision_bytes = i.precision_bytes; out->device = i.device;
   out->table_bytes = i.table_bytes; out->last_launches = p->launches();
   return 0;
-}
-
-template <typename T>
-void* create_real_plan(size_t size) {
-  const int dev = resolve_device();
-  if (dev < 0) {
-    fb200::set_last_error("no usable CUDA device (libfourier.so has no CPU fallback)");
-    return nullptr;
-  }
-  try {
-    return RealPlan<T>::create(size, dev);
-  } catch (...) {
-    fb200::set_last_error("plan construction threw");
-    return nullptr;
-  }
 }
 
 // the byte ranges [a, a + a_bytes) and [b, b + b_bytes) share a byte
@@ -170,12 +158,9 @@ int rfft_exec(void* plan, bool forward, const void* in, void* out, size_t batch,
     if (!disjoint(in, batch * p->row_bytes(forward, true), out, batch * p->row_bytes(forward, false)))
       return (int)cudaErrorInvalidValue;
     if (!async) {
-      const bool din = is_device_pointer(in), dout = is_device_pointer(out);
-      if (din != dout) {
-        fb200::set_last_error("input and output must both be host or both be device memory");
-        return (int)cudaErrorInvalidValue;
-      }
-      if (!din) return (int)p->exec_host(forward, in, out, batch, code);
+      const int dev = residence({in, out});
+      if (dev < 0) return (int)cudaErrorInvalidValue;
+      if (!dev) return (int)p->exec_host(forward, in, out, batch, code);
     }
     if (!device_pointers_aligned(in, out)) return (int)cudaErrorMisalignedAddress;
     cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
@@ -209,12 +194,10 @@ int convolve_exec(void* plan, const T* in, const void* spectrum, size_t rows, T*
       return (int)cudaErrorInvalidValue;
     }
     if (!async) {
-      const bool din = is_device_pointer(in), dspec = is_device_pointer(spectrum), dout = is_device_pointer(out);
-      if (din != dout || dspec != dout) {
-        fb200::set_last_error("input, spectrum and output must all be host or all be device memory");
-        return (int)cudaErrorInvalidValue;
-      }
-      if (!din) return (int)p->convolve_host(in, spec, rows, out, batch);
+      const int dev =
+          residence({in, spectrum, out}, "input, spectrum and output must all be host or all be device memory");
+      if (dev < 0) return (int)cudaErrorInvalidValue;
+      if (!dev) return (int)p->convolve_host(in, spec, rows, out, batch);
     }
     if (!device_pointers_aligned(in, out) || !device_pointers_aligned(spectrum, spectrum))
       return (int)cudaErrorMisalignedAddress;
@@ -228,17 +211,6 @@ int convolve_exec(void* plan, const T* in, const void* spectrum, size_t rows, T*
   }
 }
 
-template <typename T>
-int rfft_info(const void* plan, fourier_b200_plan_info* out) {
-  if (!plan || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
-  const auto* p = static_cast<const RealPlan<T>*>(plan);
-  const fb200::PlanInfo i = p->info();
-  out->size = i.size; out->path = i.path; out->inner_size = i.inner_size; out->inner_path = i.inner_path;
-  out->n1 = i.n1; out->n2 = i.n2; out->precision_bytes = i.precision_bytes; out->device = i.device;
-  out->table_bytes = i.table_bytes; out->last_launches = p->launches();
-  return 0;
-}
-
 }  // namespace
 
 using fourier::c::fourier_fft_double;
@@ -250,10 +222,10 @@ extern "C" {
 
 // ---- the eight reference symbols --------------------------------------------------------------------
 fourier_fft_float* fourier_create_float(size_t size) {
-  return static_cast<fourier_fft_float*>(create_plan<float>(size, true));
+  return static_cast<fourier_fft_float*>(create<Plan<float>>(size, true));
 }
 fourier_fft_double* fourier_create_double(size_t size) {
-  return static_cast<fourier_fft_double*>(create_plan<double>(size, true));
+  return static_cast<fourier_fft_double*>(create<Plan<double>>(size, true));
 }
 void fourier_destroy_float(fourier_fft_float* plan) {
   try { delete reinterpret_cast<Plan<float>*>(plan); } catch (...) {}
@@ -262,18 +234,18 @@ void fourier_destroy_double(fourier_fft_double* plan) {
   try { delete reinterpret_cast<Plan<double>*>(plan); } catch (...) {}
 }
 void fourier_transform_in_place_float(const fourier_fft_float* plan, std::complex<float>* data, int t) {
-  (void)transform_batch<float>(plan, data, data, 1, t);
+  (void)fft_exec<float>(plan, data, data, 1, t, false, nullptr);
 }
 void fourier_transform_in_place_double(const fourier_fft_double* plan, std::complex<double>* data, int t) {
-  (void)transform_batch<double>(plan, data, data, 1, t);
+  (void)fft_exec<double>(plan, data, data, 1, t, false, nullptr);
 }
 void fourier_transform_float(const fourier_fft_float* plan, const std::complex<float>* in,
                              std::complex<float>* out, int t) {
-  (void)transform_batch<float>(plan, in, out, 1, t);
+  (void)fft_exec<float>(plan, in, out, 1, t, false, nullptr);
 }
 void fourier_transform_double(const fourier_fft_double* plan, const std::complex<double>* in,
                               std::complex<double>* out, int t) {
-  (void)transform_batch<double>(plan, in, out, 1, t);
+  (void)fft_exec<double>(plan, in, out, 1, t, false, nullptr);
 }
 
 }  // extern "C"
@@ -301,26 +273,26 @@ int fourier_b200_device_count(void) {
 
 int fourier_b200_transform_batch_float(const fourier_fft_float* plan, const void* in, void* out,
                                        size_t batch, int t) {
-  return transform_batch<float>(plan, in, out, batch, t);
+  return fft_exec<float>(plan, in, out, batch, t, false, nullptr);
 }
 int fourier_b200_transform_batch_double(const fourier_fft_double* plan, const void* in, void* out,
                                         size_t batch, int t) {
-  return transform_batch<double>(plan, in, out, batch, t);
+  return fft_exec<double>(plan, in, out, batch, t, false, nullptr);
 }
 int fourier_b200_transform_batch_async_float(const fourier_fft_float* plan, const void* in, void* out,
                                              size_t batch, int t, void* stream) {
-  return transform_async<float>(plan, in, out, batch, t, stream);
+  return fft_exec<float>(plan, in, out, batch, t, true, stream);
 }
 int fourier_b200_transform_batch_async_double(const fourier_fft_double* plan, const void* in, void* out,
                                               size_t batch, int t, void* stream) {
-  return transform_async<double>(plan, in, out, batch, t, stream);
+  return fft_exec<double>(plan, in, out, batch, t, true, stream);
 }
 
 int fourier_b200_plan_info_float(const fourier_fft_float* plan, fourier_b200_plan_info* out) {
-  return plan_info<float>(plan, out);
+  return plan_info<Plan<float>>(plan, out);
 }
 int fourier_b200_plan_info_double(const fourier_fft_double* plan, fourier_b200_plan_info* out) {
-  return plan_info<double>(plan, out);
+  return plan_info<Plan<double>>(plan, out);
 }
 const char* fourier_b200_path_name(int path) { return fb200::path_name((fb200::Path)path); }
 const char* fourier_b200_plan_kernel_float(const fourier_fft_float* plan) {
@@ -331,10 +303,10 @@ const char* fourier_b200_plan_kernel_double(const fourier_fft_double* plan) {
 }
 
 fourier_fft_float* fourier_b200_create_general_float(size_t size) {
-  return static_cast<fourier_fft_float*>(create_plan<float>(size, false));
+  return static_cast<fourier_fft_float*>(create<Plan<float>>(size, false));
 }
 fourier_fft_double* fourier_b200_create_general_double(size_t size) {
-  return static_cast<fourier_fft_double*>(create_plan<double>(size, false));
+  return static_cast<fourier_fft_double*>(create<Plan<double>>(size, false));
 }
 
 int fourier_b200_fill_input_float(void* dev_out, unsigned long long first, size_t count,
@@ -407,10 +379,10 @@ int fourier_b200_twiddle_rows_double(void* data, size_t rows, size_t cols, unsig
 
 // ---- real-input transforms ------------------------------------------------------------------------------
 fourier_b200_rfft_float* fourier_b200_rfft_create_float(size_t n) {
-  return static_cast<fourier_b200_rfft_float*>(create_real_plan<float>(n));
+  return static_cast<fourier_b200_rfft_float*>(create<RealPlan<float>>(n, true));
 }
 fourier_b200_rfft_double* fourier_b200_rfft_create_double(size_t n) {
-  return static_cast<fourier_b200_rfft_double*>(create_real_plan<double>(n));
+  return static_cast<fourier_b200_rfft_double*>(create<RealPlan<double>>(n, true));
 }
 void fourier_b200_rfft_destroy_float(fourier_b200_rfft_float* plan) {
   try { delete reinterpret_cast<RealPlan<float>*>(plan); } catch (...) {}
@@ -447,10 +419,10 @@ int fourier_b200_rfft_inverse_async_double(fourier_b200_rfft_double* plan, const
   return rfft_exec<double>(plan, false, in, out, batch, t, true, stream);
 }
 int fourier_b200_rfft_info_float(const fourier_b200_rfft_float* plan, fourier_b200_plan_info* out) {
-  return rfft_info<float>(plan, out);
+  return plan_info<RealPlan<float>>(plan, out);
 }
 int fourier_b200_rfft_info_double(const fourier_b200_rfft_double* plan, fourier_b200_plan_info* out) {
-  return rfft_info<double>(plan, out);
+  return plan_info<RealPlan<double>>(plan, out);
 }
 const char* fourier_b200_rfft_kernel_float(const fourier_b200_rfft_float* plan) {
   return plan ? reinterpret_cast<const RealPlan<float>*>(plan)->kernel_name() : "";

@@ -13,15 +13,6 @@
 
 namespace fb200 {
 
-#define FB_CHECK(expr)                                                                       \
-  do {                                                                                       \
-    cudaError_t _e = (expr);                                                                 \
-    if (_e != cudaSuccess) {                                                                 \
-      set_last_error(std::string(#expr) + ": " + cudaGetErrorString(_e));                    \
-      return _e;                                                                             \
-    }                                                                                        \
-  } while (0)
-
 namespace {
 
 using onchip::OnChipCfg;
@@ -152,20 +143,6 @@ template <> const OnChipOps<double>* onchip_lookup<double>(size_t l) {
   }
 }
 
-template <typename T, typename U>
-cudaError_t upload_vec(DeviceBuffer& buf, const std::vector<U>& host) {
-  cudaError_t e = buf.reserve(host.size() * sizeof(U));
-  if (e != cudaSuccess) return e;
-  return cudaMemcpy(buf.data(), host.data(), host.size() * sizeof(U), cudaMemcpyHostToDevice);
-}
-
-int sm_count() {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms;
-}
-
 }  // namespace
 
 template <typename T>
@@ -173,9 +150,9 @@ cudaError_t Plan<T>::init_onchip() {
   const OnChipOps<T>* ops = onchip_lookup<T>(n_);
   if (!ops) return cudaErrorNotSupported;
   FB_CHECK(ops->prepare());
-  FB_CHECK((upload_vec<T, TwPair<T>>(tw_a_, twopass::make_twa<T>(ops->ra, ops->rb))));
+  FB_CHECK(upload(tw_a_, twopass::make_twa<T>(ops->ra, ops->rb)));
   fast_ops_ = ops;
-  sm_count_ = sm_count();
+  sm_count_ = sm_count(device_);
   return cudaSuccess;
 }
 
@@ -183,11 +160,8 @@ template <typename T>
 cudaError_t Plan<T>::exec_onchip(const C* in, C* out, size_t batch, int code, cudaStream_t s) {
   const auto* ops = static_cast<const OnChipOps<T>*>(fast_ops_);
   const bool fwd = transform_is_forward(code);
-  const bool do_scale = !(code == kFft || code == kUnscaledIfft);
-  T scale = (T)1;
-  if (code == kIfft) scale = (T)1 / (T)n_;
-  else if (do_scale) scale = (T)1 / std::sqrt((T)n_);
-  FB_CHECK(ops->fft(in, out, tw_a_.data(), batch, fwd, scale, do_scale, sm_count_, s));
+  const bool do_scale = code != kFft && code != kUnscaledIfft;
+  FB_CHECK(ops->fft(in, out, tw_a_.data(), batch, fwd, scale_for<T>(code, n_), do_scale, sm_count_, s));
   launches_ += 1;
   return cudaSuccess;
 }
@@ -201,7 +175,7 @@ cudaError_t Plan<T>::init_bluestein_fused(const std::vector<double>& chirp_re, c
   const OnChipOps<T>* ops = onchip_lookup<T>(l);
   if (!ops || !ops->bluestein) return cudaErrorNotSupported;
   FB_CHECK(ops->prepare());
-  FB_CHECK((upload_vec<T, TwPair<T>>(tw_a_, twopass::make_twa<T>(ops->ra, ops->rb))));
+  FB_CHECK(upload(tw_a_, twopass::make_twa<T>(ops->ra, ops->rb)));
   // layout per direction d (0 forward, 1 inverse): [chirp | wm | wce | wco], L entries each
   std::vector<cpx<T>> tab(2 * 4 * l, mk<T>((T)0, (T)0));
   for (int d = 0; d < 2; ++d) {
@@ -216,9 +190,9 @@ cudaError_t Plan<T>::init_bluestein_fused(const std::vector<double>& chirp_re, c
       t[3 * l + i] = mk<T>((T)w_re[2 * i + 1], (T)(-sgn * w_im[2 * i + 1]));  // conj(W_dir[2k+1])
     }
   }
-  FB_CHECK((upload_vec<T, cpx<T>>(tbase_, tab)));
+  FB_CHECK(upload(tbase_, tab));
   fast_ops_ = ops;
-  sm_count_ = sm_count();
+  sm_count_ = sm_count(device_);
   return cudaSuccess;
 }
 
@@ -226,10 +200,7 @@ template <typename T>
 cudaError_t Plan<T>::exec_bluestein_fused(const C* in, C* out, size_t batch, int code, cudaStream_t s) {
   const auto* ops = static_cast<const OnChipOps<T>*>(fast_ops_);
   const bool fwd = transform_is_forward(code);
-  T scale = (T)1;
-  if (code == kIfft) scale = (T)1 / (T)n_;
-  else if (code == kSqrtScaledFft || code == kSqrtScaledIfft) scale = (T)1 / std::sqrt((T)n_);
-  scale /= (T)m_;
+  const T scale = scale_for<T>(code, n_) / (T)m_;
   const size_t l = m_ / 2;
   const C* t = (const C*)tbase_.data() + (fwd ? 0 : 4 * l);
   FB_CHECK(ops->bluestein(in, out, tw_a_.data(), t, t + l, t + 2 * l, t + 3 * l, n_, batch, scale, sm_count_, s));

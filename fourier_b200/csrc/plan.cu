@@ -12,7 +12,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <exception>
 
 namespace fb200 {
 
@@ -22,15 +21,6 @@ namespace fb200 {
 static thread_local std::string g_last_error;
 void set_last_error(const std::string& s) { g_last_error = s; }
 const char* last_error() { return g_last_error.c_str(); }
-
-#define FB_CHECK(expr)                                                                       \
-  do {                                                                                       \
-    cudaError_t _e = (expr);                                                                 \
-    if (_e != cudaSuccess) {                                                                 \
-      set_last_error(std::string(#expr) + ": " + cudaGetErrorString(_e));                    \
-      return _e;                                                                             \
-    }                                                                                        \
-  } while (0)
 
 const char* path_name(Path p) {
   switch (p) {
@@ -82,24 +72,6 @@ cudaError_t DeviceBuffer::reserve(size_t bytes) {
 
 namespace {
 
-template <typename T>
-cudaError_t upload(DeviceBuffer& buf, const std::vector<cpx<T>>& host) {
-  cudaError_t e = buf.reserve(std::max<size_t>(host.size(), 1) * sizeof(cpx<T>));
-  if (e != cudaSuccess) return e;
-  if (host.empty()) return cudaSuccess;
-  return cudaMemcpy(buf.data(), host.data(), host.size() * sizeof(cpx<T>), cudaMemcpyHostToDevice);
-}
-
-// Scale factor of a Transform code for length n (autosort/mod.rs:381-385, bluesteins.rs:240-258).
-template <typename T> T scale_for(int code, size_t n) {
-  switch (code) {
-    case kIfft: return (T)1 / (T)n;
-    case kSqrtScaledFft:
-    case kSqrtScaledIfft: return (T)1 / std::sqrt((T)n);
-    default: return (T)1;
-  }
-}
-
 constexpr size_t kHostSmallBytes = (size_t)1 << 20;        // below this a host call takes the single-stream latency path
 constexpr size_t kHostZeroCopyBytes = (size_t)64 << 10;    // below this the kernel reads / writes mapped host memory itself
 
@@ -108,27 +80,6 @@ constexpr size_t kHostZeroCopyBytes = (size_t)64 << 10;    // below this the ker
 // ---------------------------------------------------------------------------------------------------
 // construction
 // ---------------------------------------------------------------------------------------------------
-template <typename T>
-Plan<T>* Plan<T>::create(size_t n, int device, bool allow_fast_paths) {
-  if (n == 0) {
-    set_last_error("size 0 is not a valid transform length");
-    return nullptr;
-  }
-  Plan<T>* p = new (std::nothrow) Plan<T>();
-  if (!p) return nullptr;
-  cudaError_t e = cudaErrorUnknown;
-  try {
-    e = p->init(n, device, allow_fast_paths);
-  } catch (const std::exception& ex) {   // e.g. bad_alloc while building an N-entry host table
-    set_last_error(std::string("plan construction threw: ") + ex.what());
-  }
-  if (e != cudaSuccess) {
-    delete p;
-    return nullptr;
-  }
-  return p;
-}
-
 template <typename T>
 const char* Plan<T>::kernel_name() const {
   switch (path_) {
@@ -210,7 +161,7 @@ cudaError_t Plan<T>::init_global_stages() {
     host_twiddle(k, n_, &re, &im);
     w[k] = mk<T>((T)re, (T)im);
   }
-  FB_CHECK(upload<T>(wtab_, w));
+  FB_CHECK(upload(wtab_, w));
   return cudaSuccess;
 }
 
@@ -244,16 +195,16 @@ cudaError_t Plan<T>::init_bluestein(bool allow_fast_paths) {
   }
   if (allow_fast_paths && init_cta(m_) == cudaSuccess) {
     // inner size above the warp-level kernel: the CTA-level kernel in chirp mode, still one launch
-    FB_CHECK(upload<T>(chirp_, chirp));
-    FB_CHECK(upload<T>(wf_, wf));
+    FB_CHECK(upload(chirp_, chirp));
+    FB_CHECK(upload(wf_, wf));
     cta_chirp_ = true;
     path_ = Path::kBluesteinFused;
     return cudaSuccess;
   }
   inner_.reset(Plan<T>::create(m_, device_, allow_fast_paths));
   if (!inner_) return cudaErrorUnknown;
-  FB_CHECK(upload<T>(chirp_, chirp));
-  FB_CHECK(upload<T>(wf_, wf));
+  FB_CHECK(upload(chirp_, chirp));
+  FB_CHECK(upload(wf_, wf));
   path_ = Path::kBluestein;
   return cudaSuccess;
 }

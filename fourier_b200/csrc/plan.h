@@ -9,9 +9,13 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
+#include <cmath>
 #include <cstddef>
+#include <exception>
 #include <memory>
+#include <new>
 #include <string>
 #include <vector>
 
@@ -48,6 +52,45 @@ constexpr int kMaxPeers = 16;   // ranks of one box (peer-memory exchange, excha
 bool is_23_smooth(size_t n);
 size_t bluestein_inner_size(size_t n);  // bluesteins.rs:110
 
+// thread-local error text for the C ABI
+void set_last_error(const std::string& s);
+const char* last_error();
+
+// Returns the error of a failing CUDA call from the enclosing function, with last_error set to the call and its text.
+#define FB_CHECK(expr)                                                                       \
+  do {                                                                                       \
+    cudaError_t _e = (expr);                                                                 \
+    if (_e != cudaSuccess) {                                                                 \
+      set_last_error(std::string(#expr) + ": " + cudaGetErrorString(_e));                    \
+      return _e;                                                                             \
+    }                                                                                        \
+  } while (0)
+
+// Scale factor of a Transform code for length n (autosort/mod.rs:381-385, bluesteins.rs:240-258).
+template <typename T> T scale_for(int code, size_t n) {
+  switch (code) {
+    case kIfft: return (T)1 / (T)n;
+    case kSqrtScaledFft:
+    case kSqrtScaledIfft: return (T)1 / std::sqrt((T)n);
+    default: return (T)1;
+  }
+}
+
+// Multiprocessor count of `device`; 132 (H100 SXM) when the query fails.
+inline int sm_count(int device) {
+  int sms = 132;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) sms = 132;
+  return sms;
+}
+
+// Grid of the grid-stride kernels (stockham_generic.cu, real.cu): kThreads per CTA, one thread per element up to
+// 32 CTAs per SM of a 132-SM H100, grid-stride beyond.
+constexpr int kThreads = 256;
+inline unsigned grid_for(size_t total) {
+  const size_t blocks = (total + kThreads - 1) / kThreads;
+  return (unsigned)std::max<size_t>(1, std::min<size_t>(blocks, 132u * 32u));
+}
+
 // Makes `dev` the current device for the lifetime of the guard.
 struct DeviceGuard {
   int prev = -1;
@@ -63,15 +106,19 @@ struct DeviceGuard {
 };
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is a per-device setting: done once per kernel AND device (a process
-// may hold plans on several GPUs).  `done` is the kernel's own bit mask of prepared devices.
+// may hold plans on several GPUs).  `done` is the kernel's own bit mask of prepared devices.  carveout >= 0 also sets
+// the kernel's preferred shared-memory carveout (percent, or a cudaSharedmemCarveout value) on the same terms.
 template <class Kernel>
-inline cudaError_t ensure_dynamic_smem(Kernel kernel, size_t bytes, std::atomic<unsigned long long>& done) {
+inline cudaError_t ensure_dynamic_smem(Kernel kernel, size_t bytes, std::atomic<unsigned long long>& done,
+                                       int carveout = -1) {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
   const unsigned long long bit = 1ull << (dev & 63);
   if (done.load(std::memory_order_acquire) & bit) return cudaSuccess;
   e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (e == cudaSuccess && carveout >= 0)
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carveout);
   if (e == cudaSuccess) done.fetch_or(bit, std::memory_order_release);
   return e;
 }
@@ -93,6 +140,37 @@ class DeviceBuffer {
   size_t bytes_ = 0;
 };
 
+// Copies a host table into `buf`, which keeps at least one element so that an empty table still has an address.
+template <typename U>
+cudaError_t upload(DeviceBuffer& buf, const std::vector<U>& host) {
+  cudaError_t e = buf.reserve(std::max<size_t>(host.size(), 1) * sizeof(U));
+  if (e != cudaSuccess || host.empty()) return e;
+  return cudaMemcpy(buf.data(), host.data(), host.size() * sizeof(U), cudaMemcpyHostToDevice);
+}
+
+// create() of Plan and RealPlan: nullptr (and last_error set) when the plan cannot be built; size 0 is refused
+// (the reference never returns for 0: autosort/mod.rs:112).
+template <class P>
+P* create_plan(size_t n, int device, bool allow_fast_paths) {
+  if (n == 0) {
+    set_last_error("size 0 is not a valid transform length");
+    return nullptr;
+  }
+  P* p = new (std::nothrow) P();
+  if (!p) return nullptr;
+  cudaError_t e = cudaErrorUnknown;
+  try {
+    e = p->init(n, device, allow_fast_paths);
+  } catch (const std::exception& ex) {   // e.g. bad_alloc while building an N-entry host table
+    set_last_error(std::string("plan construction threw: ") + ex.what());
+  }
+  if (e != cudaSuccess) {
+    delete p;
+    return nullptr;
+  }
+  return p;
+}
+
 struct PlanInfo {
   size_t size = 0;
   int path = 0;
@@ -109,9 +187,10 @@ class Plan {
  public:
   using C = cpx<T>;
 
-  // Returns nullptr (and sets last_error) when the plan cannot be built; size 0 is refused
-  // (the reference never returns for 0: autosort/mod.rs:112).
-  static Plan* create(size_t n, int device, bool allow_fast_paths = true);
+  // Returns nullptr (and sets last_error) when the plan cannot be built; size 0 is refused.
+  static Plan* create(size_t n, int device, bool allow_fast_paths = true) {
+    return create_plan<Plan>(n, device, allow_fast_paths);
+  }
   ~Plan();
 
   size_t size() const { return n_; }
@@ -149,6 +228,7 @@ class Plan {
   const char* kernel_name() const;
 
  private:
+  template <class P> friend P* create_plan(size_t, int, bool);
   Plan() = default;
   cudaError_t init(size_t n, int device, bool allow_fast_paths);
 
@@ -234,7 +314,9 @@ class RealPlan {
   using C = cpx<T>;
 
   // nullptr (and last_error set) when the plan cannot be built; size 0 is refused
-  static RealPlan* create(size_t n, int device, bool allow_fast_paths = true);
+  static RealPlan* create(size_t n, int device, bool allow_fast_paths = true) {
+    return create_plan<RealPlan>(n, device, allow_fast_paths);
+  }
   ~RealPlan();
 
   size_t size() const { return n_; }
@@ -271,10 +353,15 @@ class RealPlan {
   }
 
  private:
+  template <class P> friend P* create_plan(size_t, int, bool);
   RealPlan() = default;
   cudaError_t init(size_t n, int device, bool allow_fast_paths);
   // convolve_device with row b using spectrum row (row0 + b) mod rows; adds its kernels to launches_
   cudaError_t convolve_rows(const T* in, const C* spec, size_t rows, size_t row0, T* out, size_t batch, cudaStream_t s);
+  // The host-pointer loop of exec_host and convolve_host (real.cu): chunks of rows of in_row / out_row bytes go H2D,
+  // through step(dev_in, dev_out, first_row, rows) on host_stream_, and D2H; launches() then counts all chunks.
+  template <class Step>
+  cudaError_t stage_rows(const void* in, void* out, size_t batch, size_t in_row, size_t out_row, Step step);
 
   size_t n_ = 0, m_ = 0;        // m_ = N/2 (even N)
   int device_ = 0;
@@ -290,10 +377,6 @@ class RealPlan {
   cudaStream_t host_stream_ = nullptr;
   std::string kernel_desc_;
 };
-
-// thread-local error text for the C ABI
-void set_last_error(const std::string& s);
-const char* last_error();
 
 // ---- kernel launchers implemented in the .cu files ------------------------------------------------
 

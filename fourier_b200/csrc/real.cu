@@ -9,9 +9,6 @@
 // Convolution of real rows (DESIGN.md §4.11) runs on the same three paths: onchip_conv_kernel; the inner FFT,
 // conv_pair_kernel and the inner inverse, in place in `out`; widen, FFT, hermitian_mul_kernel, inverse, real part.
 #include <algorithm>
-#include <cmath>
-#include <exception>
-#include <new>
 #include <string>
 #include <vector>
 
@@ -21,24 +18,7 @@
 
 namespace fb200 {
 
-#define FB_CHECK(expr)                                                                       \
-  do {                                                                                       \
-    cudaError_t _e = (expr);                                                                 \
-    if (_e != cudaSuccess) {                                                                 \
-      set_last_error(std::string(#expr) + ": " + cudaGetErrorString(_e));                    \
-      return _e;                                                                             \
-    }                                                                                        \
-  } while (0)
-
 namespace {
-
-constexpr int kThreads = 256;
-
-inline unsigned grid_for(size_t total) {
-  size_t blocks = (total + kThreads - 1) / kThreads;
-  const size_t cap = 132u * 32u;
-  return (unsigned)std::max<size_t>(1, std::min(blocks, cap));
-}
 
 // One thread per pair (k, M-k), k <= M/2, of one row: consecutive threads read Z[k] ascending and Z[M-k] descending.
 template <typename T, bool FWD>
@@ -113,41 +93,7 @@ real_part_kernel(const cpx<T>* __restrict__ y, T* __restrict__ out, size_t count
     out[g] = y[g].x;
 }
 
-template <typename T> T scale_of(int code, size_t n) {
-  if (code == kIfft) return (T)1 / (T)n;
-  if (code == kSqrtScaledFft || code == kSqrtScaledIfft) return (T)1 / std::sqrt((T)n);
-  return (T)1;
-}
-
-template <typename T, typename U>
-cudaError_t upload_vec(DeviceBuffer& buf, const std::vector<U>& host) {
-  cudaError_t e = buf.reserve(std::max<size_t>(host.size(), 1) * sizeof(U));
-  if (e != cudaSuccess || host.empty()) return e;
-  return cudaMemcpy(buf.data(), host.data(), host.size() * sizeof(U), cudaMemcpyHostToDevice);
-}
-
 }  // namespace
-
-template <typename T>
-RealPlan<T>* RealPlan<T>::create(size_t n, int device, bool allow_fast_paths) {
-  if (n == 0) {
-    set_last_error("size 0 is not a valid transform length");
-    return nullptr;
-  }
-  RealPlan<T>* p = new (std::nothrow) RealPlan<T>();
-  if (!p) return nullptr;
-  cudaError_t e = cudaErrorUnknown;
-  try {
-    e = p->init(n, device, allow_fast_paths);
-  } catch (const std::exception& ex) {
-    set_last_error(std::string("plan construction threw: ") + ex.what());
-  }
-  if (e != cudaSuccess) {
-    delete p;
-    return nullptr;
-  }
-  return p;
-}
 
 template <typename T>
 RealPlan<T>::~RealPlan() {
@@ -175,11 +121,11 @@ cudaError_t RealPlan<T>::init(size_t n, int device, bool allow_fast_paths) {
     host_twiddle(k, n, &re, &im);
     tab[k] = mk<T>((T)re, (T)im);
   }
-  FB_CHECK((upload_vec<T, C>(tab_, tab)));
+  FB_CHECK(upload(tab_, tab));
   if (allow_fast_paths && (fused_ = real_onchip_lookup<T>(m_)) != nullptr) {
     FB_CHECK(fused_->prepare());
-    FB_CHECK((upload_vec<T, TwPair<T>>(twa_, twopass::make_twa<T>(fused_->ra, fused_->rb))));
-    if (cudaDeviceGetAttribute(&sm_count_, cudaDevAttrMultiProcessorCount, device_) != cudaSuccess) sm_count_ = 132;
+    FB_CHECK(upload(twa_, twopass::make_twa<T>(fused_->ra, fused_->rb)));
+    sm_count_ = sm_count(device_);
     path_ = Path::kRealFused;
     kernel_desc_ = "onchip::onchip_real_kernel";
     return cudaSuccess;
@@ -223,7 +169,7 @@ cudaError_t RealPlan<T>::exec_device(bool forward, const void* in, void* out, si
   if (cudaError_t e = check_code(forward, code)) return e;
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
-  const T scale = scale_of<T>(code, n_);
+  const T scale = scale_for<T>(code, n_);
   if (path_ == Path::kRealFused) {
     FB_CHECK(fused_->run(in, out, twa_.data(), (const C*)tab_.data(), batch, forward, forward ? scale / 2 : scale,
                          sm_count_, s));
@@ -274,30 +220,42 @@ cudaError_t RealPlan<T>::exec_device(bool forward, const void* in, void* out, si
   return cudaSuccess;
 }
 
-// Host pointers: chunks of rows go H2D into stage_in_, through exec_device into stage_out_, and D2H, one chunk at a
-// time on the plan's own stream (no pipelining: the results are those of the device path, bit for bit).
+// Host pointers: chunks of rows go H2D into stage_in_, through `step` into stage_out_, and D2H, one chunk at a time on
+// the plan's own stream (no pipelining: the results are those of the device path, bit for bit).  The caller holds the
+// DeviceGuard.
+template <typename T>
+template <class Step>
+cudaError_t RealPlan<T>::stage_rows(const void* in, void* out, size_t batch, size_t in_row, size_t out_row, Step step) {
+  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
+  const size_t rows = std::min(batch, std::max<size_t>(1, kHostChunkBytes / std::max(in_row, out_row)));
+  FB_CHECK(stage_in_.reserve(rows * in_row));
+  FB_CHECK(stage_out_.reserve(rows * out_row));
+  unsigned long long total = 0;
+  for (size_t b0 = 0; b0 < batch; b0 += rows) {
+    const size_t nb = std::min(rows, batch - b0);
+    FB_CHECK(cudaMemcpyAsync(stage_in_.data(), (const char*)in + b0 * in_row, nb * in_row, cudaMemcpyHostToDevice,
+                             host_stream_));
+    launches_ = 0;
+    FB_CHECK(step(stage_in_.data(), stage_out_.data(), b0, nb));
+    total += launches_;
+    FB_CHECK(cudaMemcpyAsync((char*)out + b0 * out_row, stage_out_.data(), nb * out_row, cudaMemcpyDeviceToHost,
+                             host_stream_));
+    FB_CHECK(cudaStreamSynchronize(host_stream_));
+  }
+  launches_ = total;
+  return cudaSuccess;
+}
+
 template <typename T>
 cudaError_t RealPlan<T>::exec_host(bool forward, const void* in, void* out, size_t batch, int code) {
   launches_ = 0;
   if (cudaError_t e = check_code(forward, code)) return e;
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
-  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
-  const size_t ib = row_bytes(forward, true), ob = row_bytes(forward, false);
-  const size_t rows = std::min(batch, std::max<size_t>(1, kHostChunkBytes / std::max(ib, ob)));
-  FB_CHECK(stage_in_.reserve(rows * ib));
-  FB_CHECK(stage_out_.reserve(rows * ob));
-  unsigned long long total = 0;
-  for (size_t b0 = 0; b0 < batch; b0 += rows) {
-    const size_t nb = std::min(rows, batch - b0);
-    FB_CHECK(cudaMemcpyAsync(stage_in_.data(), (const char*)in + b0 * ib, nb * ib, cudaMemcpyHostToDevice, host_stream_));
-    FB_CHECK(exec_device(forward, stage_in_.data(), stage_out_.data(), nb, code, host_stream_));
-    total += launches_;
-    FB_CHECK(cudaMemcpyAsync((char*)out + b0 * ob, stage_out_.data(), nb * ob, cudaMemcpyDeviceToHost, host_stream_));
-    FB_CHECK(cudaStreamSynchronize(host_stream_));
-  }
-  launches_ = total;
-  return cudaSuccess;
+  return stage_rows(in, out, batch, row_bytes(forward, true), row_bytes(forward, false),
+                    [&](const void* din, void* dout, size_t, size_t nb) {
+                      return exec_device(forward, din, dout, nb, code, host_stream_);
+                    });
 }
 
 template <typename T>
@@ -354,21 +312,13 @@ cudaError_t RealPlan<T>::convolve_host(const T* in, const C* spec, size_t rows, 
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
   if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
-  const size_t rb = n_ * sizeof(T);
-  const size_t nrows = std::min(batch, std::max<size_t>(1, kHostChunkBytes / rb));
   FB_CHECK(stage_spec_.reserve(spec_bytes(rows)));
-  FB_CHECK(stage_in_.reserve(nrows * rb));
-  FB_CHECK(stage_out_.reserve(nrows * rb));
   FB_CHECK(cudaMemcpyAsync(stage_spec_.data(), spec, spec_bytes(rows), cudaMemcpyHostToDevice, host_stream_));
-  for (size_t b0 = 0; b0 < batch; b0 += nrows) {
-    const size_t nb = std::min(nrows, batch - b0);
-    FB_CHECK(cudaMemcpyAsync(stage_in_.data(), (const char*)in + b0 * rb, nb * rb, cudaMemcpyHostToDevice, host_stream_));
-    FB_CHECK(convolve_rows((const T*)stage_in_.data(), (const C*)stage_spec_.data(), rows, b0, (T*)stage_out_.data(), nb,
-                           host_stream_));
-    FB_CHECK(cudaMemcpyAsync((char*)out + b0 * rb, stage_out_.data(), nb * rb, cudaMemcpyDeviceToHost, host_stream_));
-    FB_CHECK(cudaStreamSynchronize(host_stream_));
-  }
-  return cudaSuccess;
+  return stage_rows(in, out, batch, n_ * sizeof(T), n_ * sizeof(T),
+                    [&](const void* din, void* dout, size_t b0, size_t nb) {
+                      return convolve_rows((const T*)din, (const C*)stage_spec_.data(), rows, b0, (T*)dout, nb,
+                                           host_stream_);
+                    });
 }
 
 template class RealPlan<float>;

@@ -13,8 +13,6 @@ namespace fb200 {
 
 namespace {
 
-constexpr int kThreads = 256;
-
 // One thread = one radix-R butterfly.  q = i*stride + j enumerates butterflies of one transform with
 // j (contiguous in memory) fastest, so loads are coalesced for every stride.
 template <typename T, int R, bool FWD>
@@ -109,14 +107,6 @@ chirp_out_kernel(const cpx<T>* __restrict__ work, cpx<T>* __restrict__ out,
     const size_t b = g / n, i = g - b * n;
     out[g] = cscale(ctw<FWD>(work[b * m + i], chirp[i]), scale);
   }
-}
-
-inline unsigned grid_for(size_t total) {
-  size_t blocks = (total + kThreads - 1) / kThreads;
-  const size_t cap = 132u * 32u;  // grid-stride beyond 32 CTAs per SM
-  if (blocks > cap) blocks = cap;
-  if (blocks == 0) blocks = 1;
-  return (unsigned)blocks;
 }
 
 }  // namespace

@@ -23,15 +23,6 @@
 
 namespace fb200 {
 
-#define FB_CHECK(expr)                                                                       \
-  do {                                                                                       \
-    cudaError_t _e = (expr);                                                                 \
-    if (_e != cudaSuccess) {                                                                 \
-      set_last_error(std::string(#expr) + ": " + cudaGetErrorString(_e));                    \
-      return _e;                                                                             \
-    }                                                                                        \
-  } while (0)
-
 using namespace twopass;
 
 namespace {
@@ -148,8 +139,8 @@ cudaError_t Plan<T>::init_twopass() {
   FB_CHECK(ops->prepare());
   n1_ = ops->n1;
   n2_ = ops->n2;
-  FB_CHECK((upload_vec<T, TwPair<T>>(tw_a_, make_twa<T>(ops->ra1, ops->rb1))));
-  FB_CHECK((upload_vec<T, TwPair<T>>(tw_b_, make_twa<T>(ops->ra2, ops->rb2))));
+  FB_CHECK(upload(tw_a_, make_twa<T>(ops->ra1, ops->rb1)));
+  FB_CHECK(upload(tw_b_, make_twa<T>(ops->ra2, ops->rb2)));
   // inter-pass twiddles in the layout of the intermediate: T[k1*N2 + n2] = w_N^{n2*k1}
   std::vector<cpx<T>> tw2(n_);
   for (size_t k1 = 0; k1 < n1_; ++k1)
@@ -158,7 +149,7 @@ cudaError_t Plan<T>::init_twopass() {
       host_twiddle(k1 * c, n_, &re, &im);
       tw2[k1 * n2_ + c] = mk<T>((T)re, (T)im);
     }
-  FB_CHECK((upload_vec<T, cpx<T>>(tw2_, tw2)));
+  FB_CHECK(upload(tw2_, tw2));
   // transforms per chunk: the intermediate of one chunk should sit comfortably inside the L2
   size_t mb = 32;
   if (const char* env = std::getenv("FOURIER_B200_CHUNK_MB")) mb = (size_t)std::max(1, atoi(env));
@@ -170,14 +161,14 @@ cudaError_t Plan<T>::init_twopass() {
     const FusedOps<T>* f = fused_lookup<T>(n_);
     if (f && f->prepare() == cudaSuccess) {
       // the persistent kernel has its own split and register tile (the tile kernels above stay as its fallback)
-      FB_CHECK((upload_vec<T, TwPair<T>>(tw_f_, make_twa<T>(f->ra, f->rb))));
-      FB_CHECK((upload_vec<T, TwPair<T>>(tw_f2_, make_twa<T>(f->ra2, f->rb2))));
+      FB_CHECK(upload(tw_f_, make_twa<T>(f->ra, f->rb)));
+      FB_CHECK(upload(tw_f2_, make_twa<T>(f->ra2, f->rb2)));
       // factored inter-pass twiddles, contiguous per pass-1 tile of `tile_c` columns:
       //   tbase[tile][col][p] = w_N^{n2*p},  tstep[tile][r][col] = w_N^{R*n2*r},  n2 = tile*tile_c + col
       std::vector<cpx<T>> tb, ts;
       make_factored_twiddles<T>(n_, f->n2, f->ra, f->rb, f->tile_c, tb, ts, f->base_pcol);
-      FB_CHECK((upload_vec<T, cpx<T>>(tbase_, tb)));
-      FB_CHECK((upload_vec<T, cpx<T>>(tstep_, ts)));
+      FB_CHECK(upload(tbase_, tb));
+      FB_CHECK(upload(tstep_, ts));
       fused_ops_ = f;
       ring_ = std::max(2, env_int("FOURIER_B200_RING", f->default_ring));
       lag_ = std::min(ring_ - 1, std::max(1, env_int("FOURIER_B200_LAG", f->default_lag)));
@@ -185,10 +176,7 @@ cudaError_t Plan<T>::init_twopass() {
       snprintf(desc, sizeof desc, "fused::fused_twopass_kernel [%zux%zu, %d groups x %d, %s, ring %d, lag %d]", f->n1,
                f->n2, f->groups, f->group_threads, f->direct ? "direct loads" : "TMA staging", ring_, lag_);
       kernel_desc_ = desc;
-      int dev = 0, sms = 132;
-      cudaGetDevice(&dev);
-      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-      sm_count_ = sms;
+      sm_count_ = sm_count(device_);
     }
   }
   return cudaSuccess;
@@ -198,10 +186,8 @@ template <typename T>
 cudaError_t Plan<T>::exec_twopass(const C* in, C* out, size_t batch, int code, cudaStream_t s) {
   const auto* ops = static_cast<const TwoPassOps<T>*>(fast_ops_);
   const bool fwd = transform_is_forward(code);
-  const bool do_scale = !(code == kFft || code == kUnscaledIfft);
-  T scale = (T)1;
-  if (code == kIfft) scale = (T)1 / (T)n_;
-  else if (do_scale) scale = (T)1 / std::sqrt((T)n_);
+  const bool do_scale = code != kFft && code != kUnscaledIfft;
+  const T scale = scale_for<T>(code, n_);
   if (fused_ops_ && batch <= (size_t)1 << 24) {
     const auto* f = static_cast<const FusedOps<T>*>(fused_ops_);
     const fused::RingLag rl = fused::launch_ring(ring_, lag_, (long)batch);

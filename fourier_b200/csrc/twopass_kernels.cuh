@@ -186,13 +186,5 @@ template <typename T> const TwoPassOps<T>* lookup(size_t n) {
   return o;
 }
 
-template <typename T, typename U>
-cudaError_t upload_vec(DeviceBuffer& buf, const std::vector<U>& host) {
-  cudaError_t e = buf.reserve(host.size() * sizeof(U));
-  if (e != cudaSuccess) return e;
-  return cudaMemcpy(buf.data(), host.data(), host.size() * sizeof(U), cudaMemcpyHostToDevice);
-}
-
-
 }  // namespace twopass
 }  // namespace fb200

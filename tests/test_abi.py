@@ -129,6 +129,26 @@ def test_distributed_building_blocks_reject_bad_arguments(libfourier):
     assert L.fourier_b200_peer_close(None) == 0 and L.fourier_b200_peer_free(None) == 0              # no-ops
 
 
+def test_null_arguments_of_plan_calls_are_refused_with_a_message(libfourier):
+    """A NULL plan or output needs no device to be refused: nonzero return code and "null argument" in
+    fourier_b200_last_error(), for the info and transform calls of both plan kinds."""
+    import ctypes
+    L = _lib.load()
+    outs = (ctypes.c_void_p * 2)(None, None)
+    buf = ctypes.create_string_buffer(64)
+    info = _lib.PlanInfo()
+    for t in ("float", "double"):
+        for call in (lambda: getattr(L, f"fourier_b200_plan_info_{t}")(None, ctypes.byref(info)),
+                     lambda: getattr(L, f"fourier_b200_plan_info_{t}")(buf, None),
+                     lambda: getattr(L, f"fourier_b200_rfft_info_{t}")(None, ctypes.byref(info)),
+                     lambda: getattr(L, f"fourier_b200_transform_batch_{t}")(None, buf, buf, 1, 0),
+                     lambda: getattr(L, f"fourier_b200_transform_batch_async_{t}")(None, buf, buf, 1, 0, None)):
+            assert L.fourier_b200_exchange_float(None, outs, 2, 0, 8, 8, 16, 16, 0, 0, 0, 0, None) != 0
+            assert "null argument" not in _lib.last_error()
+            assert call() != 0
+            assert "null argument" in _lib.last_error()
+
+
 def test_product_never_imports_the_oracle():
     """oracle/ is test infrastructure: nothing under fourier_b200/ may include, import, link or dlopen it
     (comments may mention it)."""
