@@ -14,7 +14,7 @@
 // along r (the batch), so one tile takes the SAME intermediate row k1 of C ADJACENT TRANSFORMS (instead of C adjacent
 // rows of one transform, twopass_kernels.cuh Body2): loads are C contiguous runs of N2 samples, stores are C-sample
 // (64 / 128-byte) pieces, one per output k = k1 + N1 * k2, whose destination rank is k / cb.
-// Every member is __host__ __device__ (tools/emulate.cu runs it on the CPU).
+// Every member is __host__ __device__; the two phases follow tilefft.cuh's protocol.
 #pragma once
 
 #include <cmath>
@@ -111,17 +111,18 @@ struct RowsExchangeBody {
       });
     });
   }
+
+  // phase protocol (tilefft.cuh); the stage twiddles come from Args
+  static constexpr int kPhases = 2;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long block, int t, V* smem, const TwPair<T>*) {
+    if constexpr (P == 0) phase1(f, a, block, t, smem);
+    else phase2(f, a, block, t, smem);
+  }
 };
 
 template <class Body, class Tile, int MINB>
 __global__ void __launch_bounds__(Tile::THREADS, MINB) rows_exchange_kernel(const typename Body::Args a) {
-  using V = typename Tile::V;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  V* smem = reinterpret_cast<V*>(smem_raw);
-  Tile f;
-  Body::phase1(f, a, blockIdx.x, threadIdx.x, smem);
-  __syncthreads();
-  Body::phase2(f, a, blockIdx.x, threadIdx.x, smem);
+  run_cta_tile<Tile, Body>(a);
 }
 
 }  // namespace dist

@@ -38,12 +38,23 @@ struct OnChipImpl {
       BCfg::EX_BYTES + BCfg::TWA_BYTES + sizeof(cpx<T>) * (4 * (size_t)BCfg::L + (LOCAL_STASH ? 0 : (size_t)E * BCfg::THREADS));
   static constexpr bool kHasBluestein = (RA == RB) && (E == RA);
 
+  // the fft / real / conv kernels: the exchange and the stage twiddles in shared memory, groups of C transforms
+  // grid-stride over at most sms * MINB * 4 CTAs
+  template <class Args> static cudaError_t allow_smem(void (*kernel)(Args)) {
+    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_fft);
+  }
+  template <class Args>
+  static cudaError_t launch(void (*kernel)(Args), const Args& a, size_t batch, int sms, cudaStream_t s) {
+    const size_t groups = (batch + Cfg<true>::C - 1) / Cfg<true>::C;
+    const unsigned grid = (unsigned)std::min<size_t>(groups, (size_t)sms * MINB * 4);
+    kernel<<<grid, Cfg<true>::THREADS, smem_fft, s>>>(a);
+    return cudaGetLastError();
+  }
+
   static cudaError_t prepare() {
     cudaError_t e;
-    if ((e = cudaFuncSetAttribute(onchip::onchip_fft_kernel<Cfg<true>, MINB>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_fft))) return e;
-    if ((e = cudaFuncSetAttribute(onchip::onchip_fft_kernel<Cfg<false>, MINB>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_fft))) return e;
+    if ((e = allow_smem(onchip::onchip_fft_kernel<Cfg<true>, MINB>))) return e;
+    if ((e = allow_smem(onchip::onchip_fft_kernel<Cfg<false>, MINB>))) return e;
     if constexpr (kHasBluestein) {
       if ((e = cudaFuncSetAttribute(onchip::bluestein_fused_kernel<BCfg, 1, LOCAL_STASH>,
                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_blue))) return e;
@@ -52,16 +63,11 @@ struct OnChipImpl {
   }
   static cudaError_t fft(const cpx<T>* in, cpx<T>* out, const void* twa, size_t batch, bool fwd, T scale,
                          bool do_scale, int sms, cudaStream_t s) {
-    const size_t groups = (batch + Cfg<true>::C - 1) / Cfg<true>::C;
-    const unsigned grid = (unsigned)std::min<size_t>(groups, (size_t)sms * MINB * 4);
-    if (fwd) {
-      typename onchip::FftBody<Cfg<true>>::Args a = {in, out, (const TwPair<T>*)twa, (long)batch, scale, do_scale};
-      onchip::onchip_fft_kernel<Cfg<true>, MINB><<<grid, Cfg<true>::THREADS, smem_fft, s>>>(a);
-    } else {
-      typename onchip::FftBody<Cfg<false>>::Args a = {in, out, (const TwPair<T>*)twa, (long)batch, scale, do_scale};
-      onchip::onchip_fft_kernel<Cfg<false>, MINB><<<grid, Cfg<false>::THREADS, smem_fft, s>>>(a);
-    }
-    return cudaGetLastError();
+    if (fwd)
+      return launch(onchip::onchip_fft_kernel<Cfg<true>, MINB>,
+                    {in, out, (const TwPair<T>*)twa, (long)batch, scale, do_scale}, batch, sms, s);
+    return launch(onchip::onchip_fft_kernel<Cfg<false>, MINB>,
+                  {in, out, (const TwPair<T>*)twa, (long)batch, scale, do_scale}, batch, sms, s);
   }
   static cudaError_t bluestein(const cpx<T>* in, cpx<T>* out, const void* twa, const cpx<T>* chirp,
                                const cpx<T>* wm, const cpx<T>* wce, const cpx<T>* wco, size_t n, size_t batch,
@@ -79,36 +85,23 @@ struct OnChipImpl {
   }
   static cudaError_t real_prepare() {
     cudaError_t e;
-    if ((e = cudaFuncSetAttribute(onchip::onchip_real_kernel<Cfg<true>, MINB>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_fft))) return e;
-    if ((e = cudaFuncSetAttribute(onchip::onchip_real_kernel<Cfg<false>, MINB>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_fft))) return e;
-    return cudaFuncSetAttribute(onchip::onchip_conv_kernel<Cfg<true>, MINB>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_fft);
+    if ((e = allow_smem(onchip::onchip_real_kernel<Cfg<true>, MINB>))) return e;
+    if ((e = allow_smem(onchip::onchip_real_kernel<Cfg<false>, MINB>))) return e;
+    return allow_smem(onchip::onchip_conv_kernel<Cfg<true>, MINB>);
   }
   static cudaError_t conv(const void* in, void* out, const void* twa, const cpx<T>* tab, const cpx<T>* spec,
                           size_t rows, size_t row0, size_t batch, T h, int sms, cudaStream_t s) {
-    const size_t groups = (batch + Cfg<true>::C - 1) / Cfg<true>::C;
-    const unsigned grid = (unsigned)std::min<size_t>(groups, (size_t)sms * MINB * 4);
-    const typename onchip::ConvBody<Cfg<true>>::Args a = {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab,
-                                                          spec, (long)rows, (long)row0, (long)batch, h};
-    onchip::onchip_conv_kernel<Cfg<true>, MINB><<<grid, Cfg<true>::THREADS, smem_fft, s>>>(a);
-    return cudaGetLastError();
+    return launch(onchip::onchip_conv_kernel<Cfg<true>, MINB>,
+                  {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab, spec, (long)rows, (long)row0, (long)batch, h},
+                  batch, sms, s);
   }
   static cudaError_t real(const void* in, void* out, const void* twa, const cpx<T>* tab, size_t batch, bool fwd, T h,
                           int sms, cudaStream_t s) {
-    const size_t groups = (batch + Cfg<true>::C - 1) / Cfg<true>::C;
-    const unsigned grid = (unsigned)std::min<size_t>(groups, (size_t)sms * MINB * 4);
-    if (fwd) {
-      const typename onchip::RealBody<Cfg<true>>::Args a = {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab,
-                                                            (long)batch, h};
-      onchip::onchip_real_kernel<Cfg<true>, MINB><<<grid, Cfg<true>::THREADS, smem_fft, s>>>(a);
-    } else {
-      const typename onchip::RealBody<Cfg<false>>::Args a = {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab,
-                                                             (long)batch, h};
-      onchip::onchip_real_kernel<Cfg<false>, MINB><<<grid, Cfg<false>::THREADS, smem_fft, s>>>(a);
-    }
-    return cudaGetLastError();
+    if (fwd)
+      return launch(onchip::onchip_real_kernel<Cfg<true>, MINB>,
+                    {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab, (long)batch, h}, batch, sms, s);
+    return launch(onchip::onchip_real_kernel<Cfg<false>, MINB>,
+                  {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab, (long)batch, h}, batch, sms, s);
   }
   static const OnChipOps<T>* ops() {
     static const RealOnChipOps<T> r = {RA, RB, &real_prepare, &real, &conv};

@@ -6,6 +6,7 @@
 //                             one warp-private shared-memory exchange -> registers -> global.
 //   * onchip_real_kernel:     real-input transforms of length 2L (forward and inverse) on the same tiles.
 //   * onchip_conv_kernel:     y = irfft(rfft(x) . H) of real rows of length 2L, both transforms in one kernel.
+//     (these three run the phases of FftBody / RealBody / ConvBody through run_onchip_groups, tilefft.cuh)
 //   * bluestein_fused_kernel: the whole chirp-z transform of the reference (bluesteins.rs:218-259) for
 //                             N <= L, M = 2L, in one kernel and without touching HBM in between.
 //
@@ -79,27 +80,18 @@ template <class Cfg> struct FftBody {
       });
     });
   }
+
+  // phase protocol (tilefft.cuh)
+  static constexpr int kPhases = 2;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    if constexpr (P == 0) phase1(f, a, grp, t, smem, twa);
+    else phase2(f, a, grp, t, smem);
+  }
 };
 
 template <class Cfg, int MINB>
-__global__ void __launch_bounds__(Cfg::THREADS, MINB)
-onchip_fft_kernel(const typename FftBody<Cfg>::Args a) {
-  using Body = FftBody<Cfg>;
-  using V = typename Cfg::Tile::V;
-  using T = decltype(V::x);
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  V* exch = reinterpret_cast<V*>(smem_raw);
-  TwPair<T>* twa = reinterpret_cast<TwPair<T>*>(smem_raw + Cfg::EX_BYTES);
-  for (int i = threadIdx.x; i < (Cfg::Tile::RA / 2) * Cfg::Tile::RB; i += Cfg::THREADS) twa[i] = a.twa[i];
-  __syncthreads();
-  const long groups = (a.batch + Cfg::C - 1) / Cfg::C;
-  typename Cfg::Tile f;
-  for (long grp = blockIdx.x; grp < groups; grp += gridDim.x) {
-    Body::phase1(f, a, grp, threadIdx.x, exch, twa);
-    __syncwarp();
-    Body::phase2(f, a, grp, threadIdx.x, exch);
-    __syncwarp();
-  }
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_fft_kernel(const typename FftBody<Cfg>::Args a) {
+  run_onchip_groups<Cfg, FftBody<Cfg>>(a);
 }
 
 // ---- fused real-input transforms, N = 2L (real_kernels.cuh) ----------------------------------------------------
@@ -165,37 +157,25 @@ template <class Cfg> struct RealBody {
     const typename Fft::Args fa = {nullptr, a.out, nullptr, a.batch, (T)1, 0};
     Fft::phase2(f, fa, grp, t, smem);
   }
+
+  // phase protocol (tilefft.cuh): forward load + stage A, stage B, park, untangle; inverse tangle + stage A, stage B
+  static constexpr int kPhases = Tile::FWD ? 4 : 2;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    if constexpr (Tile::FWD) {
+      if constexpr (P == 0) fwd_phase1(f, a, grp, t, smem, twa);
+      else if constexpr (P == 1) fwd_gather(f, t, smem);
+      else if constexpr (P == 2) fwd_park(f, t, smem);
+      else fwd_store(a, grp, t, smem);
+    } else {
+      if constexpr (P == 0) inv_phase1(f, a, grp, t, smem, twa);
+      else inv_phase2(f, a, grp, t, smem);
+    }
+  }
 };
 
 template <class Cfg, int MINB>
-__global__ void __launch_bounds__(Cfg::THREADS, MINB)
-onchip_real_kernel(const typename RealBody<Cfg>::Args a) {
-  using Body = RealBody<Cfg>;
-  using V = typename Cfg::Tile::V;
-  using T = decltype(V::x);
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  V* exch = reinterpret_cast<V*>(smem_raw);
-  TwPair<T>* twa = reinterpret_cast<TwPair<T>*>(smem_raw + Cfg::EX_BYTES);
-  for (int i = threadIdx.x; i < (Cfg::Tile::RA / 2) * Cfg::Tile::RB; i += Cfg::THREADS) twa[i] = a.twa[i];
-  __syncthreads();
-  const long groups = (a.batch + Cfg::C - 1) / Cfg::C;
-  typename Cfg::Tile f;
-  for (long grp = blockIdx.x; grp < groups; grp += gridDim.x) {
-    if constexpr (Cfg::Tile::FWD) {
-      Body::fwd_phase1(f, a, grp, threadIdx.x, exch, twa);
-      __syncwarp();
-      Body::fwd_gather(f, threadIdx.x, exch);
-      __syncwarp();
-      Body::fwd_park(f, threadIdx.x, exch);
-      __syncwarp();
-      Body::fwd_store(a, grp, threadIdx.x, exch);
-    } else {
-      Body::inv_phase1(f, a, grp, threadIdx.x, exch, twa);
-      __syncwarp();
-      Body::inv_phase2(f, a, grp, threadIdx.x, exch);
-    }
-    __syncwarp();
-  }
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_real_kernel(const typename RealBody<Cfg>::Args a) {
+  run_onchip_groups<Cfg, RealBody<Cfg>>(a);
 }
 
 // ---- fused convolution of real rows, y = irfft(rfft(x) . H), N = 2L (real_kernels.cuh, DESIGN.md §4.11) ----------
@@ -254,37 +234,23 @@ template <class Cfg> struct ConvBody {
       });
     });
   }
+
+  // phase protocol (tilefft.cuh): RealBody's forward up to the park, the pairs, then the inverse on the forward tile
+  static constexpr int kPhases = 7;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    if constexpr (P == 0) fwd_phase1(f, a, grp, t, smem, twa);
+    else if constexpr (P == 1) Real::fwd_gather(f, t, smem);
+    else if constexpr (P == 2) Real::fwd_park(f, t, smem);
+    else if constexpr (P == 3) pairs(a, grp, t, smem);
+    else if constexpr (P == 4) inv_stage_a(f, t, smem, twa);
+    else if constexpr (P == 5) inv_scatter(f, t, smem);
+    else inv_store(f, a, grp, t, smem);
+  }
 };
 
 template <class Cfg, int MINB>
-__global__ void __launch_bounds__(Cfg::THREADS, MINB)
-onchip_conv_kernel(const typename ConvBody<Cfg>::Args a) {
-  using Body = ConvBody<Cfg>;
-  using V = typename Cfg::Tile::V;
-  using T = decltype(V::x);
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  V* exch = reinterpret_cast<V*>(smem_raw);
-  TwPair<T>* twa = reinterpret_cast<TwPair<T>*>(smem_raw + Cfg::EX_BYTES);
-  for (int i = threadIdx.x; i < (Cfg::Tile::RA / 2) * Cfg::Tile::RB; i += Cfg::THREADS) twa[i] = a.twa[i];
-  __syncthreads();
-  const long groups = (a.batch + Cfg::C - 1) / Cfg::C;
-  typename Cfg::Tile f;
-  for (long grp = blockIdx.x; grp < groups; grp += gridDim.x) {
-    Body::fwd_phase1(f, a, grp, threadIdx.x, exch, twa);
-    __syncwarp();
-    Body::Real::fwd_gather(f, threadIdx.x, exch);
-    __syncwarp();
-    Body::Real::fwd_park(f, threadIdx.x, exch);
-    __syncwarp();
-    Body::pairs(a, grp, threadIdx.x, exch);
-    __syncwarp();
-    Body::inv_stage_a(f, threadIdx.x, exch, twa);
-    __syncwarp();
-    Body::inv_scatter(f, threadIdx.x, exch);
-    __syncwarp();
-    Body::inv_store(f, a, grp, threadIdx.x, exch);
-    __syncwarp();
-  }
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_conv_kernel(const typename ConvBody<Cfg>::Args a) {
+  run_onchip_groups<Cfg, ConvBody<Cfg>>(a);
 }
 
 // ---- fused Bluestein -------------------------------------------------------------------------------------------

@@ -67,17 +67,18 @@ struct ColumnBody {
       });
     });
   }
+
+  // phase protocol (tilefft.cuh); the stage twiddles come from Args
+  static constexpr int kPhases = 2;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long block, int t, V* smem, const TwPair<T>*) {
+    if constexpr (P == 0) phase1(f, a, block, t, smem);
+    else phase2(f, a, block, t, smem);
+  }
 };
 
 template <class Body, class Tile, int MINB>
 __global__ void __launch_bounds__(Tile::THREADS, MINB) column_kernel(const typename Body::Args a) {
-  using V = typename Tile::V;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  V* smem = reinterpret_cast<V*>(smem_raw);
-  Tile f;
-  Body::phase1(f, a, blockIdx.x, threadIdx.x, smem);
-  __syncthreads();
-  Body::phase2(f, a, blockIdx.x, threadIdx.x, smem);
+  run_cta_tile<Tile, Body>(a);
 }
 
 // Outer pass of length B = 3, 9 or 27 for N = B * Nb (Nb a two-pass power of two): the radix-3 stages of the

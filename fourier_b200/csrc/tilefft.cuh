@@ -22,8 +22,17 @@
 //                    a warp reads 256 contiguous bytes and only 8 different stage twiddles (broadcast)
 // The mapping is a template argument MAP of each access: kMapCF = 0 (false), kMapUF = 1 (true), kMapBF = 2.
 //
-// Every member is __host__ __device__: tools/emulate.cu runs the identical code thread by thread on
-// the CPU (there is no GPU in the build container), tests/test_kernel_emulation.py checks it.
+// Every member is __host__ __device__, so the CPU emulators (tools/emulate*.cu) run the identical code thread by
+// thread on the CPU.
+//
+// Phase protocol.  A kernel body built on these tiles (FftBody, RealBody, ConvBody in onchip_kernels.cuh,
+// twopass::TileBody, dist::RowsExchangeBody, outer::ColumnBody) states once what runs between two barriers, and in
+// what order:
+//   static constexpr int kPhases;
+//   template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa);
+// for P = 0 .. kPhases-1, thread t of group (tile) grp, exchange buffer smem, stage twiddles twa in shared memory (the
+// bodies that read theirs from Args ignore it).  The caller puts a barrier between consecutive phases: the device
+// drivers below, and the CPU driver of tools/emulate_common.h, which runs each phase for every thread before the next.
 #pragma once
 
 #include "cplx.cuh"
@@ -302,5 +311,38 @@ struct TileFFT {
     });
   }
 };
+
+// ---- device drivers of the phase protocol -------------------------------------------------------------------------
+// On-chip kernels (onchip_kernels.cuh): the stage twiddles are copied to shared memory behind the exchange buffer, then
+// the CTA loops grid-stride over groups of Cfg::C transforms, each phase followed by __syncwarp (the last one too: the
+// next group reuses the exchange buffer).
+template <class Cfg, class Body> __device__ __forceinline__ void run_onchip_groups(const typename Body::Args& a) {
+  using Tile = typename Cfg::Tile;
+  using T = typename Body::T;
+  extern __shared__ __align__(128) unsigned char onchip_smem[];
+  typename Tile::V* exch = reinterpret_cast<typename Tile::V*>(onchip_smem);
+  TwPair<T>* twa = reinterpret_cast<TwPair<T>*>(onchip_smem + Cfg::EX_BYTES);
+  for (int i = threadIdx.x; i < (Tile::RA / 2) * Tile::RB; i += Cfg::THREADS) twa[i] = a.twa[i];
+  __syncthreads();
+  const long groups = (a.batch + Cfg::C - 1) / Cfg::C;
+  Tile f;
+  for (long grp = blockIdx.x; grp < groups; grp += gridDim.x) {
+    static_for<0, Body::kPhases>([&](auto P) FB_LAMBDA {
+      Body::template phase<decltype(P)::value>(f, a, grp, threadIdx.x, exch, twa);
+      __syncwarp();
+    });
+  }
+}
+
+// Single-tile CTA kernels: CTA blockIdx.x runs the phases of its tile, with __syncthreads between them.
+template <class Tile, class Body> __device__ __forceinline__ void run_cta_tile(const typename Body::Args& a) {
+  extern __shared__ __align__(16) unsigned char tile_smem[];
+  typename Tile::V* smem = reinterpret_cast<typename Tile::V*>(tile_smem);
+  Tile f;
+  static_for<0, Body::kPhases>([&](auto P) FB_LAMBDA {
+    if constexpr (decltype(P)::value > 0) __syncthreads();
+    Body::template phase<decltype(P)::value>(f, a, blockIdx.x, threadIdx.x, smem, nullptr);
+  });
+}
 
 }  // namespace fb200

@@ -14,8 +14,7 @@ namespace twopass {
 
 // ---- kernels ------------------------------------------------------------------------------------------
 // One CTA = one tile of Tile::C FFTs of one transform of the chunk.
-// The body of one tile, split at the CTA barrier so that tools/emulate.cu can run the identical code on
-// the CPU: phase1 for every thread, then phase2 for every thread.
+// The body of one tile, split at the CTA barrier into the two phases of tilefft.cuh's protocol.
 template <class Tile, class LAY, long NS, long CS, bool LOAD_UF, long KS, long OCS, bool TW2>
 struct TileBody {
   using V = typename Tile::V;
@@ -42,20 +41,20 @@ struct TileBody {
     if (a.do_scale) f.template store<false, KS, OCS, TW2, true>(t, dst, t2, a.scale);
     else f.template store<false, KS, OCS, TW2, false>(t, dst, t2, a.scale);
   }
+
+  // phase protocol (tilefft.cuh); the stage twiddles come from Args
+  static constexpr int kPhases = 2;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long block, int t, V* smem, const TwPair<T>*) {
+    if constexpr (P == 0) phase1(f, a, block, t, smem);
+    else phase2(f, a, block, t, smem);
+  }
 };
 
 // One CTA = one tile of Tile::C FFTs of one transform of the chunk.
 template <class Tile, class LAY, long NS, long CS, bool LOAD_UF, long KS, long OCS, bool TW2, int MINB>
 __global__ void __launch_bounds__(Tile::THREADS, MINB)
 tile_kernel(const typename TileBody<Tile, LAY, NS, CS, LOAD_UF, KS, OCS, TW2>::Args a) {
-  using Body = TileBody<Tile, LAY, NS, CS, LOAD_UF, KS, OCS, TW2>;
-  using V = typename Tile::V;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  V* smem = reinterpret_cast<V*>(smem_raw);
-  Tile f;
-  Body::phase1(f, a, blockIdx.x, threadIdx.x, smem);
-  __syncthreads();
-  Body::phase2(f, a, blockIdx.x, threadIdx.x, smem);
+  run_cta_tile<Tile, TileBody<Tile, LAY, NS, CS, LOAD_UF, KS, OCS, TW2>>(a);
 }
 
 template <typename T> struct TwoPassOps {

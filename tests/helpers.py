@@ -1,10 +1,14 @@
-"""Shared test helpers: the reference test-suite's comparison rule and input procedure."""
+"""Shared test helpers: the reference test-suite's comparison rule and input procedure, and the CPU emulators."""
 import json
 import os
+import shutil
+import subprocess
 
 import numpy as np
+import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+ROOT = os.path.dirname(HERE)
 
 
 def golden_10pt():
@@ -116,3 +120,19 @@ def truth_f64(x, code):
         y = np.fft.ifft(x, axis=-1) * n
     scale = {0: 1.0, 1: 1.0 / n, 2: 1.0, 3: 1.0 / np.sqrt(n), 4: 1.0 / np.sqrt(n)}[code]
     return y * scale
+
+
+def run_emulator(name, tmp_dir):
+    """Compiles tools/<name>.cu (host code only, nvcc; the test skips without it) into tmp_dir, runs it and returns the
+    CompletedProcess, after printing its stdout."""
+    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+    if not os.path.exists(nvcc):
+        pytest.skip("nvcc not available")
+    exe = os.path.join(str(tmp_dir), name)
+    csrc = os.path.join(ROOT, "fourier_b200", "csrc")
+    subprocess.run([nvcc, "-std=c++17", "-O1", "--expt-relaxed-constexpr", "-gencode", "arch=compute_90a,code=sm_90a",
+                    "-I", csrc, os.path.join(ROOT, "tools", name + ".cu"), os.path.join(csrc, "host_math.cu"),
+                    "-o", exe], check=True, capture_output=True)
+    r = subprocess.run([exe], capture_output=True, text=True)
+    print(r.stdout)
+    return r

@@ -3,29 +3,16 @@ onchip_kernels.cuh) on the CPU through tools/emulate_conv.cu: the fused on-chip 
 in both precisions with three spectrum rows, and the pair step alone for even and odd M = N/2, thread by thread against
 a direct circular convolution in double.  The emulator records every read of H: none may be wider than one complex
 value or misaligned, and f32 rows of odd index (8 bytes off a 16-byte boundary) must really be read."""
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from helpers import run_emulator
 
 
 @pytest.fixture(scope="module")
 def emulation(tmp_path_factory):
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("nvcc not available")
-    exe = tmp_path_factory.mktemp("emulate_conv") / "emulate_conv"
-    csrc = os.path.join(ROOT, "fourier_b200", "csrc")
-    subprocess.run([nvcc, "-std=c++17", "-O1", "--expt-relaxed-constexpr", "-gencode", "arch=compute_90a,code=sm_90a",
-                    "-I", csrc, os.path.join(ROOT, "tools", "emulate_conv.cu"), os.path.join(csrc, "host_math.cu"),
-                    "-o", str(exe)], check=True, capture_output=True)
-    r = subprocess.run([str(exe)], capture_output=True, text=True)
-    print(r.stdout)
-    return r
+    return run_emulator("emulate_conv", tmp_path_factory.mktemp("emulate_conv"))
 
 
 def test_emulated_conv_matches_direct_convolution(emulation):

@@ -3,29 +3,16 @@ through tools/emulate_real.cu: the fused on-chip real kernel of every on-chip si
 and inverse, and the untangle / tangle steps for even and odd M = N/2, thread by thread against a double-precision
 DFT.  The emulator records every spectrum access: none may be wider than one complex value or misaligned (f32
 spectrum rows of odd index start 8 bytes off a 16-byte boundary)."""
-import os
 import re
-import shutil
-import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from helpers import run_emulator
 
 
 @pytest.fixture(scope="module")
 def emulation(tmp_path_factory):
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("nvcc not available")
-    exe = tmp_path_factory.mktemp("emulate_real") / "emulate_real"
-    csrc = os.path.join(ROOT, "fourier_b200", "csrc")
-    subprocess.run([nvcc, "-std=c++17", "-O1", "--expt-relaxed-constexpr", "-gencode", "arch=compute_90a,code=sm_90a",
-                    "-I", csrc, os.path.join(ROOT, "tools", "emulate_real.cu"), os.path.join(csrc, "host_math.cu"),
-                    "-o", str(exe)], check=True, capture_output=True)
-    r = subprocess.run([str(exe)], capture_output=True, text=True)
-    print(r.stdout)
-    return r
+    return run_emulator("emulate_real", tmp_path_factory.mktemp("emulate_real"))
 
 
 def test_emulated_real_kernels_match_f64_dft(emulation):

@@ -4,18 +4,13 @@
 // twiddle tables and shared-memory layouts are verified before a kernel ever runs on the GPU.
 // It also reports shared-memory bank conflicts of the exchange (64-bit/128-bit access model).
 // Build: nvcc -std=c++17 -O1 --expt-relaxed-constexpr -I fourier_b200/csrc tools/emulate.cu \
-//             fourier_b200/csrc/plan.cu ... (host only, never run on the device)
-#include <algorithm>
-#include <cmath>
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
+//             fourier_b200/csrc/host_math.cu (host only, never run on the device)
+#include "emulate_common.h"
 
 #include "cta_kernels.cuh"
 #include "dist_kernels.cuh"
 #include "fused_configs.cuh"
 #include "fused_kernels.cuh"
-#include "onchip_kernels.cuh"
 #include "outer_kernels.cuh"
 #include "twopass_kernels.cuh"
 
@@ -25,52 +20,7 @@
 #ifndef FB_PADX
 #define FB_PADX 8
 #endif
-using namespace fb200;
 using namespace fb200::twopass;
-
-template <typename T> static void fill(std::vector<cpx<T>>& x, unsigned seed) {
-  unsigned long long s = seed * 2654435761ull + 12345;
-  for (auto& v : x) {
-    s = s * 6364136223846793005ull + 1442695040888963407ull;
-    v.x = (T)((double)(s >> 11) / 9007199254740992.0 * 2 - 1);
-    s = s * 6364136223846793005ull + 1442695040888963407ull;
-    v.y = (T)((double)(s >> 11) / 9007199254740992.0 * 2 - 1);
-  }
-}
-
-// worst-case bank conflict degree of one warp-wide shared access, element size B bytes:
-// lanes are served in groups of 128 bytes worth of lanes (half-warp for 8 B, quarter-warp for 16 B)
-template <int B> static int conflict_degree(const std::vector<long>& elem_index) {
-  const int group = 128 / B;
-  int worst = 1;
-  for (size_t g = 0; g + group <= elem_index.size(); g += group) {
-    int count[32] = {0};
-    // distinct addresses in the same bank conflict; identical addresses broadcast
-    std::vector<long> seen;
-    for (int l = 0; l < group; ++l) {
-      long e = elem_index[g + l];
-      bool dup = false;
-      for (long s : seen) dup |= (s == e);
-      if (dup) continue;
-      seen.push_back(e);
-      int bank = (int)((e * B / 4) % 32);
-      worst = std::max(worst, ++count[bank]);
-    }
-  }
-  return worst;
-}
-
-// Runs one tile body (both phases) for `blocks` CTAs on the CPU.
-template <class Body, class Tile, class LAY>
-static void run_body(const typename Body::Args& a, long blocks) {
-  using V = typename Tile::V;
-  std::vector<V> smem(Tile::template smem_elems<LAY>());
-  std::vector<Tile> thr(Tile::THREADS);
-  for (long b = 0; b < blocks; ++b) {
-    for (int t = 0; t < Tile::THREADS; ++t) Body::phase1(thr[t], a, b, t, smem.data());
-    for (int t = 0; t < Tile::THREADS; ++t) Body::phase2(thr[t], a, b, t, smem.data());
-  }
-}
 
 // Bank-conflict report for the exchange of a tile: scatter with mapping UF_A, gather with col-fast.
 template <class Tile, class LAY, int UF_A, int UF_B = 0>
@@ -168,14 +118,8 @@ static int check_onchip(const char* name, double tol) {
     auto run = [&](auto cfg_tag) {
       using Cfg = decltype(cfg_tag);
       using Body = onchip::FftBody<Cfg>;
-      typename Body::Args a = {x.data(), out.data(), twa.data(), batch, (T)0.5, 1};
-      std::vector<cpx<T>> smem(Cfg::Tile::template smem_elems<typename Cfg::Lay>());
-      std::vector<typename Cfg::Tile> thr(Cfg::THREADS);
-      const long groups = (batch + Cfg::C - 1) / Cfg::C;
-      for (long g = 0; g < groups; ++g) {
-        for (int t = 0; t < Cfg::THREADS; ++t) Body::phase1(thr[t], a, g, t, smem.data(), twa.data());
-        for (int t = 0; t < Cfg::THREADS; ++t) Body::phase2(thr[t], a, g, t, smem.data());
-      }
+      run_body<Body, typename Cfg::Tile, typename Cfg::Lay>({x.data(), out.data(), twa.data(), batch, (T)0.5, 1},
+                                                            (batch + Cfg::C - 1) / Cfg::C, twa.data());
       report_conflicts<typename Cfg::Tile, typename Cfg::Lay, true, true>("exchange");
     };
     if (fwd) run(onchip::OnChipCfg<T, RA, RB, E, WARPS, true>{}); else run(onchip::OnChipCfg<T, RA, RB, E, WARPS, false>{});

@@ -5,68 +5,13 @@
 //     batch of 5 and a batch that is not a multiple of the rows per CTA, starting at spectrum row 0 and 2;
 //   * real::conv_pair alone (the half-length path's conv_pair_kernel), for even and odd M = N/2.
 // H is the rfft of random real taps h, with random imaginary parts added to bins 0 and N/2 (they must not count).
-// Every spectrum access goes through FB_SPEC_ACCESS, which records its address and width: the check fails on any
-// access wider than one complex value, misaligned, or outside H, and when no odd row of H (8 bytes off a 16-byte
-// boundary for f32) was read.  It also reports the bank-conflict degree of the pair step's write-back into the park
-// and of the stage-A reads of Z' from it.
+// Every spectrum access goes through FB_SPEC_ACCESS, which records its address and width (emulate_common.h): the
+// check fails on any access wider than one complex value, misaligned, or outside H, and when no odd row of H (8 bytes
+// off a 16-byte boundary for f32) was read.  It also reports the bank-conflict degree of the pair step's write-back
+// into the park and of the stage-A reads of Z' from it.
 // Build: nvcc -std=c++17 -O1 --expt-relaxed-constexpr -I fourier_b200/csrc tools/emulate_conv.cu \
 //             fourier_b200/csrc/host_math.cu (host only, never run on the device)
-#include <algorithm>
-#include <cmath>
-#include <cstdint>
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
-
-static void spec_record(const void* p, int bytes);
-#ifdef __CUDA_ARCH__
-#define FB_SPEC_ACCESS(p, bytes)
-#else
-#define FB_SPEC_ACCESS(p, bytes) spec_record((const void*)(p), (int)(bytes))
-#endif
-
-#include "onchip_kernels.cuh"
-#include "plan.h"
-#include "tables.cuh"
-
-using namespace fb200;
-
-// ---- spectrum access log ------------------------------------------------------------------------------------------
-struct Access { uintptr_t addr; int bytes; };
-static std::vector<Access> g_access;
-__attribute__((unused)) static void spec_record(const void* p, int bytes) { g_access.push_back({(uintptr_t)p, bytes}); }
-
-// Checks the log against H = [base, base + rows * row_bytes): every access inside it, aligned to its width, at most
-// `widest_allowed` bytes wide, and some at odd rows.  Prints one line; returns the number of failures.
-static int check_access(const void* base, size_t rows, size_t row_bytes, int widest_allowed) {
-  size_t odd = 0, outside = 0, misaligned = 0;
-  int widest = 0;
-  const uintptr_t b = (uintptr_t)base;
-  for (const Access& a : g_access) {
-    widest = std::max(widest, a.bytes);
-    if (a.addr < b || a.addr + a.bytes > b + rows * row_bytes) { ++outside; continue; }
-    if (a.addr % a.bytes) ++misaligned;
-    if (((a.addr - b) / row_bytes) % 2 == 1) ++odd;
-  }
-  const bool ok = !g_access.empty() && widest <= widest_allowed && !outside && !misaligned && odd > 0;
-  printf("  H accesses: %zu (%zu at odd rows), widest %d B, misaligned %zu, outside %zu %s\n", g_access.size(), odd,
-         widest, misaligned, outside, ok ? "OK" : "FAIL");
-  g_access.clear();
-  return !ok;
-}
-
-// 16-byte aligned storage (what cudaMalloc gives), so that the row offsets are the ones a device buffer would have
-template <typename V> struct Buf {
-  std::vector<double2> raw;
-  V* p;
-  explicit Buf(size_t n) : raw((n * sizeof(V) + 15) / 16 + 1), p(reinterpret_cast<V*>(raw.data())) {}
-  V& operator[](size_t i) { return p[i]; }
-};
-
-static double rnd(unsigned long long& s) {
-  s = s * 6364136223846793005ull + 1442695040888963407ull;
-  return (double)(s >> 11) / 9007199254740992.0 * 2 - 1;
-}
+#include "emulate_common.h"
 
 // F rows of taps h (double) and their spectra H = rfft(h) rounded to T, bins 0 and N/2 (N even) with random
 // imaginary parts
@@ -107,34 +52,6 @@ static double conv_err(const std::vector<double>& x, const std::vector<double>& 
   return worst;
 }
 
-// degree of one warp-wide shared access (lanes served in groups of 128 bytes; identical addresses broadcast;
-// inactive lanes < 0)
-template <int B> static int conflict_degree(const std::vector<long>& idx) {
-  const int group = 128 / B;
-  int worst = 1;
-  for (size_t g = 0; g + group <= idx.size(); g += group) {
-    int count[32] = {0};
-    std::vector<long> seen;
-    for (int l = 0; l < group; ++l) {
-      const long e = idx[g + l];
-      if (e < 0 || std::find(seen.begin(), seen.end(), e) != seen.end()) continue;
-      seen.push_back(e);
-      worst = std::max(worst, ++count[(int)((e * B / 4) % 32)]);
-    }
-  }
-  return worst;
-}
-
-template <typename T> static std::vector<cpx<T>> pair_table(long m) {
-  std::vector<cpx<T>> tab(m / 2 + 1);
-  for (long k = 0; k <= m / 2; ++k) {
-    double re, im;
-    host_twiddle((size_t)k, (size_t)(2 * m), &re, &im);
-    tab[k] = mk<T>((T)re, (T)im);
-  }
-  return tab;
-}
-
 // ---- fused on-chip conv kernel --------------------------------------------------------------------------------------
 template <typename T, int RA, int RB, int E, int WARPS>
 static int check_fused(const char* name, double tol) {
@@ -155,25 +72,15 @@ static int check_fused(const char* name, double tol) {
       Buf<T> x(N * batch), y(N * batch);
       std::vector<double> xd(N * batch), yd(N * batch);
       for (long i = 0; i < N * batch; ++i) { x[i] = (T)rnd(seed); xd[i] = x[i]; y[i] = (T)NAN; }
-      const typename Body::Args a = {reinterpret_cast<const V*>(x.p), reinterpret_cast<V*>(y.p), twa.data(), tab.data(),
-                                     H.p, rows, row0, batch, (T)(1.0 / (2 * N))};
-      std::vector<V> smem(Tile::template smem_elems<typename Cfg::Lay>());
-      std::vector<Tile> thr(Cfg::THREADS);
-      for (long g = 0; g < (batch + Cfg::C - 1) / Cfg::C; ++g) {
-        for (int t = 0; t < Cfg::THREADS; ++t) Body::fwd_phase1(thr[t], a, g, t, smem.data(), twa.data());
-        for (int t = 0; t < Cfg::THREADS; ++t) Body::Real::fwd_gather(thr[t], t, smem.data());
-        for (int t = 0; t < Cfg::THREADS; ++t) Body::Real::fwd_park(thr[t], t, smem.data());
-        for (int t = 0; t < Cfg::THREADS; ++t) Body::pairs(a, g, t, smem.data());
-        for (int t = 0; t < Cfg::THREADS; ++t) Body::inv_stage_a(thr[t], t, smem.data(), twa.data());
-        for (int t = 0; t < Cfg::THREADS; ++t) Body::inv_scatter(thr[t], t, smem.data());
-        for (int t = 0; t < Cfg::THREADS; ++t) Body::inv_store(thr[t], a, g, t, smem.data());
-      }
+      run_body<Body, Tile, typename Cfg::Lay>({reinterpret_cast<const V*>(x.p), reinterpret_cast<V*>(y.p), twa.data(),
+                                               tab.data(), H.p, rows, row0, batch, (T)(1.0 / (2 * N))},
+                                              (batch + Cfg::C - 1) / Cfg::C, twa.data());
       for (long i = 0; i < N * batch; ++i) yd[i] = y[i];
       const double worst = conv_err(xd, h, yd, N, batch, rows, row0);
       printf("%s N=%ld F=%ld batch=%ld row0=%ld: max rel err vs direct circular convolution %.3e %s\n", name, N, rows,
              batch, row0, worst, worst < tol ? "OK" : "FAIL");
       bad += !(worst < tol);
-      bad += check_access(H.p, rows, (L + 1) * sizeof(V), (int)sizeof(V));
+      bad += check_access("H", H.p, rows, (L + 1) * sizeof(V), (int)sizeof(V));
     }
   }
   // bank conflicts: the pair step writes z[k] ascending and z[L-k] descending back into the park; the inverse reads
@@ -212,40 +119,20 @@ static int check_pair(const char* name, long m, double tol) {
   const long n = 2 * m, batch = 5, rows = 3, row0 = 1;
   const auto tab = pair_table<T>(m);
   unsigned long long seed = 5151 + m;
-  std::vector<double> h, x(n * batch), y(n * batch);
+  std::vector<double> h, x(n * batch);
   Buf<V> H(rows * (m + 1));
   make_filters<T>(n, rows, seed, h, H);
   for (auto& v : x) v = (T)rnd(seed);
-  std::vector<double> wr(m), wi(m);
-  for (long j = 0; j < m; ++j) host_twiddle((size_t)j, (size_t)m, &wr[j], &wi[j]);
-  std::vector<V> z(m * batch);
-  for (long b = 0; b < batch; ++b)
-    for (long k = 0; k < m; ++k) {
-      double a = 0, c = 0;
-      for (long j = 0; j < m; ++j) {
-        const double zr = x[b * n + 2 * j], zi = x[b * n + 2 * j + 1], tr = wr[(k * j) % m], ti = wi[(k * j) % m];
-        a += zr * tr - zi * ti; c += zr * ti + zi * tr;
-      }
-      z[b * m + k] = mk<T>((T)a, (T)c);
-    }
+  std::vector<V> z = packed_fft<T>(x, m, batch);
   for (long b = 0; b < batch; ++b)
     for (long k = 0; k <= m / 2; ++k)
       real::conv_pair(z.data() + b * m, H.p + ((row0 + b) % rows) * (m + 1), m, k, tab.data(), (T)(1.0 / (2 * n)));
-  for (long b = 0; b < batch; ++b)   // unscaled inverse FFT_M in double, interleaved
-    for (long j = 0; j < m; ++j) {
-      double a = 0, c = 0;
-      for (long k = 0; k < m; ++k) {
-        const V v = z[b * m + k];
-        const double tr = wr[(k * j) % m], ti = -wi[(k * j) % m];
-        a += v.x * tr - v.y * ti; c += v.x * ti + v.y * tr;
-      }
-      y[b * n + 2 * j] = a; y[b * n + 2 * j + 1] = c;
-    }
+  const std::vector<double> y = packed_ifft<T>(z, m, batch);   // unscaled inverse, interleaved
   const double worst = conv_err(x, h, y, n, batch, rows, row0);
   printf("%s conv_pair N=%ld (M=%ld): max rel err vs direct circular convolution %.3e %s\n", name, n, m, worst,
          worst < tol ? "OK" : "FAIL");
   int bad = !(worst < tol);
-  bad += check_access(H.p, rows, (m + 1) * sizeof(V), (int)sizeof(V));
+  bad += check_access("H", H.p, rows, (m + 1) * sizeof(V), (int)sizeof(V));
   return bad;
 }
 

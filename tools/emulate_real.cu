@@ -3,74 +3,13 @@
 // DFT:
 //   * the fused on-chip real kernel, forward and inverse, for every on-chip size class of both precisions;
 //   * the untangle / tangle steps of the half-length path, for even and odd M = N/2.
-// Every spectrum access goes through FB_SPEC_ACCESS, which records its address and width here: the check fails on
-// any access wider than one complex value or not aligned to its width (f32 spectrum rows of odd index start 8 bytes
-// off a 16-byte boundary).  It also reports the bank-conflict degree of the forward kernel's natural-order park and
-// of the untangle's ascending / descending reads.
+// Every spectrum access goes through FB_SPEC_ACCESS, which records its address and width (emulate_common.h): the
+// check fails on any access wider than one complex value or not aligned to its width (f32 spectrum rows of odd index
+// start 8 bytes off a 16-byte boundary).  It also reports the bank-conflict degree of the forward kernel's
+// natural-order park and of the untangle's ascending / descending reads.
 // Build: nvcc -std=c++17 -O1 --expt-relaxed-constexpr -I fourier_b200/csrc tools/emulate_real.cu \
 //             fourier_b200/csrc/host_math.cu (host only, never run on the device)
-#include <algorithm>
-#include <cmath>
-#include <cstdint>
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
-
-static void spec_record(const void* p, int bytes);
-#ifdef __CUDA_ARCH__
-#define FB_SPEC_ACCESS(p, bytes)
-#else
-#define FB_SPEC_ACCESS(p, bytes) spec_record((const void*)(p), (int)(bytes))
-#endif
-
-#include "onchip_kernels.cuh"
-#include "plan.h"
-#include "tables.cuh"
-
-using namespace fb200;
-
-// ---- spectrum access log ------------------------------------------------------------------------------------------
-struct Access { uintptr_t addr; int bytes; };
-static std::vector<Access> g_access;
-__attribute__((unused)) static void spec_record(const void* p, int bytes) { g_access.push_back({(uintptr_t)p, bytes}); }
-
-// Checks the log against the spectrum buffer [base, base + rows * row_bytes): every access inside it, aligned to its
-// width, at most `widest_allowed` bytes wide.  Prints one line; returns the number of failures.
-static int check_access(const char* name, const void* base, size_t rows, size_t row_bytes, int widest_allowed) {
-  size_t odd = 0, outside = 0, misaligned = 0;
-  int widest = 0;
-  const uintptr_t b = (uintptr_t)base;
-  for (const Access& a : g_access) {
-    widest = std::max(widest, a.bytes);
-    if (a.addr < b || a.addr + a.bytes > b + rows * row_bytes) { ++outside; continue; }
-    if (a.addr % a.bytes) ++misaligned;
-    if (((a.addr - b) / row_bytes) % 2 == 1) ++odd;
-  }
-  const bool ok = !g_access.empty() && widest <= widest_allowed && !outside && !misaligned && (rows < 2 || odd > 0);
-  printf("  %s spectrum accesses: %zu (%zu at odd rows), widest %d B, misaligned %zu, outside %zu %s\n", name,
-         g_access.size(), odd, widest, misaligned, outside, ok ? "OK" : "FAIL");
-  g_access.clear();
-  return !ok;
-}
-
-// 16-byte aligned storage (what cudaMalloc gives), so that the row offsets are the ones a device buffer would have
-template <typename V> struct Buf {
-  std::vector<double2> raw;
-  V* p;
-  explicit Buf(size_t n) : raw((n * sizeof(V) + 15) / 16 + 1), p(reinterpret_cast<V*>(raw.data())) {}
-  V& operator[](size_t i) { return p[i]; }
-};
-
-static double rnd(unsigned long long& s) {
-  s = s * 6364136223846793005ull + 1442695040888963407ull;
-  return (double)(s >> 11) / 9007199254740992.0 * 2 - 1;
-}
-
-// w[j] = exp(-2 pi i j / n)
-static void twiddles(long n, std::vector<double>& wr, std::vector<double>& wi) {
-  wr.resize(n); wi.resize(n);
-  for (long j = 0; j < n; ++j) host_twiddle((size_t)j, (size_t)n, &wr[j], &wi[j]);
-}
+#include "emulate_common.h"
 
 // numpy.fft.rfft of the reals x[0 .. n) times s, in double
 static void ref_rfft(const double* x, long n, double s, std::vector<double>& re, std::vector<double>& im) {
@@ -107,24 +46,6 @@ static double rel(const std::vector<double>& got, const std::vector<double>& ref
   return std::isnan(e) ? INFINITY : e / r;
 }
 
-// degree of one warp-wide shared access (lanes served in groups of 128 bytes; identical addresses broadcast;
-// inactive lanes < 0)
-template <int B> static int conflict_degree(const std::vector<long>& idx) {
-  const int group = 128 / B;
-  int worst = 1;
-  for (size_t g = 0; g + group <= idx.size(); g += group) {
-    int count[32] = {0};
-    std::vector<long> seen;
-    for (int l = 0; l < group; ++l) {
-      const long e = idx[g + l];
-      if (e < 0 || std::find(seen.begin(), seen.end(), e) != seen.end()) continue;
-      seen.push_back(e);
-      worst = std::max(worst, ++count[(int)((e * B / 4) % 32)]);
-    }
-  }
-  return worst;
-}
-
 // ---- fused on-chip real kernel ------------------------------------------------------------------------------------
 template <typename T, int RA, int RB, int E, int WARPS>
 static int check_fused(const char* name, double tol) {
@@ -133,12 +54,7 @@ static int check_fused(const char* name, double tol) {
   const double s = 0.5;
   int bad = 0;
   auto twa = twopass::make_twa<T>(RA, RB);
-  std::vector<V> tab(L / 2 + 1);
-  for (long k = 0; k <= L / 2; ++k) {
-    double re, im;
-    host_twiddle((size_t)k, (size_t)N, &re, &im);
-    tab[k] = mk<T>((T)re, (T)im);
-  }
+  const auto tab = pair_table<T>(L);
   unsigned long long seed = 977 + L;
   {  // forward
     using Cfg = onchip::OnChipCfg<T, RA, RB, E, WARPS, true>;
@@ -147,15 +63,9 @@ static int check_fused(const char* name, double tol) {
     for (long i = 0; i < N * batch; ++i) x[i] = (T)rnd(seed);
     Buf<V> out((L + 1) * batch);
     for (long i = 0; i < (L + 1) * batch; ++i) out[i] = mk<T>((T)NAN, (T)NAN);
-    const typename Body::Args a = {reinterpret_cast<const V*>(x.p), out.p, twa.data(), tab.data(), batch, (T)(s / 2)};
-    std::vector<V> smem(Cfg::Tile::template smem_elems<typename Cfg::Lay>());
-    std::vector<typename Cfg::Tile> thr(Cfg::THREADS);
-    for (long g = 0; g < (batch + Cfg::C - 1) / Cfg::C; ++g) {
-      for (int t = 0; t < Cfg::THREADS; ++t) Body::fwd_phase1(thr[t], a, g, t, smem.data(), twa.data());
-      for (int t = 0; t < Cfg::THREADS; ++t) Body::fwd_gather(thr[t], t, smem.data());
-      for (int t = 0; t < Cfg::THREADS; ++t) Body::fwd_park(thr[t], t, smem.data());
-      for (int t = 0; t < Cfg::THREADS; ++t) Body::fwd_store(a, g, t, smem.data());
-    }
+    run_body<Body, typename Cfg::Tile, typename Cfg::Lay>(
+        {reinterpret_cast<const V*>(x.p), out.p, twa.data(), tab.data(), batch, (T)(s / 2)}, (batch + Cfg::C - 1) / Cfg::C,
+        twa.data());
     double worst = 0;
     bool zero_imag = true;
     for (long b = 0; b < batch; ++b) {
@@ -172,7 +82,7 @@ static int check_fused(const char* name, double tol) {
     printf("%s N=%ld forward: max rel err vs f64 DFT %.3e, Im X[0], Im X[N/2] == +0: %s %s\n", name, N, worst,
            zero_imag ? "yes" : "no", worst < tol && zero_imag ? "OK" : "FAIL");
     bad += !(worst < tol && zero_imag);
-    bad += check_access("forward", out.p, batch, (L + 1) * sizeof(V), (int)sizeof(V));
+    bad += check_access("forward spectrum", out.p, batch, (L + 1) * sizeof(V), (int)sizeof(V));
 
     // bank conflicts: natural-order park (write), untangle reads z[k] ascending and z[L-k] descending
     using Tile = typename Cfg::Tile;
@@ -207,13 +117,9 @@ static int check_fused(const char* name, double tol) {
     for (long i = 0; i < (L + 1) * batch; ++i) x[i] = mk<T>((T)rnd(seed), (T)rnd(seed));
     Buf<T> y(N * batch);
     for (long i = 0; i < N * batch; ++i) y[i] = (T)NAN;
-    const typename Body::Args a = {x.p, reinterpret_cast<V*>(y.p), twa.data(), tab.data(), batch, (T)(1.0 / N)};
-    std::vector<V> smem(Cfg::Tile::template smem_elems<typename Cfg::Lay>());
-    std::vector<typename Cfg::Tile> thr(Cfg::THREADS);
-    for (long g = 0; g < (batch + Cfg::C - 1) / Cfg::C; ++g) {
-      for (int t = 0; t < Cfg::THREADS; ++t) Body::inv_phase1(thr[t], a, g, t, smem.data(), twa.data());
-      for (int t = 0; t < Cfg::THREADS; ++t) Body::inv_phase2(thr[t], a, g, t, smem.data());
-    }
+    run_body<Body, typename Cfg::Tile, typename Cfg::Lay>(
+        {x.p, reinterpret_cast<V*>(y.p), twa.data(), tab.data(), batch, (T)(1.0 / N)}, (batch + Cfg::C - 1) / Cfg::C,
+        twa.data());
     double worst = 0;
     for (long b = 0; b < batch; ++b) {
       std::vector<double> xr(L + 1), xi(L + 1), got(N), ref;
@@ -224,7 +130,7 @@ static int check_fused(const char* name, double tol) {
     }
     printf("%s N=%ld inverse: max rel err vs f64 DFT %.3e %s\n", name, N, worst, worst < tol ? "OK" : "FAIL");
     bad += !(worst < tol);
-    bad += check_access("inverse", x.p, batch, (L + 1) * sizeof(V), (int)sizeof(V));
+    bad += check_access("inverse spectrum", x.p, batch, (L + 1) * sizeof(V), (int)sizeof(V));
   }
   return bad;
 }
@@ -235,29 +141,13 @@ static int check_steps(const char* name, long m, double tol) {
   using V = cpx<T>;
   const long n = 2 * m, batch = 3;
   const double s = 1.0 / std::sqrt((double)n);   // SqrtScaledFft / SqrtScaledIfft
-  std::vector<V> tab(m / 2 + 1);
-  for (long k = 0; k <= m / 2; ++k) {
-    double re, im;
-    host_twiddle((size_t)k, (size_t)n, &re, &im);
-    tab[k] = mk<T>((T)re, (T)im);
-  }
-  std::vector<double> wr, wi;
-  twiddles(m, wr, wi);
+  const auto tab = pair_table<T>(m);
   unsigned long long seed = 4242 + m;
   int bad = 0;
   {  // forward: Z = FFT_M(z) in double, rounded to T; untangle; compare with rfft
     std::vector<double> x(n * batch);
     for (auto& v : x) v = (T)rnd(seed);
-    std::vector<V> z(m * batch);
-    for (long b = 0; b < batch; ++b)
-      for (long k = 0; k < m; ++k) {
-        double a = 0, c = 0;
-        for (long j = 0; j < m; ++j) {
-          const double zr = x[b * n + 2 * j], zi = x[b * n + 2 * j + 1], tr = wr[(k * j) % m], ti = wi[(k * j) % m];
-          a += zr * tr - zi * ti; c += zr * ti + zi * tr;
-        }
-        z[b * m + k] = mk<T>((T)a, (T)c);
-      }
+    std::vector<V> z = packed_fft<T>(x, m, batch);
     Buf<V> out((m + 1) * batch);
     for (long i = 0; i < (m + 1) * batch; ++i) out[i] = mk<T>((T)NAN, (T)NAN);
     for (long b = 0; b < batch; ++b)
@@ -277,7 +167,7 @@ static int check_steps(const char* name, long m, double tol) {
     printf("%s untangle N=%ld (M=%ld): max rel err vs f64 DFT %.3e, Im X[0], Im X[N/2] == +0: %s %s\n", name, n, m,
            worst, zero_imag ? "yes" : "no", worst < tol && zero_imag ? "OK" : "FAIL");
     bad += !(worst < tol && zero_imag);
-    bad += check_access("untangle", out.p, batch, (m + 1) * sizeof(V), (int)sizeof(V));
+    bad += check_access("untangle spectrum", out.p, batch, (m + 1) * sizeof(V), (int)sizeof(V));
   }
   {  // inverse: tangle; unscaled IFFT_M in double; compare with irfft (random imaginary parts in bins 0 and M)
     Buf<V> x((m + 1) * batch);
@@ -285,25 +175,17 @@ static int check_steps(const char* name, long m, double tol) {
     std::vector<V> z(m * batch, mk<T>((T)NAN, (T)NAN));
     for (long b = 0; b < batch; ++b)
       for (long k = 0; k <= m / 2; ++k) real::tangle(x.p + b * (m + 1), z.data() + b * m, m, k, tab.data(), (T)s);
+    const std::vector<double> y = packed_ifft<T>(z, m, batch);
     double worst = 0;
     for (long b = 0; b < batch; ++b) {
-      std::vector<double> got(n), ref, xr(m + 1), xi(m + 1);
-      for (long j = 0; j < m; ++j) {
-        double a = 0, c = 0;
-        for (long k = 0; k < m; ++k) {
-          const V v = z[b * m + k];
-          const double tr = wr[(k * j) % m], ti = -wi[(k * j) % m];
-          a += v.x * tr - v.y * ti; c += v.x * ti + v.y * tr;
-        }
-        got[2 * j] = a; got[2 * j + 1] = c;
-      }
+      std::vector<double> got(y.begin() + b * n, y.begin() + (b + 1) * n), ref, xr(m + 1), xi(m + 1);
       for (long k = 0; k <= m; ++k) { xr[k] = x[b * (m + 1) + k].x; xi[k] = x[b * (m + 1) + k].y; }
       ref_irfft(xr.data(), xi.data(), n, s, ref);
       worst = std::max(worst, rel(got, ref));
     }
     printf("%s tangle N=%ld (M=%ld): max rel err vs f64 DFT %.3e %s\n", name, n, m, worst, worst < tol ? "OK" : "FAIL");
     bad += !(worst < tol);
-    bad += check_access("tangle", x.p, batch, (m + 1) * sizeof(V), (int)sizeof(V));
+    bad += check_access("tangle spectrum", x.p, batch, (m + 1) * sizeof(V), (int)sizeof(V));
   }
   return bad;
 }
