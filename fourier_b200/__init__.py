@@ -15,6 +15,9 @@ reference's operator interface name for name:
                                                             batched rfft / irfft of real rows
     (no counterpart)                                      RealFft.convolve: y = irfft(rfft(x) * H) of real
                                                             rows, one or several spectra H, one call
+    (no counterpart)                                      RealFft.convolve_linear: linear convolution of real
+                                                            rows of any length with K <= N taps (scipy's
+                                                            full / same / valid), overlap-save in one call
 
 Buffers are numpy arrays (host memory: staged over PCIe by the library) or torch CUDA tensors
 (device memory: transformed in HBM on torch's current stream).  A leading batch dimension is
@@ -203,7 +206,7 @@ def create_fft_f64(size, general=False):
 class RealFft:
     """A plan for real-input transforms of one length N (numpy's rfft / irfft, batched): reals of shape (..., N) and
     spectra of shape (..., N//2+1), with equal leading dimensions.  rfft / irfft are out of place only; convolve
-    (irfft(rfft(x) * H) in one call) may run in place."""
+    (irfft(rfft(x) * H) in one call) may run in place; convolve_linear filters rows of any length, out of place."""
 
     def __init__(self, size, real):
         if real not in ("f32", "f64"):
@@ -244,9 +247,11 @@ class RealFft:
         """The real kernel of the plan, and for the half-length and full-length paths the inner plan's kernel."""
         return getattr(_lib.load(), f"fourier_b200_rfft_kernel_{self._t}")(self._plan).decode()
 
-    def _describe(self, x, kind):
-        """kind 'real' (last dimension N) or 'spec' (N//2+1) -> (pointer, leading shape, is_device, stream)"""
-        last = self._size if kind == "real" else self._size // 2 + 1
+    def _describe(self, x, kind, last=None):
+        """kind 'real' (last dimension N, or `last`) or 'spec' (N//2+1) -> (pointer, leading shape, is_device,
+        stream)"""
+        if last is None:
+            last = self._size if kind == "real" else self._size // 2 + 1
         if _is_torch(x):
             import torch
             want = {("real", "f32"): torch.float32, ("real", "f64"): torch.float64,
@@ -319,6 +324,55 @@ class RealFft:
             rc = getattr(L, f"fourier_b200_convolve_real_{self._t}")(self._plan, pi, ps, rows, po, batch)
         if rc != 0:
             raise RuntimeError(f"real convolution failed (cuda error {rc}): {_lib.last_error()}")
+
+    LINEAR_MODES = {"full": 0, "same": 1, "valid": 2}
+
+    def convolve_linear(self, input, spectrum, taps, output, mode="full"):
+        """output = scipy.signal.convolve(input, h, mode) for every row of `input` (shape (..., L), any L >= 1), where
+        `spectrum` (shape (..., N//2+1), this plan's rfft layout) is rfft(h, n=N) of `taps` = K <= N taps h.  `output`
+        has shape (..., out_len): out_len = L + K - 1 (mode "full"), L ("same") or L - K + 1 ("valid", L >= K).  The
+        spectrum broadcasts over the input's leading shape as in convolve.  Rows are filtered by overlap-save in
+        segments of N - K + 1 outputs, so N should be a few times K.  If irfft(spectrum) has non-zero samples beyond
+        the first K, the result is unspecified.  Out of place only; correlation: pass conj(H), resolved."""
+        for x in (input, spectrum, output):
+            if _is_torch(x) and (x.is_conj() or x.is_neg()):
+                raise ValueError("torch tensors with the conj or neg bit set hold unconjugated data: "
+                                 "pass x.resolve_conj() (and resolve_neg()) instead")
+        if mode not in self.LINEAR_MODES:
+            raise ValueError(f"mode must be one of {sorted(self.LINEAR_MODES)}, got {mode!r}")
+        taps = int(taps)
+        if not 1 <= taps <= self._size:
+            raise ValueError(f"taps must be in [1, {self._size}], got {taps}")
+        in_len = input.shape[-1] if getattr(input, "ndim", 0) > 0 else 0
+        if in_len < 1:
+            raise ValueError("input rows must hold at least one sample")
+        if mode == "valid" and in_len < taps:
+            raise ValueError(f"mode 'valid' needs rows of at least taps = {taps} samples, got {in_len}")
+        out_len = {"full": in_len + taps - 1, "same": in_len, "valid": in_len - taps + 1}[mode]
+        pi, li, di, si = self._describe(input, "real", last=in_len)
+        ps, ls, ds, _ = self._describe(spectrum, "spec")
+        if getattr(output, "ndim", 0) == 0 or output.shape[-1] != out_len:
+            raise ValueError(f"output rows must hold out_len = {out_len} samples for mode {mode!r} "
+                             f"(L = {in_len}, taps = {taps})")
+        po, lo, do_, _ = self._describe(output, "real", last=out_len)
+        if li != lo:
+            raise ValueError(f"input and output leading shapes differ: {li} and {lo}")
+        if len(ls) > len(li) or tuple(li[len(li) - len(ls):]) != ls:
+            raise ValueError(f"spectrum leading shape {ls} is not a trailing part of the input's {li}")
+        if not (di == ds == do_):
+            raise ValueError("input, spectrum and output must all be host or all be device buffers")
+        batch = int(np.prod(li, dtype=np.int64))
+        rows = int(np.prod(ls, dtype=np.int64))
+        code = self.LINEAR_MODES[mode]
+        L = _lib.load()
+        if di:
+            rc = getattr(L, f"fourier_b200_linear_convolve_real_async_{self._t}")(
+                self._plan, pi, in_len, ps, rows, taps, code, po, batch, si)
+        else:
+            rc = getattr(L, f"fourier_b200_linear_convolve_real_{self._t}")(
+                self._plan, pi, in_len, ps, rows, taps, code, po, batch)
+        if rc != 0:
+            raise RuntimeError(f"linear convolution failed (cuda error {rc}): {_lib.last_error()}")
 
     def rfft(self, input, output, transform=Transform.Fft):
         """output[..., :N//2+1] = numpy.fft.rfft(input) (Fft) or that times 1/sqrt(N) (SqrtScaledFft)."""

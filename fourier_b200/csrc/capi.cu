@@ -211,6 +211,53 @@ int convolve_exec(void* plan, const T* in, const void* spectrum, size_t rows, T*
   }
 }
 
+// Linear convolution of real rows by overlap-save: out of place only; scalar arguments are checked before the plan is
+// touched, even for batch == 0.
+template <typename T>
+int linear_exec(void* plan, const T* in, size_t in_len, const void* spectrum, size_t rows, size_t taps, int mode, T* out,
+                size_t batch, bool async, void* stream) {
+  if (!plan || !in || !out || !spectrum) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
+  const char* bad = rows == 0                                      ? "spectrum_rows must be at least 1"
+                    : taps == 0                                    ? "taps must be at least 1"
+                    : in_len == 0                                  ? "in_len must be at least 1"
+                    : mode < 0 || mode > 2                         ? "unknown mode (FOURIER_B200_LINEAR_FULL, _SAME or _VALID)"
+                    : mode == fb200::real::kLinearValid && in_len < taps ? "mode valid needs in_len >= taps"
+                                                                   : nullptr;
+  if (bad) { fb200::set_last_error(bad); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  using C = typename RealPlan<T>::C;
+  const C* spec = static_cast<const C*>(spectrum);
+  if (taps > p->size()) { fb200::set_last_error("taps must not exceed the plan length N"); return (int)cudaErrorInvalidValue; }
+  try {
+    if (batch == 0) return (int)p->linear_convolve_device(in, in_len, spec, rows, taps, mode, out, 0, nullptr);
+    const size_t in_bytes = batch * in_len * sizeof(T);
+    const size_t out_bytes = batch * (size_t)fb200::real::linear_out_len(mode, (long)in_len, (long)taps) * sizeof(T);
+    if (ranges_meet(in, in_bytes, out, out_bytes)) {
+      fb200::set_last_error("input and output overlap (linear convolution is out of place only)");
+      return (int)cudaErrorInvalidValue;
+    }
+    if (ranges_meet(spectrum, p->spec_bytes(rows), out, out_bytes)) {
+      fb200::set_last_error("spectrum and output overlap");
+      return (int)cudaErrorInvalidValue;
+    }
+    if (!async) {
+      const int dev =
+          residence({in, spectrum, out}, "input, spectrum and output must all be host or all be device memory");
+      if (dev < 0) return (int)cudaErrorInvalidValue;
+      if (!dev) return (int)p->linear_convolve_host(in, in_len, spec, rows, taps, mode, out, batch);
+    }
+    if (!device_pointers_aligned(in, out) || !device_pointers_aligned(spectrum, spectrum))
+      return (int)cudaErrorMisalignedAddress;
+    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
+    cudaError_t e = p->linear_convolve_device(in, in_len, spec, rows, taps, mode, out, batch, s);
+    if (e != cudaSuccess || async) return (int)e;
+    return (int)cudaStreamSynchronize(s);
+  } catch (...) {
+    fb200::set_last_error("linear convolution threw");
+    return (int)cudaErrorUnknown;
+  }
+}
+
 }  // namespace
 
 using fourier::c::fourier_fft_double;
@@ -447,6 +494,28 @@ int fourier_b200_convolve_real_async_double(fourier_b200_rfft_double* plan, cons
                                             const void* spectrum_dev, size_t spectrum_rows, double* out_dev,
                                             size_t batch, void* stream) {
   return convolve_exec<double>(plan, in_dev, spectrum_dev, spectrum_rows, out_dev, batch, true, stream);
+}
+
+int fourier_b200_linear_convolve_real_float(fourier_b200_rfft_float* plan, const float* in, size_t in_len,
+                                            const void* spectrum, size_t spectrum_rows, size_t taps, int mode,
+                                            float* out, size_t batch) {
+  return linear_exec<float>(plan, in, in_len, spectrum, spectrum_rows, taps, mode, out, batch, false, nullptr);
+}
+int fourier_b200_linear_convolve_real_double(fourier_b200_rfft_double* plan, const double* in, size_t in_len,
+                                             const void* spectrum, size_t spectrum_rows, size_t taps, int mode,
+                                             double* out, size_t batch) {
+  return linear_exec<double>(plan, in, in_len, spectrum, spectrum_rows, taps, mode, out, batch, false, nullptr);
+}
+int fourier_b200_linear_convolve_real_async_float(fourier_b200_rfft_float* plan, const float* in_dev, size_t in_len,
+                                                  const void* spectrum_dev, size_t spectrum_rows, size_t taps, int mode,
+                                                  float* out_dev, size_t batch, void* stream) {
+  return linear_exec<float>(plan, in_dev, in_len, spectrum_dev, spectrum_rows, taps, mode, out_dev, batch, true, stream);
+}
+int fourier_b200_linear_convolve_real_async_double(fourier_b200_rfft_double* plan, const double* in_dev, size_t in_len,
+                                                   const void* spectrum_dev, size_t spectrum_rows, size_t taps,
+                                                   int mode, double* out_dev, size_t batch, void* stream) {
+  return linear_exec<double>(plan, in_dev, in_len, spectrum_dev, spectrum_rows, taps, mode, out_dev, batch, true,
+                             stream);
 }
 
 const char* fourier_b200_last_error(void) { return fb200::last_error(); }

@@ -87,13 +87,25 @@ struct OnChipImpl {
     cudaError_t e;
     if ((e = allow_smem(onchip::onchip_real_kernel<Cfg<true>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_real_kernel<Cfg<false>, MINB>))) return e;
-    return allow_smem(onchip::onchip_conv_kernel<Cfg<true>, MINB>);
+    if ((e = allow_smem(onchip::onchip_conv_kernel<Cfg<true>, MINB>))) return e;
+    return allow_smem(onchip::onchip_lconv_kernel<Cfg<true>, MINB>);
   }
   static cudaError_t conv(const void* in, void* out, const void* twa, const cpx<T>* tab, const cpx<T>* spec,
-                          size_t rows, size_t row0, size_t batch, T h, int sms, cudaStream_t s) {
+                          size_t rows, size_t row0, size_t per, size_t batch, T h, int sms, cudaStream_t s) {
     return launch(onchip::onchip_conv_kernel<Cfg<true>, MINB>,
-                  {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab, spec, (long)rows, (long)row0, (long)batch, h},
+                  {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab, spec, (long)rows, (long)row0, (long)batch, h,
+                   (long)per},
                   batch, sms, s);
+  }
+  static cudaError_t lconv(const T* in, T* out, const real::SegMap& m, size_t nseg, const void* twa, const cpx<T>* tab,
+                           const cpx<T>* spec, size_t rows, T h, int sms, cudaStream_t s) {
+    typename onchip::LinConvBody<Cfg<true>>::Args a;
+    static_cast<typename onchip::ConvBody<Cfg<true>>::Args&>(a) = {
+        nullptr, nullptr, (const TwPair<T>*)twa, tab, spec, (long)rows, m.g0, (long)nseg, h, m.per};
+    a.x = in;
+    a.y = out;
+    a.m = m;
+    return launch(onchip::onchip_lconv_kernel<Cfg<true>, MINB>, a, nseg, sms, s);
   }
   static cudaError_t real(const void* in, void* out, const void* twa, const cpx<T>* tab, size_t batch, bool fwd, T h,
                           int sms, cudaStream_t s) {
@@ -104,7 +116,7 @@ struct OnChipImpl {
                   {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab, (long)batch, h}, batch, sms, s);
   }
   static const OnChipOps<T>* ops() {
-    static const RealOnChipOps<T> r = {RA, RB, &real_prepare, &real, &conv};
+    static const RealOnChipOps<T> r = {RA, RB, &real_prepare, &real, &conv, &lconv};
     static const OnChipOps<T> o = {RA, RB, &prepare, &fft, kHasBluestein ? &bluestein : nullptr, &r};
     return &o;
   }

@@ -6,7 +6,8 @@
 //                             one warp-private shared-memory exchange -> registers -> global.
 //   * onchip_real_kernel:     real-input transforms of length 2L (forward and inverse) on the same tiles.
 //   * onchip_conv_kernel:     y = irfft(rfft(x) . H) of real rows of length 2L, both transforms in one kernel.
-//     (these three run the phases of FftBody / RealBody / ConvBody through run_onchip_groups, tilefft.cuh)
+//   * onchip_lconv_kernel:    linear convolution of real rows of any length by overlap-save on the same phases.
+//     (these four run the phases of FftBody / RealBody / ConvBody / LinConvBody through run_onchip_groups, tilefft.cuh)
 //   * bluestein_fused_kernel: the whole chirp-z transform of the reference (bluesteins.rs:218-259) for
 //                             N <= L, M = 2L, in one kernel and without touching HBM in between.
 //
@@ -182,7 +183,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_real_kernel(const t
 // The forward phase is RealBody's: Z parked in natural order in the FFT's own exchange block.  Each lane then runs
 // real::conv_pair on the pairs it owns (k = u + TP*j, lane u = 0 also k = L/2), in place on the park.  The inverse
 // FFT of Z' runs on the same forward tile as conj(FFT(conj Z')), as bluestein_fused_kernel does: the stage-A reads
-// conjugate, and so does the store.  Row b uses spectrum row (row0 + b) mod rows.
+// conjugate, and so does the store.  Row b uses spectrum row ((row0 + b) / per) mod rows.
 template <class Cfg> struct ConvBody {
   using Tile = typename Cfg::Tile;   // FWD = true
   using V = typename Tile::V;
@@ -190,7 +191,9 @@ template <class Cfg> struct ConvBody {
   using Fft = FftBody<Cfg>;
   using Real = RealBody<Cfg>;
   static constexpr int L = Cfg::L, TP = Tile::TP, RA = Tile::RA, RB = Tile::RB, E = Tile::E;
-  struct Args { const V* in; V* out; const TwPair<T>* twa; const V* tab; const V* spec; long rows, row0, batch; T h; };
+  // per: rows of the batch per spectrum row step (the segments of one row, LinConvBody); 1 for circular convolution
+  struct Args { const V* in; V* out; const TwPair<T>* twa; const V* tab; const V* spec; long rows, row0, batch; T h;
+                long per = 1; };
 
   static FB_HD void fwd_phase1(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
     const typename Fft::Args fa = {a.in, nullptr, twa, a.batch, (T)1, 0};
@@ -202,7 +205,7 @@ template <class Cfg> struct ConvBody {
     const long b = grp * Cfg::C + Tile::template col_of<true>(t);
     if (b >= a.batch) return;
     V* z = smem + Real::park(t);
-    const V* hs = a.spec + ((a.row0 + b) % a.rows) * (L + 1);
+    const V* hs = a.spec + (((a.row0 + b) / a.per) % a.rows) * (L + 1);
 #pragma unroll 4
     for (int j = 0; j < E / 2; ++j) real::conv_pair(z, hs, (long)L, (long)(u + TP * j), a.tab, a.h);
     if (u == 0) real::conv_pair(z, hs, (long)L, (long)(L / 2), a.tab, a.h);
@@ -251,6 +254,76 @@ template <class Cfg> struct ConvBody {
 template <class Cfg, int MINB>
 __global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_conv_kernel(const typename ConvBody<Cfg>::Args a) {
   run_onchip_groups<Cfg, ConvBody<Cfg>>(a);
+}
+
+// ---- fused linear convolution of real rows by overlap-save, N = 2L (real::SegMap, DESIGN.md §4.12) ---------------
+// ConvBody's phases 1-5 as they are, on groups of C consecutive segments instead of rows.
+//   * load (phase 0): each lane reads its tile values' reals as scalars, issuing no read outside the row's [lo, hi)
+//     (zeros there), pairs them into complex values, runs stage A and scatters;
+//   * store (phases 6-8): RealBody's gather and park put the inverse's output in natural order into the FFT's park,
+//     and the TP lanes of the FFT store only the segment's kept outputs [lo, hi) from it, consecutive lanes writing
+//     consecutive samples, conjugating on the way out as ConvBody's store does.
+// Masking the store per tile register instead, or unrolling the store loop 1, 4 or 8 deep, makes ptxas spill a few
+// bytes at the f32 L = 128 and L = 1024 register caps; unrolled 2 deep no instance spills.
+// Segment q of the launch uses spectrum row ((g0 + q) / per) mod rows (ConvBody::pairs with row0 = g0).
+template <class Cfg> struct LinConvBody {
+  using Conv = ConvBody<Cfg>;
+  using Real = RealBody<Cfg>;
+  using Tile = typename Cfg::Tile;   // FWD = true
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  static constexpr int L = Cfg::L, TP = Tile::TP, RA = Tile::RA, RB = Tile::RB;
+  // Conv::Args with in = out = nullptr, row0 = m.g0, per = m.per, batch = segments of the launch
+  struct Args : Conv::Args { const T* x; T* y; real::SegMap m; };
+
+  static FB_HD void load(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    const int u = Tile::template u_of<true>(t);
+    long q = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (q >= a.batch) q = a.batch - 1;
+    const real::SegMap::Window w = a.m.in_window(q);
+    const T* src = a.x + w.base;
+    const unsigned n = w.hi - w.lo;
+    const long g = a.m.g0 + q;
+#pragma unroll
+    for (int qa = 0; qa < Tile::NA; ++qa)
+#pragma unroll
+      for (int i = 0; i < RA; ++i) {
+        // d = p - lo: one unsigned compare against hi - lo; a signed offset, so that the constant part folds into the
+        // load's immediate
+        const int d = 2 * (u + TP * qa + RB * i) - w.lo;
+        f.v[qa * RA + i] = mk<T>((unsigned)d < n ? real::lin_ld(src + d, g) : (T)0,
+                                 (unsigned)(d + 1) < n ? real::lin_ld(src + (d + 1), g) : (T)0);
+      }
+    f.template stage_a<true>(t, twa);
+    f.template scatter<true, typename Cfg::Lay>(t, smem);
+  }
+  // the park holds Z'' = FFT(conj Z') in natural order; the output is conj Z'' as interleaved reals
+  static FB_HD void store(const Args& a, long grp, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const long q = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (q >= a.batch) return;
+    const real::SegMap::Window w = a.m.out_window(q);
+    T* dst = a.y + w.base;
+    const long g = a.m.g0 + q;
+    const T* z = reinterpret_cast<const T*>(smem + Real::park(t));
+#pragma unroll 2
+    for (int p = w.lo + u; p < w.hi; p += TP) real::lin_st(dst + (p - w.lo), (p & 1) ? -z[p] : z[p], g);
+  }
+
+  // phase protocol (tilefft.cuh): load + stage A + scatter; ConvBody's phases 1-5; gather + stage B, park, store
+  static constexpr int kPhases = 9;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    if constexpr (P == 0) load(f, a, grp, t, smem, twa);
+    else if constexpr (P <= 5) Conv::template phase<P>(f, a, grp, t, smem, twa);
+    else if constexpr (P == 6) Real::fwd_gather(f, t, smem);
+    else if constexpr (P == 7) Real::fwd_park(f, t, smem);
+    else store(a, grp, t, smem);
+  }
+};
+
+template <class Cfg, int MINB>
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_lconv_kernel(const typename LinConvBody<Cfg>::Args a) {
+  run_onchip_groups<Cfg, LinConvBody<Cfg>>(a);
 }
 
 // ---- fused Bluestein -------------------------------------------------------------------------------------------

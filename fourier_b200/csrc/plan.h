@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "cplx.cuh"
+#include "real_kernels.cuh"   // real::SegMap
 
 namespace fb200 {
 
@@ -294,20 +295,24 @@ class Plan {
 // none.  run(): `in` / `out` are the reals (L complex values per row) and the spectrum (L+1 per row), swapped for the
 // inverse; tab = w_N^k, k <= L/2; h = scale / 2 (forward) or scale (inverse).  conv(): y = irfft(rfft(x) . H) of
 // real rows, in == out allowed; spec holds `rows` spectrum rows of L+1 bins, row b of the batch uses spectrum row
-// (row0 + b) mod rows; h = 1 / (2N).
+// ((row0 + b) / per) mod rows; h = 1 / (2N).  lconv(): segments g0 .. g0 + nseg - 1 of the linear convolution map m
+// (real::SegMap, DESIGN.md §4.12), out of place; segment g uses spectrum row (g / m.per) mod rows; h = 1 / (2N).
 template <typename T> struct RealOnChipOps {
   int ra, rb;
   cudaError_t (*prepare)();
   cudaError_t (*run)(const void* in, void* out, const void* twa, const cpx<T>* tab, size_t batch, bool fwd, T h,
                      int sms, cudaStream_t);
   cudaError_t (*conv)(const void* in, void* out, const void* twa, const cpx<T>* tab, const cpx<T>* spec, size_t rows,
-                      size_t row0, size_t batch, T h, int sms, cudaStream_t);
+                      size_t row0, size_t per, size_t batch, T h, int sms, cudaStream_t);
+  cudaError_t (*lconv)(const T* in, T* out, const real::SegMap& m, size_t nseg, const void* twa, const cpx<T>* tab,
+                       const cpx<T>* spec, size_t rows, T h, int sms, cudaStream_t);
 };
 template <typename T> const RealOnChipOps<T>* real_onchip_lookup(size_t l);
 
 // Batched real-input transform of length N (real.cu, DESIGN.md §4.10).  Forward: `batch` rows of N reals -> rows of
 // N/2+1 complex bins (numpy's rfft layout); inverse: the other way round (numpy's irfft).  Out of place only.
 // convolve_*: both in one call with a pointwise multiply between them (DESIGN.md §4.11), in place allowed.
+// linear_convolve_*: linear convolution of rows of any length by overlap-save on the same paths (DESIGN.md §4.12).
 template <typename T>
 class RealPlan {
  public:
@@ -334,11 +339,22 @@ class RealPlan {
   // enqueued on `stream`, not synchronised.
   cudaError_t convolve_device(const T* in, const C* spec, size_t rows, T* out, size_t batch, cudaStream_t stream) {
     launches_ = 0;
-    return convolve_rows(in, spec, rows, 0, out, batch, stream);
+    return convolve_rows(in, spec, rows, 0, 1, out, batch, stream);
   }
   // Host pointers: the spectra are staged once, the rows in chunks as in exec_host; returns when `out` is done.
   cudaError_t convolve_host(const T* in, const C* spec, size_t rows, T* out, size_t batch);
   size_t spec_bytes(size_t rows) const { return rows * (n_ / 2 + 1) * sizeof(C); }
+
+  // Linear convolution by overlap-save (DESIGN.md §4.12): `batch` rows of in_len reals -> rows of
+  // real::linear_out_len(mode, in_len, taps) reals, out[b][i] = y_full[off + i], y_full = row b (*) c, where
+  // c = irfft(spec[b mod rows], n = N) must vanish beyond its first `taps` samples.  1 <= taps <= N, in_len >= 1 (>= taps
+  // for valid), mode real::kLinear*; checked by the caller.  Out of place only.  Device pointers, enqueued on `stream`.
+  cudaError_t linear_convolve_device(const T* in, size_t in_len, const C* spec, size_t rows, size_t taps, int mode,
+                                     T* out, size_t batch, cudaStream_t stream);
+  // Host pointers: the spectra are staged once; whole rows in chunks when a row's input and output fit the staging
+  // chunk, else runs of segments of one row with only the input window they read; the same device code and bits.
+  cudaError_t linear_convolve_host(const T* in, size_t in_len, const C* spec, size_t rows, size_t taps, int mode,
+                                   T* out, size_t batch);
 
   unsigned long long launches() const { return launches_; }
   const char* kernel_name() const { return kernel_desc_.c_str(); }
@@ -356,8 +372,13 @@ class RealPlan {
   template <class P> friend P* create_plan(size_t, int, bool);
   RealPlan() = default;
   cudaError_t init(size_t n, int device, bool allow_fast_paths);
-  // convolve_device with row b using spectrum row (row0 + b) mod rows; adds its kernels to launches_
-  cudaError_t convolve_rows(const T* in, const C* spec, size_t rows, size_t row0, T* out, size_t batch, cudaStream_t s);
+  // convolve_device with row b using spectrum row ((row0 + b) / per) mod rows; adds its kernels to launches_
+  cudaError_t convolve_rows(const T* in, const C* spec, size_t rows, size_t row0, size_t per, T* out, size_t batch,
+                            cudaStream_t s);
+  // segments m.g0 .. m.g0 + nseg - 1 of a linear convolution: the fused kernel, or chunks of gather, convolve_rows and
+  // scatter through seg_; adds its kernels to launches_
+  cudaError_t linear_segments(const T* in, T* out, const real::SegMap& m, size_t nseg, const C* spec, size_t rows,
+                              cudaStream_t s);
   // The host-pointer loop of exec_host and convolve_host (real.cu): chunks of rows of in_row / out_row bytes go H2D,
   // through step(dev_in, dev_out, first_row, rows) on host_stream_, and D2H; launches() then counts all chunks.
   template <class Step>
@@ -373,7 +394,8 @@ class RealPlan {
   DeviceBuffer tab_, twa_;           // w_N^k, k <= N/4 (even N); stage twiddles of the fused kernel
   DeviceBuffer work_;                // one chunk of inner-plan rows
   DeviceBuffer stage_in_, stage_out_;
-  DeviceBuffer stage_spec_;          // the spectra of convolve_host
+  DeviceBuffer stage_spec_;          // the spectra of convolve_host and linear_convolve_host
+  DeviceBuffer seg_;                 // one chunk of N-real segments of a linear convolution (real_half, real_full)
   cudaStream_t host_stream_ = nullptr;
   std::string kernel_desc_;
 };

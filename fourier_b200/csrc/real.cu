@@ -8,6 +8,8 @@
 //               to a Hermitian spectrum, runs the complex inverse and keeps the real parts.  Correctness path only.
 // Convolution of real rows (DESIGN.md §4.11) runs on the same three paths: onchip_conv_kernel; the inner FFT,
 // conv_pair_kernel and the inner inverse, in place in `out`; widen, FFT, hermitian_mul_kernel, inverse, real part.
+// Linear convolution by overlap-save (DESIGN.md §4.12): onchip_lconv_kernel on the fused path; otherwise chunks of
+// segments gathered into seg_, convolved there in place as above and scattered.
 #include <algorithm>
 #include <string>
 #include <vector>
@@ -34,15 +36,15 @@ untangle_kernel(const cpx<T>* __restrict__ in, cpx<T>* __restrict__ out, const c
 }
 
 // One thread per pair (k, M-k), k <= M/2, of one row, in place on z (M complex values per row); row b uses spectrum
-// row (row0 + b) mod rows.
+// row ((row0 + b) / per) mod rows.
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
 conv_pair_kernel(cpx<T>* __restrict__ z, const cpx<T>* __restrict__ spec, const cpx<T>* __restrict__ tab, long m,
-                 long batch, long rows, long row0, T h) {
+                 long batch, long rows, long row0, long per, T h) {
   const long pairs = m / 2 + 1, total = pairs * batch;
   for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
     const long b = g / pairs, k = g - b * pairs;
-    real::conv_pair(z + b * m, spec + ((row0 + b) % rows) * (m + 1), m, k, tab, h);
+    real::conv_pair(z + b * m, spec + (((row0 + b) / per) % rows) * (m + 1), m, k, tab, h);
   }
 }
 
@@ -73,16 +75,37 @@ hermitian_kernel(const cpx<T>* __restrict__ x, cpx<T>* __restrict__ y, long n, l
       y[b * n + k] = real::hermitian(x + b * bins, n, k);
 }
 
-// y[k] *= s * (Hermitian extension of the spectrum row (row0 + b) mod rows)[k]; grid as hermitian_kernel
+// y[k] *= s * (Hermitian extension of the spectrum row ((row0 + b) / per) mod rows)[k]; grid as hermitian_kernel
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
 hermitian_mul_kernel(cpx<T>* __restrict__ y, const cpx<T>* __restrict__ spec, long n, long batch, long rows, long row0,
-                     T s) {
+                     long per, T s) {
   const long bins = n / 2 + 1;
   for (long b = blockIdx.y; b < batch; b += gridDim.y) {
-    const cpx<T>* hs = spec + ((row0 + b) % rows) * bins;
+    const cpx<T>* hs = spec + (((row0 + b) / per) % rows) * bins;
     for (long k = blockIdx.x * (long)blockDim.x + threadIdx.x; k < n; k += (long)gridDim.x * blockDim.x)
       y[b * n + k] = cscale(cmul(y[b * n + k], real::hermitian(hs, n, k)), s);
+  }
+}
+
+// Linear convolution (real::SegMap): one thread per sample p < N of segment q of the launch.  gather: the N input
+// samples of each segment into seg, zero outside the row's [lo, hi); scatter: the kept outputs of each segment.
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+gather_segments_kernel(const T* __restrict__ in, T* __restrict__ seg, const real::SegMap m, long nseg) {
+  const long total = nseg * m.n;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long q = g / m.n;
+    real::gather_one(m, in, seg, q, g - q * m.n);
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+scatter_segments_kernel(const T* __restrict__ seg, T* __restrict__ out, const real::SegMap m, long nseg) {
+  const long total = nseg * m.n;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long q = g / m.n;
+    real::scatter_one(m, seg, out, q, g - q * m.n);
   }
 }
 
@@ -259,13 +282,13 @@ cudaError_t RealPlan<T>::exec_host(bool forward, const void* in, void* out, size
 }
 
 template <typename T>
-cudaError_t RealPlan<T>::convolve_rows(const T* in, const C* spec, size_t rows, size_t row0, T* out, size_t batch,
-                                       cudaStream_t s) {
+cudaError_t RealPlan<T>::convolve_rows(const T* in, const C* spec, size_t rows, size_t row0, size_t per, T* out,
+                                       size_t batch, cudaStream_t s) {
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
-  row0 %= rows;
+  row0 %= rows * per;
   if (path_ == Path::kRealFused) {
-    FB_CHECK(fused_->conv(in, out, twa_.data(), (const C*)tab_.data(), spec, rows, row0, batch, (T)1 / (T)(2 * n_),
+    FB_CHECK(fused_->conv(in, out, twa_.data(), (const C*)tab_.data(), spec, rows, row0, per, batch, (T)1 / (T)(2 * n_),
                           sm_count_, s));
     launches_ += 1;
     return cudaSuccess;
@@ -275,7 +298,8 @@ cudaError_t RealPlan<T>::convolve_rows(const T* in, const C* spec, size_t rows, 
     FB_CHECK(inner_->exec_device((const C*)in, (C*)out, batch, kFft, s));
     launches_ += inner_->launches();
     conv_pair_kernel<T><<<grid_for((m_ / 2 + 1) * batch), kThreads, 0, s>>>(
-        (C*)out, spec, (const C*)tab_.data(), (long)m_, (long)batch, (long)rows, (long)row0, (T)1 / (T)(2 * n_));
+        (C*)out, spec, (const C*)tab_.data(), (long)m_, (long)batch, (long)rows, (long)row0, (long)per,
+        (T)1 / (T)(2 * n_));
     FB_CHECK(cudaGetLastError());
     launches_ += 1;
     FB_CHECK(inner_->exec_device((C*)out, (C*)out, batch, kUnscaledIfft, s));
@@ -293,7 +317,7 @@ cudaError_t RealPlan<T>::convolve_rows(const T* in, const C* spec, size_t rows, 
     launches_ += inner_->launches();
     const dim3 grid(grid_for(n_), (unsigned)std::min<size_t>(nb, 65535));
     hermitian_mul_kernel<T><<<grid, kThreads, 0, s>>>(work, spec, (long)n_, (long)nb, (long)rows,
-                                                      (long)((row0 + b0) % rows), (T)1 / (T)n_);
+                                                      (long)((row0 + b0) % (rows * per)), (long)per, (T)1 / (T)n_);
     FB_CHECK(cudaGetLastError());
     FB_CHECK(inner_->exec_device(work, work, nb, kUnscaledIfft, s));
     launches_ += inner_->launches();
@@ -316,9 +340,103 @@ cudaError_t RealPlan<T>::convolve_host(const T* in, const C* spec, size_t rows, 
   FB_CHECK(cudaMemcpyAsync(stage_spec_.data(), spec, spec_bytes(rows), cudaMemcpyHostToDevice, host_stream_));
   return stage_rows(in, out, batch, n_ * sizeof(T), n_ * sizeof(T),
                     [&](const void* din, void* dout, size_t b0, size_t nb) {
-                      return convolve_rows((const T*)din, (const C*)stage_spec_.data(), rows, b0, (T*)dout, nb,
+                      return convolve_rows((const T*)din, (const C*)stage_spec_.data(), rows, b0, 1, (T*)dout, nb,
                                            host_stream_);
                     });
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::linear_segments(const T* in, T* out, const real::SegMap& m, size_t nseg, const C* spec,
+                                         size_t rows, cudaStream_t s) {
+  if (nseg == 0) return cudaSuccess;
+  if (path_ == Path::kRealFused) {
+    FB_CHECK(fused_->lconv(in, out, m, nseg, twa_.data(), (const C*)tab_.data(), spec, rows, (T)1 / (T)(2 * n_),
+                           sm_count_, s));
+    launches_ += 1;
+    return cudaSuccess;
+  }
+  // chunks of segments through seg_: gather, the circular convolution in place (segment q of the chunk uses spectrum
+  // row ((g0 + q) / per) mod rows), scatter
+  const size_t chunk = std::min(nseg, std::max<size_t>(1, kScratchTargetBytes / (n_ * sizeof(T))));
+  FB_CHECK(seg_.reserve(chunk * n_ * sizeof(T)));
+  T* seg = (T*)seg_.data();
+  for (size_t q0 = 0; q0 < nseg; q0 += chunk) {
+    const size_t nq = std::min(chunk, nseg - q0);
+    real::SegMap mc = m;
+    mc.g0 = m.g0 + (long)q0;
+    gather_segments_kernel<T><<<grid_for(nq * n_), kThreads, 0, s>>>(in, seg, mc, (long)nq);
+    FB_CHECK(cudaGetLastError());
+    FB_CHECK(convolve_rows(seg, spec, rows, (size_t)mc.g0, (size_t)m.per, seg, nq, s));
+    scatter_segments_kernel<T><<<grid_for(nq * n_), kThreads, 0, s>>>(seg, out, mc, (long)nq);
+    FB_CHECK(cudaGetLastError());
+    launches_ += 2;
+  }
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::linear_convolve_device(const T* in, size_t in_len, const C* spec, size_t rows, size_t taps,
+                                                int mode, T* out, size_t batch, cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  const real::SegMap m = real::linear_map((long)n_, (long)taps, mode, (long)in_len);
+  return linear_segments(in, out, m, batch * (size_t)m.per, spec, rows, s);
+}
+
+// Host pointers, on the plan's own stream and synchronised after every piece, as stage_rows does.
+template <typename T>
+cudaError_t RealPlan<T>::linear_convolve_host(const T* in, size_t in_len, const C* spec, size_t rows, size_t taps,
+                                              int mode, T* out, size_t batch) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
+  FB_CHECK(stage_spec_.reserve(spec_bytes(rows)));
+  FB_CHECK(cudaMemcpyAsync(stage_spec_.data(), spec, spec_bytes(rows), cudaMemcpyHostToDevice, host_stream_));
+  const C* dspec = (const C*)stage_spec_.data();
+  const real::SegMap m = real::linear_map((long)n_, (long)taps, mode, (long)in_len);
+  const size_t out_len = (size_t)m.out_len;
+  if (std::max(in_len, out_len) * sizeof(T) <= kHostChunkBytes) {
+    // whole rows: row b0 of the piece is global row b0 at the start of the staged buffers
+    return stage_rows(in, out, batch, in_len * sizeof(T), out_len * sizeof(T),
+                      [&](const void* din, void* dout, size_t b0, size_t nb) {
+                        real::SegMap mp = m;
+                        mp.g0 = (long)b0 * m.per;
+                        mp.r0 = (long)b0;
+                        return linear_segments((const T*)din, (T*)dout, mp, nb * (size_t)m.per, dspec, rows,
+                                               host_stream_);
+                      });
+  }
+  // runs of R segments of one row: input window [off + j0*S - (K-1), off + j1*S) within [0, L), outputs [j0*S, j1*S)
+  const size_t cap = kHostChunkBytes / sizeof(T);
+  const size_t run = cap > n_ ? std::max<size_t>(1, (cap - n_) / (size_t)m.s) : 1;
+  FB_CHECK(stage_in_.reserve((run * (size_t)m.s + n_) * sizeof(T)));
+  FB_CHECK(stage_out_.reserve(run * (size_t)m.s * sizeof(T)));
+  unsigned long long total = 0;
+  for (size_t b = 0; b < batch; ++b)
+    for (long j0 = 0; j0 < m.per; j0 += (long)run) {
+      const long j1 = std::min(m.per, j0 + (long)run);
+      real::SegMap mp = m;
+      mp.g0 = (long)b * m.per + j0;
+      mp.r0 = (long)b;
+      mp.lo = std::max(0L, m.off + j0 * m.s - (m.k - 1));
+      mp.hi = std::min((long)in_len, m.off + j1 * m.s);
+      mp.out_lo = j0 * m.s;
+      const long out_hi = std::min(m.out_len, j1 * m.s);
+      if (mp.hi > mp.lo)
+        FB_CHECK(cudaMemcpyAsync(stage_in_.data(), in + b * in_len + mp.lo, (mp.hi - mp.lo) * sizeof(T),
+                                 cudaMemcpyHostToDevice, host_stream_));
+      launches_ = 0;
+      FB_CHECK(linear_segments((const T*)stage_in_.data(), (T*)stage_out_.data(), mp, (size_t)(j1 - j0), dspec, rows,
+                               host_stream_));
+      total += launches_;
+      FB_CHECK(cudaMemcpyAsync(out + b * out_len + mp.out_lo, stage_out_.data(), (out_hi - mp.out_lo) * sizeof(T),
+                               cudaMemcpyDeviceToHost, host_stream_));
+      FB_CHECK(cudaStreamSynchronize(host_stream_));
+    }
+  launches_ = total;
+  return cudaSuccess;
 }
 
 template class RealPlan<float>;

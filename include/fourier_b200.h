@@ -217,6 +217,46 @@ int fourier_b200_convolve_real_async_double(struct fourier_b200_rfft_double *pla
                                             const void *spectrum_dev, size_t spectrum_rows, double *out_dev,
                                             size_t batch, void *cuda_stream);
 
+/* ---- Linear convolution of real rows of any length, by overlap-save ----
+ * On a real plan of length N: `batch` rows of in_len = L >= 1 reals (row b starting at element b*L) are convolved with
+ * the filter c = irfft(H[b mod F], n=N), H as for the circular convolution above (F = spectrum_rows >= 1 rows of N/2+1
+ * bins in the plan's rfft layout), of which only the first `taps` = K samples may be non-zero, 1 <= K <= N:
+ *   y_full[t] = sum_{m<K} in[b][t-m] c[m],   out[b][i] = y_full[o + i],   output row b starting at element b*out_len,
+ *   mode FOURIER_B200_LINEAR_FULL  (0): out_len = L + K - 1, o = 0
+ *   mode FOURIER_B200_LINEAR_SAME  (1): out_len = L,         o = (K - 1) / 2
+ *   mode FOURIER_B200_LINEAR_VALID (2): out_len = L - K + 1, o = K - 1 (needs L >= K)
+ * With H[f] = rfft(h) of a K-tap h zero-padded to N this is scipy.signal.convolve(in[b], h, mode).  Keeping c[K..N) zero
+ * is the caller's contract: any other H gives the overlap-save output, which is unspecified.  Correlation is the same
+ * call with conj(H).  Rows are cut into segments of S = N - K + 1 outputs (N reads each, the K - 1 before them
+ * overlapping the previous segment's), so S / N is the useful fraction of every transform: choose N a few times K.
+ * Launches: 1 on the real_fused path; on the others, per scratch chunk of segments, 2 + those of the circular
+ * convolution of that many rows; last_launches of the info call reports the total.
+ * Refused with cudaErrorInvalidValue and a message: a NULL argument, spectrum_rows == 0, taps == 0, taps > N,
+ * in_len == 0, an unknown mode, mode valid with in_len < taps (these also when batch == 0, which otherwise succeeds and
+ * launches nothing), `in` and `out` overlapping at all (out of place only), `spectrum` overlapping `out`, and a mix of
+ * host and device buffers in the synchronous calls.  Device base pointers must be 16-byte aligned
+ * (cudaErrorMisalignedAddress); rows inside them may start at any element.  Host memory is staged through the plan's
+ * buffers, whole rows while a row fits 64 MB and otherwise only the input each run of segments reads, and gives the
+ * same bits as device memory.  The _async calls take device memory, are enqueued on `cuda_stream` and not
+ * synchronised. */
+#define FOURIER_B200_LINEAR_FULL 0
+#define FOURIER_B200_LINEAR_SAME 1
+#define FOURIER_B200_LINEAR_VALID 2
+int fourier_b200_linear_convolve_real_float(struct fourier_b200_rfft_float *plan, const float *in, size_t in_len,
+                                            const void *spectrum, size_t spectrum_rows, size_t taps, int mode,
+                                            float *out, size_t batch);
+int fourier_b200_linear_convolve_real_double(struct fourier_b200_rfft_double *plan, const double *in, size_t in_len,
+                                             const void *spectrum, size_t spectrum_rows, size_t taps, int mode,
+                                             double *out, size_t batch);
+int fourier_b200_linear_convolve_real_async_float(struct fourier_b200_rfft_float *plan, const float *in_dev,
+                                                  size_t in_len, const void *spectrum_dev, size_t spectrum_rows,
+                                                  size_t taps, int mode, float *out_dev, size_t batch,
+                                                  void *cuda_stream);
+int fourier_b200_linear_convolve_real_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev,
+                                                   size_t in_len, const void *spectrum_dev, size_t spectrum_rows,
+                                                   size_t taps, int mode, double *out_dev, size_t batch,
+                                                   void *cuda_stream);
+
 const char *fourier_b200_last_error(void);
 const char *fourier_b200_version(void);
 
