@@ -2,7 +2,8 @@
 // one place for the library (fused_lookup in twopass.cu) and the CPU emulator (tools/emulate.cu).
 //
 // FusedConfig<T, LOG2N>: the default configuration of N = 2^LOG2N; FusedConfig<T, LOG2N, true>: the other load
-// strategy, selected with FOURIER_B200_CFG=1 (HAS = false where there is none).  Cfg is the kernel configuration,
+// strategy, selected with FOURIER_B200_CFG=1 (HAS = false where there is none).  A default with pair items
+// (PairCfg) runs its Cfg::Unpaired with FOURIER_B200_PAIR=0.  Cfg is the kernel configuration,
 // RING / LAG its default ring and lag.
 // Ring (intermediates kept in L2) = 32 MB / transform size, lag = ring / 2: the ring must stay well inside the
 // H100's 50 MB L2 next to the prefetched input tiles.  The ring may have any size >= 2.  Measured on one H100 SXM
@@ -25,8 +26,9 @@ template <typename T, int LOG2N, bool ALT = false> struct FusedConfig { static c
   };
 
 // template arguments: <T, RA, C, G, PAD1, EXB, DIRECT, RB, RA2, RB2, E1, E2, C1, TABG>
-// 1024 x 1024: two 256-thread groups, TMA staging, one shared exchange buffer taken under a lock
-FB_FUSED_CONFIG(float, 20, false, FusedCfg<float, 32, 8, 2, 8, 1>)
+// 1024 x 1024: two 256-thread groups, TMA staging, one shared exchange buffer taken under a lock; pair items
+// (FOURIER_B200_PAIR=0: one item per group)
+FB_FUSED_CONFIG(float, 20, false, PairCfg<FusedCfg<float, 32, 8, 2, 8, 1>>)
 FB_FUSED_CONFIG(float, 20, true, FusedCfg<float, 32, 8, 2, 8, 2, true>)
 // 512 (32 x 16) x 1024 (32 x 32), 16-column pass-1 tiles: two 256-thread groups; tile tables read from L2
 FB_FUSED_CONFIG(float, 19, false, FusedCfg<float, 32, 8, 2, 0, 1, false, 16, 32, 32, 32, 32, 16, true>)

@@ -247,6 +247,19 @@ struct FusedCfg {
   static constexpr size_t SMEM_BYTES = OFF_CTL + 2048 /* control block: G * sizeof(GroupCtl) + locks */;
   static constexpr int BOX_ROWS = N1 < 256 ? (int)N1 : 256;   // TMA box limit: 256 per dimension
   static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB of shared memory per CTA");
+  static constexpr bool PAIR = false;
+  using Unpaired = FusedCfg;
+};
+
+// Pair items: one producer lane per CTA claims two adjacent tiles at a time (pass-1 tiles 2j, 2j+1 or pass-2 tiles
+// 2i, 2i+1) and loads tile 2 x item + g into the staging buffer of group g, once both groups have emptied theirs.  The
+// two groups then load and store the two halves of the same 128-byte lines of HBM at about the same time, where
+// single items leave each half to a different SM at an unrelated moment (DESIGN.md 4.2, 5).  Everything a group
+// does is unchanged: its staging layout, its tile, its counters.
+template <class Base> struct PairCfg : Base {
+  static_assert(Base::G == 2 && !Base::DIRECT && Base::T1 % 2 == 0 && Base::T2 % 2 == 0, "pairs: two staged groups");
+  static constexpr bool PAIR = true;
+  using Unpaired = Base;
 };
 
 constexpr int kStoreRing = 16;
@@ -449,6 +462,38 @@ fused_twopass_kernel(const __grid_constant__ CUtensorMap in_map, const FusedArgs
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(Cfg::REGS_PRODUCER));
     const int pw = (tid - Cfg::CONSUMERS) >> 5;
     if ((tid & 31) != 0) return;
+    if constexpr (Cfg::PAIR) {
+      if (pw == 0) {
+        // ---- the producer of both groups (pair items): the same just-in-time claim, for a tile per group.  The CTA
+        // holds at most two claimed, unfinished items (one in both groups' registers, one staged or in flight), every
+        // dependency points to an earlier queue position, and the lane claims only once both staging buffers are
+        // empty: the argument of the header comment holds item by item.
+        const int g = 0;   // (trace row)
+        uint32_t n_p1 = 0;
+        for (uint32_t it = 0;; ++it) {
+          FB_PTRACE(0);
+          if (it > 0)
+            for (int h = 0; h < G; ++h) mbar_wait(&ctl_all[h].empty, (it - 1) & 1);
+          FB_PTRACE(2);
+          const WorkItem wi = decode_work((long)atomicAdd(queue, 1u), a.batch, a.lag, T1 / 2, T2 / 2);
+          unsigned target;
+          const unsigned* dep = dep_counter<Cfg>(wi, a, &target);   // counted in tiles, as for single items
+          if (dep) { spin_until_ge(dep, target); fence_proxy_async(); }
+          FB_PTRACE(1);
+          for (int h = 0; h < G; ++h) {
+            WorkItem wh = wi;
+            wh.tile = 2 * wi.tile + h;
+            issue_tile<Cfg>(wh, &in_map, a, reinterpret_cast<V*>(staging + (size_t)h * Cfg::BUF_BYTES),
+                            tabs + (size_t)h * 2 * Cfg::TAB_ELEMS + (size_t)(n_p1 & 1) * Cfg::TAB_ELEMS, &ctl_all[h]);
+          }
+          FB_PTRACE(3);
+          n_p1 += wi.pass == 1;
+          if (wi.pass < 0) break;
+        }
+        return;
+      }
+      if (pw < G) return;
+    }
     if (pw < G) {
       // ---- producer of group pw: wait until the group has emptied its staging buffer, only then claim a queue
       // item, wait for its dependencies (blocking is fine here: nothing a consumer needs is held back by it),

@@ -364,11 +364,12 @@ static bool check_queue_order(int t1, int t2, int batch, int ring, int lag, long
 
 // The queue of one persistent configuration (fused_configs.cuh: the library's table): its (T1, T2) at its default
 // ring / lag and at rings 2, 3, 5 and 24 with every lag, over a range of batches, and the ring / lag the launch
-// actually uses (fused::launch_ring, the rule the library runs) for every batch 1 .. 3 x ring.
+// actually uses (fused::launch_ring, the rule the library runs) for every batch 1 .. 3 x ring.  With pair items
+// (PairCfg) the queue holds T1 / 2 and T2 / 2 items per transform, two tiles each.
 template <class Conf>
 static int check_queue(const char* name) {
   using Cfg = typename Conf::Cfg;
-  constexpr int t1 = Cfg::T1, t2 = Cfg::T2;
+  constexpr int t1 = Cfg::PAIR ? Cfg::T1 / 2 : Cfg::T1, t2 = Cfg::PAIR ? Cfg::T2 / 2 : Cfg::T2;
   const int ring0 = Conf::RING, lag0 = Conf::LAG;
   int layouts = 0, bad = 0;
   long gaps = 0;
@@ -394,9 +395,9 @@ static int check_queue(const char* name) {
     shrunk += rl.ring < ring0;
     one(batch, rl.ring, rl.lag);
   }
-  printf("fused work queue %s (T1 %d, T2 %d; ring %d, lag %d; rings 2, 3, 5, 24; launch rings of batches 1..%d, %d "
+  printf("fused work queue %s%s (T1 %d, T2 %d; ring %d, lag %d; rings 2, 3, 5, 24; launch rings of batches 1..%d, %d "
          "shrunk): %d layouts, %ld steady-state gaps, permutation / dependency-order / gap properties %s\n",
-         name, t1, t2, ring0, lag0, 3 * ring0, shrunk, layouts, gaps, bad ? "FAILED" : "OK");
+         name, Cfg::PAIR ? ", pair items" : "", t1, t2, ring0, lag0, 3 * ring0, shrunk, layouts, gaps, bad ? "FAILED" : "OK");
   return bad;
 }
 
@@ -767,6 +768,8 @@ int main() {
   bad += check_queue<fused::FusedConfig<float, 18>>("f32 2^18");
   bad += check_queue<fused::FusedConfig<float, 19>>("f32 2^19");
   bad += check_queue<fused::FusedConfig<float, 20>>("f32 2^20");
+  struct Single20 : fused::FusedConfig<float, 20> { using Cfg = fused::FusedConfig<float, 20>::Cfg::Unpaired; };
+  bad += check_queue<Single20>("f32 2^20 (FOURIER_B200_PAIR=0)");
   bad += check_queue<fused::FusedConfig<double, 12>>("f64 2^12");
   bad += check_queue<fused::FusedConfig<double, 13>>("f64 2^13");
   bad += check_queue<fused::FusedConfig<double, 14>>("f64 2^14");
