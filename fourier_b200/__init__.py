@@ -18,6 +18,9 @@ reference's operator interface name for name:
     (no counterpart)                                      RealFft.convolve_linear: linear convolution of real
                                                             rows of any length with K <= N taps (scipy's
                                                             full / same / valid), overlap-save in one call
+    (no counterpart)                                      RealFft.stft / istft / stft_frames: short-time Fourier
+                                                            transform of real rows and its overlap-add inverse
+                                                            (torch.stft / istft, frames frame-major)
 
 Buffers are numpy arrays (host memory: staged over PCIe by the library) or torch CUDA tensors
 (device memory: transformed in HBM on torch's current stream).  A leading batch dimension is
@@ -373,6 +376,102 @@ class RealFft:
                 self._plan, pi, in_len, ps, rows, taps, code, po, batch)
         if rc != 0:
             raise RuntimeError(f"linear convolution failed (cuda error {rc}): {_lib.last_error()}")
+
+    STFT_PAD_MODES = {"constant": 1, "reflect": 2}
+
+    def stft_frames(self, in_len, hop, center=True):
+        """F, the number of frames `stft` makes of rows of in_len samples: 1 + (in_len + 2 pad - N) // hop with
+        pad = N//2 if center else 0."""
+        pad = self._size // 2 if center else 0
+        return 1 + (int(in_len) + 2 * pad - self._size) // int(hop)
+
+    def _stft_buffers(self, buffers):
+        for x in buffers:
+            if _is_torch(x) and (x.is_conj() or x.is_neg()):
+                raise ValueError("torch tensors with the conj or neg bit set hold unconjugated data: "
+                                 "pass x.resolve_conj() (and resolve_neg()) instead")
+
+    def stft(self, input, window, hop, output, center=True, pad_mode="reflect"):
+        """Short-time Fourier transform of every row of `input` (shape (..., L)): frames of N = size() samples every
+        `hop`, times `window` (N reals; zero-pad a shorter one), through rfft.  `output` has shape (..., F, N//2+1),
+        F = stft_frames(L, hop, center), frame-major: this is torch.stft(x, N, hop, window=window, center=center,
+        pad_mode=pad_mode, return_complex=True).transpose(-1, -2).  With center the rows are padded by N//2 on both
+        sides, with zeros (pad_mode "constant") or mirrored without repeating the edge ("reflect", needs L > N//2);
+        pad_mode is ignored without center, which needs L >= N.  Out of place only."""
+        self._stft_buffers((input, window, output))
+        if center and pad_mode not in self.STFT_PAD_MODES:
+            raise ValueError(f"pad_mode must be one of {sorted(self.STFT_PAD_MODES)}, got {pad_mode!r}")
+        hop = int(hop)
+        if hop < 1:
+            raise ValueError(f"hop must be at least 1, got {hop}")
+        boundary = self.STFT_PAD_MODES[pad_mode] if center else 0
+        n = self._size
+        in_len = input.shape[-1] if getattr(input, "ndim", 0) > 0 else 0
+        if in_len < 1:
+            raise ValueError("input rows must hold at least one sample")
+        if boundary == 0 and in_len < n:
+            raise ValueError(f"center=False needs rows of at least N = {n} samples, got {in_len}")
+        if boundary == 2 and in_len <= n // 2:
+            raise ValueError(f"pad_mode 'reflect' needs rows of more than N//2 = {n // 2} samples, got {in_len}")
+        frames = self.stft_frames(in_len, hop, center)
+        pi, li, di, si = self._describe(input, "real", last=in_len)
+        pw, lw, dw, _ = self._describe(window, "real")
+        if lw != ():
+            raise ValueError(f"window must hold exactly N = {n} reals, got shape {tuple(window.shape)}")
+        if getattr(output, "ndim", 0) < 2 or output.shape[-2] != frames:
+            raise ValueError(f"output must have shape (..., {frames}, {n // 2 + 1}) (F = {frames} frames)")
+        po, lo, do_, _ = self._describe(output, "spec")
+        if li != lo[:-1]:
+            raise ValueError(f"input and output leading shapes differ: {li} and {lo[:-1]}")
+        if not (di == dw == do_):
+            raise ValueError("input, window and output must all be host or all be device buffers")
+        batch = int(np.prod(li, dtype=np.int64))
+        L = _lib.load()
+        if di:
+            rc = getattr(L, f"fourier_b200_stft_async_{self._t}")(self._plan, pi, in_len, pw, hop, boundary, po, batch,
+                                                                   si)
+        else:
+            rc = getattr(L, f"fourier_b200_stft_{self._t}")(self._plan, pi, in_len, pw, hop, boundary, po, batch)
+        if rc != 0:
+            raise RuntimeError(f"stft failed (cuda error {rc}): {_lib.last_error()}")
+
+    def istft(self, input, window, hop, output, center=True):
+        """Inverse of stft: `input` (shape (..., F, N//2+1), stft's frame-major layout) -> `output` (shape
+        (..., out_len), any out_len >= 1).  Output i is the overlap-add of window * irfft(frame) over the frames that
+        cover padded position t = i + pad (pad = N//2 if center), divided by the sum of window^2 there; 0 where that
+        sum is below 1e-11, including positions no frame covers (torch.istft raises instead).  With out_len =
+        hop * (F - 1) + N - 2 pad this is torch.istft(input.transpose(-1, -2), N, hop, window=window, center=center,
+        length=out_len).  Out of place only."""
+        self._stft_buffers((input, window, output))
+        hop = int(hop)
+        if hop < 1:
+            raise ValueError(f"hop must be at least 1, got {hop}")
+        n = self._size
+        if getattr(input, "ndim", 0) < 2 or input.shape[-2] < 1:
+            raise ValueError(f"input must have shape (..., F, {n // 2 + 1}) with F >= 1")
+        frames = int(input.shape[-2])
+        out_len = output.shape[-1] if getattr(output, "ndim", 0) > 0 else 0
+        if out_len < 1:
+            raise ValueError("output rows must hold at least one sample")
+        pi, li, di, si = self._describe(input, "spec")
+        pw, lw, dw, _ = self._describe(window, "real")
+        if lw != ():
+            raise ValueError(f"window must hold exactly N = {n} reals, got shape {tuple(window.shape)}")
+        po, lo, do_, _ = self._describe(output, "real", last=out_len)
+        if li[:-1] != lo:
+            raise ValueError(f"input and output leading shapes differ: {li[:-1]} and {lo}")
+        if not (di == dw == do_):
+            raise ValueError("input, window and output must all be host or all be device buffers")
+        batch = int(np.prod(lo, dtype=np.int64))
+        L = _lib.load()
+        if di:
+            rc = getattr(L, f"fourier_b200_istft_async_{self._t}")(self._plan, pi, frames, pw, hop, int(bool(center)),
+                                                                    po, out_len, batch, si)
+        else:
+            rc = getattr(L, f"fourier_b200_istft_{self._t}")(self._plan, pi, frames, pw, hop, int(bool(center)), po,
+                                                              out_len, batch)
+        if rc != 0:
+            raise RuntimeError(f"istft failed (cuda error {rc}): {_lib.last_error()}")
 
     def rfft(self, input, output, transform=Transform.Fft):
         """output[..., :N//2+1] = numpy.fft.rfft(input) (Fft) or that times 1/sqrt(N) (SqrtScaledFft)."""

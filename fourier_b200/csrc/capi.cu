@@ -258,6 +258,90 @@ int linear_exec(void* plan, const T* in, size_t in_len, const void* spectrum, si
   }
 }
 
+// Short-time Fourier transform of real rows: out of place only; the arguments are checked before the plan is touched,
+// even for batch == 0, except in_len against N.
+template <typename T>
+int stft_exec(void* plan, const T* in, size_t in_len, const T* window, size_t hop, int boundary, void* out, size_t batch,
+              bool async, void* stream) {
+  if (!plan || !in || !window || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
+  const char* bad = hop == 0                          ? "hop must be at least 1"
+                    : boundary < 0 || boundary > 2    ? "unknown boundary (FOURIER_B200_STFT_NONE, _ZEROS or _REFLECT)"
+                    : in_len == 0                     ? "in_len must be at least 1"
+                                                      : nullptr;
+  if (bad) { fb200::set_last_error(bad); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  using C = typename RealPlan<T>::C;
+  const size_t n = p->size();
+  if (boundary == fb200::real::kStftNone && in_len < n) {
+    fb200::set_last_error("boundary none needs in_len >= N");
+    return (int)cudaErrorInvalidValue;
+  }
+  if (boundary == fb200::real::kStftReflect && in_len <= n / 2) {
+    fb200::set_last_error("boundary reflect needs in_len > N/2");
+    return (int)cudaErrorInvalidValue;
+  }
+  try {
+    if (batch == 0) return (int)p->stft_device(in, in_len, window, hop, boundary, (C*)out, 0, nullptr);
+    const size_t frames = (size_t)fb200::real::frame_map((long)n, (long)in_len, (long)hop, boundary).frames;
+    const size_t in_bytes = batch * in_len * sizeof(T), out_bytes = batch * frames * (n / 2 + 1) * sizeof(C);
+    if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, n * sizeof(T), out, out_bytes)) {
+      fb200::set_last_error("input or window and output overlap (the stft is out of place only)");
+      return (int)cudaErrorInvalidValue;
+    }
+    if (!async) {
+      const int dev =
+          residence({in, window, out}, "input, window and output must all be host or all be device memory");
+      if (dev < 0) return (int)cudaErrorInvalidValue;
+      if (!dev) return (int)p->stft_host(in, in_len, window, hop, boundary, (C*)out, batch);
+    }
+    if (!device_pointers_aligned(in, out)) return (int)cudaErrorMisalignedAddress;
+    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
+    cudaError_t e = p->stft_device(in, in_len, window, hop, boundary, (C*)out, batch, s);
+    if (e != cudaSuccess || async) return (int)e;
+    return (int)cudaStreamSynchronize(s);
+  } catch (...) {
+    fb200::set_last_error("stft threw");
+    return (int)cudaErrorUnknown;
+  }
+}
+
+template <typename T>
+int istft_exec(void* plan, const void* in, size_t frames, const T* window, size_t hop, int center, T* out,
+               size_t out_len, size_t batch, bool async, void* stream) {
+  if (!plan || !in || !window || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
+  const char* bad = hop == 0        ? "hop must be at least 1"
+                    : frames == 0   ? "frames must be at least 1"
+                    : out_len == 0  ? "out_len must be at least 1"
+                                    : nullptr;
+  if (bad) { fb200::set_last_error(bad); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  using C = typename RealPlan<T>::C;
+  const C* spec = static_cast<const C*>(in);
+  try {
+    if (batch == 0) return (int)p->istft_device(spec, frames, window, hop, center != 0, out, out_len, 0, nullptr);
+    const size_t n = p->size();
+    const size_t in_bytes = batch * frames * (n / 2 + 1) * sizeof(C), out_bytes = batch * out_len * sizeof(T);
+    if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, n * sizeof(T), out, out_bytes)) {
+      fb200::set_last_error("input or window and output overlap (the istft is out of place only)");
+      return (int)cudaErrorInvalidValue;
+    }
+    if (!async) {
+      const int dev =
+          residence({in, window, out}, "input, window and output must all be host or all be device memory");
+      if (dev < 0) return (int)cudaErrorInvalidValue;
+      if (!dev) return (int)p->istft_host(spec, frames, window, hop, center != 0, out, out_len, batch);
+    }
+    if (!device_pointers_aligned(in, out)) return (int)cudaErrorMisalignedAddress;
+    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
+    cudaError_t e = p->istft_device(spec, frames, window, hop, center != 0, out, out_len, batch, s);
+    if (e != cudaSuccess || async) return (int)e;
+    return (int)cudaStreamSynchronize(s);
+  } catch (...) {
+    fb200::set_last_error("istft threw");
+    return (int)cudaErrorUnknown;
+  }
+}
+
 }  // namespace
 
 using fourier::c::fourier_fft_double;
@@ -516,6 +600,43 @@ int fourier_b200_linear_convolve_real_async_double(fourier_b200_rfft_double* pla
                                                    int mode, double* out_dev, size_t batch, void* stream) {
   return linear_exec<double>(plan, in_dev, in_len, spectrum_dev, spectrum_rows, taps, mode, out_dev, batch, true,
                              stream);
+}
+
+int fourier_b200_stft_float(fourier_b200_rfft_float* plan, const float* in, size_t in_len, const float* window,
+                            size_t hop, int boundary, void* out, size_t batch) {
+  return stft_exec<float>(plan, in, in_len, window, hop, boundary, out, batch, false, nullptr);
+}
+int fourier_b200_stft_double(fourier_b200_rfft_double* plan, const double* in, size_t in_len, const double* window,
+                             size_t hop, int boundary, void* out, size_t batch) {
+  return stft_exec<double>(plan, in, in_len, window, hop, boundary, out, batch, false, nullptr);
+}
+int fourier_b200_stft_async_float(fourier_b200_rfft_float* plan, const float* in_dev, size_t in_len,
+                                  const float* window_dev, size_t hop, int boundary, void* out_dev, size_t batch,
+                                  void* stream) {
+  return stft_exec<float>(plan, in_dev, in_len, window_dev, hop, boundary, out_dev, batch, true, stream);
+}
+int fourier_b200_stft_async_double(fourier_b200_rfft_double* plan, const double* in_dev, size_t in_len,
+                                   const double* window_dev, size_t hop, int boundary, void* out_dev, size_t batch,
+                                   void* stream) {
+  return stft_exec<double>(plan, in_dev, in_len, window_dev, hop, boundary, out_dev, batch, true, stream);
+}
+int fourier_b200_istft_float(fourier_b200_rfft_float* plan, const void* in, size_t frames, const float* window,
+                             size_t hop, int center, float* out, size_t out_len, size_t batch) {
+  return istft_exec<float>(plan, in, frames, window, hop, center, out, out_len, batch, false, nullptr);
+}
+int fourier_b200_istft_double(fourier_b200_rfft_double* plan, const void* in, size_t frames, const double* window,
+                              size_t hop, int center, double* out, size_t out_len, size_t batch) {
+  return istft_exec<double>(plan, in, frames, window, hop, center, out, out_len, batch, false, nullptr);
+}
+int fourier_b200_istft_async_float(fourier_b200_rfft_float* plan, const void* in_dev, size_t frames,
+                                   const float* window_dev, size_t hop, int center, float* out_dev, size_t out_len,
+                                   size_t batch, void* stream) {
+  return istft_exec<float>(plan, in_dev, frames, window_dev, hop, center, out_dev, out_len, batch, true, stream);
+}
+int fourier_b200_istft_async_double(fourier_b200_rfft_double* plan, const void* in_dev, size_t frames,
+                                    const double* window_dev, size_t hop, int center, double* out_dev, size_t out_len,
+                                    size_t batch, void* stream) {
+  return istft_exec<double>(plan, in_dev, frames, window_dev, hop, center, out_dev, out_len, batch, true, stream);
 }
 
 const char* fourier_b200_last_error(void) { return fb200::last_error(); }

@@ -88,7 +88,18 @@ struct OnChipImpl {
     if ((e = allow_smem(onchip::onchip_real_kernel<Cfg<true>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_real_kernel<Cfg<false>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_conv_kernel<Cfg<true>, MINB>))) return e;
-    return allow_smem(onchip::onchip_lconv_kernel<Cfg<true>, MINB>);
+    if ((e = allow_smem(onchip::onchip_lconv_kernel<Cfg<true>, MINB>))) return e;
+    return allow_smem(onchip::onchip_stft_kernel<Cfg<true>, MINB>);
+  }
+  static cudaError_t stft(const T* in, const T* win, void* out, const real::FrameMap& m, size_t nframes,
+                          const void* twa, const cpx<T>* tab, int sms, cudaStream_t s) {
+    typename onchip::StftBody<Cfg<true>>::Args a;
+    static_cast<typename onchip::RealBody<Cfg<true>>::Args&>(a) = {
+        nullptr, (cpx<T>*)out, (const TwPair<T>*)twa, tab, (long)nframes, (T)0.5};
+    a.x = in;
+    a.win = win;
+    a.m = m;
+    return launch(onchip::onchip_stft_kernel<Cfg<true>, MINB>, a, nframes, sms, s);
   }
   static cudaError_t conv(const void* in, void* out, const void* twa, const cpx<T>* tab, const cpx<T>* spec,
                           size_t rows, size_t row0, size_t per, size_t batch, T h, int sms, cudaStream_t s) {
@@ -116,7 +127,7 @@ struct OnChipImpl {
                   {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab, (long)batch, h}, batch, sms, s);
   }
   static const OnChipOps<T>* ops() {
-    static const RealOnChipOps<T> r = {RA, RB, &real_prepare, &real, &conv, &lconv};
+    static const RealOnChipOps<T> r = {RA, RB, &real_prepare, &real, &conv, &lconv, &stft};
     static const OnChipOps<T> o = {RA, RB, &prepare, &fft, kHasBluestein ? &bluestein : nullptr, &r};
     return &o;
   }

@@ -7,7 +7,9 @@
 //   * onchip_real_kernel:     real-input transforms of length 2L (forward and inverse) on the same tiles.
 //   * onchip_conv_kernel:     y = irfft(rfft(x) . H) of real rows of length 2L, both transforms in one kernel.
 //   * onchip_lconv_kernel:    linear convolution of real rows of any length by overlap-save on the same phases.
-//     (these four run the phases of FftBody / RealBody / ConvBody / LinConvBody through run_onchip_groups, tilefft.cuh)
+//   * onchip_stft_kernel:     windowed frames of real rows of any length through the forward real-input phases.
+//     (these five run the phases of FftBody / RealBody / ConvBody / LinConvBody / StftBody through run_onchip_groups,
+//     tilefft.cuh)
 //   * bluestein_fused_kernel: the whole chirp-z transform of the reference (bluesteins.rs:218-259) for
 //                             N <= L, M = 2L, in one kernel and without touching HBM in between.
 //
@@ -324,6 +326,75 @@ template <class Cfg> struct LinConvBody {
 template <class Cfg, int MINB>
 __global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_lconv_kernel(const typename LinConvBody<Cfg>::Args a) {
   run_onchip_groups<Cfg, LinConvBody<Cfg>>(a);
+}
+
+// ---- fused short-time Fourier transform of real rows, N = 2L (real::FrameMap, DESIGN.md §4.13) -------------------
+// RealBody's forward on groups of C consecutive frames instead of rows, with its own load:
+//   * load (phase 0): the TP lanes of an FFT read the frame's N reals as scalars, consecutive lanes taking consecutive
+//     samples, multiply them by the window w[p] and write them into the FFT's park.  A frame inside the row reads
+//     row[t0 + p] unmasked; only a frame that reaches past either end maps each sample through FrameMap::Edge (zero or
+//     mirrored), so no read leaves [0, L);
+//   * phases 1-2: the frame as L complex values from the park in stage-A input order, stage A; the scatter (which
+//     overwrites the park) after a __syncwarp;
+//   * phases 3-5: RealBody's gather + stage B, park and untangle store, frame q of the launch writing spectrum row q of
+//     `out` (frames are spectrum rows, frame-major).
+// Loading the tile's registers straight from the row, as LinConvBody does, needs the window's N reals beside the
+// frame's: ptxas then spilled 650-700 bytes at the f32 L = 512 and 1024 register caps.  Staged through the park, no
+// instance spills.
+template <class Cfg> struct StftBody {
+  using Real = RealBody<Cfg>;
+  using Tile = typename Cfg::Tile;   // FWD = true
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  static constexpr int L = Cfg::L, TP = Tile::TP, RA = Tile::RA, RB = Tile::RB;
+  // Real::Args with in = nullptr, out = the spectrum of frame g0, batch = frames of the launch
+  struct Args : Real::Args { const T* x; const T* win; real::FrameMap m; };
+
+  static FB_HD void load(const Args& a, long grp, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    long q = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (q >= a.batch) q = a.batch - 1;
+    const long g = a.m.g0 + q, b = a.m.row_of(g), t0 = a.m.start(g, b);
+    const T* row = a.x + (b - a.m.r0) * a.m.in_ld;
+    T* z = reinterpret_cast<T*>(smem + Real::park(t));
+    if (t0 >= 0 && t0 + 2 * L <= a.m.len) {
+      const T* src = row + t0;
+#pragma unroll 2
+      for (int p = u; p < 2 * L; p += TP) z[p] = real::lin_ld(src + p, g) * a.win[p];
+    } else {
+      // 32-bit offsets from an anchor sample c of the row (see FrameMap::edge)
+      const real::FrameMap::Edge e = a.m.edge(t0);
+      const T* src = row + e.c;
+#pragma unroll 2
+      for (int p = u; p < 2 * L; p += TP) {
+        const int d = e.map(e.d0 + p);
+        z[p] = e.in(d) ? real::lin_ld(src + d, g) * a.win[p] : (T)0;
+      }
+    }
+  }
+  static FB_HD void load_stage_a(Tile& f, int t, const V* smem, const TwPair<T>* twa) {
+    const int u = Tile::template u_of<true>(t);
+    const V* z = smem + Real::park(t);
+#pragma unroll
+    for (int q = 0; q < Tile::NA; ++q)
+#pragma unroll
+      for (int i = 0; i < RA; ++i) f.v[q * RA + i] = z[u + TP * q + RB * i];
+    f.template stage_a<true>(t, twa);
+  }
+
+  // phase protocol (tilefft.cuh): load into the park; stage A; scatter; RealBody's gather + stage B, park, store
+  static constexpr int kPhases = 6;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    if constexpr (P == 0) load(a, grp, t, smem);
+    else if constexpr (P == 1) load_stage_a(f, t, smem, twa);
+    else if constexpr (P == 2) f.template scatter<true, typename Cfg::Lay>(t, smem);
+    else Real::template phase<P - 2>(f, a, grp, t, smem, twa);
+  }
+};
+
+template <class Cfg, int MINB>
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_stft_kernel(const typename StftBody<Cfg>::Args a) {
+  run_onchip_groups<Cfg, StftBody<Cfg>>(a);
 }
 
 // ---- fused Bluestein -------------------------------------------------------------------------------------------

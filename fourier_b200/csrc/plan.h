@@ -297,6 +297,8 @@ class Plan {
 // real rows, in == out allowed; spec holds `rows` spectrum rows of L+1 bins, row b of the batch uses spectrum row
 // ((row0 + b) / per) mod rows; h = 1 / (2N).  lconv(): segments g0 .. g0 + nseg - 1 of the linear convolution map m
 // (real::SegMap, DESIGN.md §4.12), out of place; segment g uses spectrum row (g / m.per) mod rows; h = 1 / (2N).
+// stft(): the rfft of the windowed frames g0 .. g0 + nframes - 1 of the frame map m (real::FrameMap, DESIGN.md
+// §4.13) into consecutive spectrum rows from `out` on.
 template <typename T> struct RealOnChipOps {
   int ra, rb;
   cudaError_t (*prepare)();
@@ -306,6 +308,8 @@ template <typename T> struct RealOnChipOps {
                       size_t row0, size_t per, size_t batch, T h, int sms, cudaStream_t);
   cudaError_t (*lconv)(const T* in, T* out, const real::SegMap& m, size_t nseg, const void* twa, const cpx<T>* tab,
                        const cpx<T>* spec, size_t rows, T h, int sms, cudaStream_t);
+  cudaError_t (*stft)(const T* in, const T* win, void* out, const real::FrameMap& m, size_t nframes, const void* twa,
+                      const cpx<T>* tab, int sms, cudaStream_t);
 };
 template <typename T> const RealOnChipOps<T>* real_onchip_lookup(size_t l);
 
@@ -356,6 +360,20 @@ class RealPlan {
   cudaError_t linear_convolve_host(const T* in, size_t in_len, const C* spec, size_t rows, size_t taps, int mode,
                                    T* out, size_t batch);
 
+  // Short-time Fourier transform (DESIGN.md §4.13): `batch` rows of in_len reals -> F = real::stft_frames(...) rows of
+  // N/2+1 bins per input row, frame-major, frame f = rfft(window . frame f of the row).  hop >= 1, boundary
+  // real::kStft*, in_len legal for it; checked by the caller.  Out of place only.  Device pointers, on `stream`.
+  cudaError_t stft_device(const T* in, size_t in_len, const T* win, size_t hop, int boundary, C* out, size_t batch,
+                          cudaStream_t stream);
+  // Inverse: `batch` rows of `frames` spectra -> rows of out_len reals, the windowed overlap-add of the frames' irfft
+  // divided by the window envelope (0 where it is below 1e-11); pad = N/2 if center.  Device pointers, on `stream`.
+  cudaError_t istft_device(const C* in, size_t frames, const T* win, size_t hop, bool center, T* out, size_t out_len,
+                           size_t batch, cudaStream_t stream);
+  // Host pointers: the window is staged once, whole rows in chunks through stage_rows; the same device code and bits.
+  cudaError_t stft_host(const T* in, size_t in_len, const T* win, size_t hop, int boundary, C* out, size_t batch);
+  cudaError_t istft_host(const C* in, size_t frames, const T* win, size_t hop, bool center, T* out, size_t out_len,
+                         size_t batch);
+
   unsigned long long launches() const { return launches_; }
   const char* kernel_name() const { return kernel_desc_.c_str(); }
 
@@ -394,8 +412,10 @@ class RealPlan {
   DeviceBuffer tab_, twa_;           // w_N^k, k <= N/4 (even N); stage twiddles of the fused kernel
   DeviceBuffer work_;                // one chunk of inner-plan rows
   DeviceBuffer stage_in_, stage_out_;
-  DeviceBuffer stage_spec_;          // the spectra of convolve_host and linear_convolve_host
-  DeviceBuffer seg_;                 // one chunk of N-real segments of a linear convolution (real_half, real_full)
+  DeviceBuffer stage_spec_;          // the spectra of convolve_host and linear_convolve_host, the window of stft_host
+                                     // and istft_host
+  DeviceBuffer seg_;                 // one chunk of N-real segments of a linear convolution (real_half, real_full), of
+                                     // windowed frames (stft) or of inverted frames (istft)
   cudaStream_t host_stream_ = nullptr;
   std::string kernel_desc_;
 };

@@ -10,6 +10,9 @@
 // conv_pair_kernel and the inner inverse, in place in `out`; widen, FFT, hermitian_mul_kernel, inverse, real part.
 // Linear convolution by overlap-save (DESIGN.md §4.12): onchip_lconv_kernel on the fused path; otherwise chunks of
 // segments gathered into seg_, convolved there in place as above and scattered.
+// Short-time Fourier transform (DESIGN.md §4.13): onchip_stft_kernel on the fused path; otherwise chunks of windowed
+// frames gathered into seg_ and transformed from there by the plan's own rfft.  The inverse inverts runs of frames into
+// seg_ with the plan's own irfft and overlap-adds them on every path.
 #include <algorithm>
 #include <string>
 #include <vector>
@@ -106,6 +109,30 @@ scatter_segments_kernel(const T* __restrict__ seg, T* __restrict__ out, const re
   for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
     const long q = g / m.n;
     real::scatter_one(m, seg, out, q, g - q * m.n);
+  }
+}
+
+// Short-time Fourier transform (real::FrameMap).  gather: one thread per sample p < N of frame q of the launch, the
+// windowed frame into seg.  overlap-add: one thread per output i0 <= i < i1 of rows b0 .. b0 + nb - 1, from the
+// inverted frames in seg (global frames gs on); out is output 0 of row b0, rows out_ld apart.
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+gather_frames_kernel(const T* __restrict__ in, const T* __restrict__ win, T* __restrict__ seg, const real::FrameMap m,
+                     long nframes) {
+  const long total = nframes * m.n;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long q = g / m.n;
+    real::gather_frame_one(m, in, win, seg, q, g - q * m.n);
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+overlap_add_kernel(const T* __restrict__ seg, const T* __restrict__ win, T* __restrict__ out, const real::FrameMap m,
+                   long gs, long b0, long nb, long i0, long i1, long out_ld) {
+  const long cnt = i1 - i0, total = nb * cnt;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long r = g / cnt;
+    real::overlap_add_one(m, seg, win, gs, out + r * out_ld, b0 + r, i0 + (g - r * cnt));
   }
 }
 
@@ -437,6 +464,105 @@ cudaError_t RealPlan<T>::linear_convolve_host(const T* in, size_t in_len, const 
     }
   launches_ = total;
   return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::stft_device(const T* in, size_t in_len, const T* win, size_t hop, int boundary, C* out,
+                                     size_t batch, cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  const real::FrameMap m = real::frame_map((long)n_, (long)in_len, (long)hop, boundary);
+  const size_t total = batch * (size_t)m.frames, bins = n_ / 2 + 1;
+  if (path_ == Path::kRealFused) {
+    FB_CHECK(fused_->stft(in, win, out, m, total, twa_.data(), (const C*)tab_.data(), sm_count_, s));
+    launches_ = 1;
+    return cudaSuccess;
+  }
+  // chunks of frames through seg_: gather the windowed frames, then the plan's own rfft straight into the output rows
+  const size_t chunk = std::min(total, std::max<size_t>(1, kScratchTargetBytes / (n_ * sizeof(T))));
+  FB_CHECK(seg_.reserve(chunk * n_ * sizeof(T)));
+  T* seg = (T*)seg_.data();
+  unsigned long long count = 0;
+  for (size_t q0 = 0; q0 < total; q0 += chunk) {
+    const size_t nq = std::min(chunk, total - q0);
+    real::FrameMap mc = m;
+    mc.g0 = (long)q0;
+    gather_frames_kernel<T><<<grid_for(nq * n_), kThreads, 0, s>>>(in, win, seg, mc, (long)nq);
+    FB_CHECK(cudaGetLastError());
+    FB_CHECK(exec_device(true, seg, out + q0 * bins, nq, kFft, s));
+    count += 1 + launches_;
+  }
+  launches_ = count;
+  return cudaSuccess;
+}
+
+// Runs of frames through seg_ (real::istft_runs): each run's spectra are inverted there by the plan's own irfft, then
+// overlap_add_kernel writes the outputs the run owns.  Every output is written once, by the same sum in the same order
+// wherever the runs are cut.
+template <typename T>
+cudaError_t RealPlan<T>::istft_device(const C* in, size_t frames, const T* win, size_t hop, bool center, T* out,
+                                      size_t out_len, size_t batch, cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  real::FrameMap m = real::frame_map((long)n_, (long)n_, (long)hop, real::kStftNone);
+  m.pad = center ? (long)n_ / 2 : 0;
+  m.frames = (long)frames;
+  m.rcp = 1.0 / (double)frames;
+  const size_t bins = n_ / 2 + 1;
+  const size_t cap = real::istft_scratch_frames(std::max<size_t>(1, kScratchTargetBytes / (n_ * sizeof(T))), n_, hop,
+                                                frames);
+  FB_CHECK(seg_.reserve(std::min(cap, batch * frames) * n_ * sizeof(T)));
+  T* seg = (T*)seg_.data();
+  unsigned long long count = 0;
+  const int e = real::istft_runs(n_, hop, (size_t)m.pad, frames, out_len, batch, cap,
+                                 [&](size_t gs, size_t ge, size_t b0, size_t nb, size_t i0, size_t i1) -> int {
+    FB_CHECK(exec_device(false, in + gs * bins, seg, ge - gs, kIfft, s));
+    count += launches_;
+    overlap_add_kernel<T><<<grid_for(nb * (i1 - i0)), kThreads, 0, s>>>(
+        seg, win, out + b0 * out_len, m, (long)gs, (long)b0, (long)nb, (long)i0, (long)i1, (long)out_len);
+    FB_CHECK(cudaGetLastError());
+    count += 1;
+    return 0;
+  });
+  if (e) return (cudaError_t)e;
+  launches_ = count;
+  return cudaSuccess;
+}
+
+// Host pointers, on the plan's own stream: the window is staged once into stage_spec_, whole rows through stage_rows.
+template <typename T>
+cudaError_t RealPlan<T>::stft_host(const T* in, size_t in_len, const T* win, size_t hop, int boundary, C* out,
+                                   size_t batch) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
+  FB_CHECK(stage_spec_.reserve(n_ * sizeof(T)));
+  FB_CHECK(cudaMemcpyAsync(stage_spec_.data(), win, n_ * sizeof(T), cudaMemcpyHostToDevice, host_stream_));
+  const size_t frames = (size_t)real::frame_map((long)n_, (long)in_len, (long)hop, boundary).frames;
+  return stage_rows(in, out, batch, in_len * sizeof(T), frames * (n_ / 2 + 1) * sizeof(C),
+                    [&](const void* din, void* dout, size_t, size_t nb) {
+                      return stft_device((const T*)din, in_len, (const T*)stage_spec_.data(), hop, boundary, (C*)dout,
+                                         nb, host_stream_);
+                    });
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::istft_host(const C* in, size_t frames, const T* win, size_t hop, bool center, T* out,
+                                    size_t out_len, size_t batch) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
+  FB_CHECK(stage_spec_.reserve(n_ * sizeof(T)));
+  FB_CHECK(cudaMemcpyAsync(stage_spec_.data(), win, n_ * sizeof(T), cudaMemcpyHostToDevice, host_stream_));
+  return stage_rows(in, out, batch, frames * (n_ / 2 + 1) * sizeof(C), out_len * sizeof(T),
+                    [&](const void* din, void* dout, size_t, size_t nb) {
+                      return istft_device((const C*)din, frames, (const T*)stage_spec_.data(), hop, center, (T*)dout,
+                                          out_len, nb, host_stream_);
+                    });
 }
 
 template class RealPlan<float>;

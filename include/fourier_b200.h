@@ -257,6 +257,55 @@ int fourier_b200_linear_convolve_real_async_double(struct fourier_b200_rfft_doub
                                                    size_t taps, int mode, double *out_dev, size_t batch,
                                                    void *cuda_stream);
 
+/* ---- Short-time Fourier transform of real rows ----
+ * On a real plan of length N (the frame length): `batch` rows of in_len = L reals (row b starting at element b*L),
+ * `window` N reals applied to every frame (zero-pad a shorter window to N), hop H >= 1 (H > N leaves gaps).  With
+ * pad = N/2 for FOURIER_B200_STFT_ZEROS / _REFLECT and 0 for _NONE, a row has F = 1 + (L + 2*pad - N) / H frames and
+ *   u_f[p] = x_b[f*H - pad + p] * window[p],  p < N,   out[b][f][k] = rfft(u_f)[k],  k <= N/2 (numpy's scale),
+ * where samples outside [0, L) are 0 (_ZEROS) or mirrored without repeating the edge, -t -> t and L-1+t -> L-1-t
+ * (_REFLECT).  This is torch.stft(x, N, H, window=window, center=boundary != _NONE, pad_mode="constant" / "reflect",
+ * return_complex=True) with the last two dimensions swapped: the output is frame-major, row b starting at complex
+ * element b*F*(N/2+1), each frame one row in the plan's rfft layout (tf.signal.stft's layout).  _NONE needs L >= N,
+ * _REFLECT L > N/2.  Launches: 1 on the real_fused path; otherwise, per scratch chunk of frames, 1 + those of the
+ * plan's rfft of that many rows.
+ * Inverse: `frames` = F >= 1 spectra per row in that layout -> out_len >= 1 reals per row (row b at element b*out_len).
+ * Output i has padded position t = i + pad, pad = N/2 if `center` is non-zero and 0 otherwise, and is
+ *   y[i] = sum_f window[t - f*H] * v_f[t - f*H]  /  sum_f window[t - f*H]^2,   v_f = irfft(out[b][f], n=N),
+ * over the frames f < F with 0 <= t - f*H < N in ascending f (deterministic).  Where the denominator is below 1e-11,
+ * including positions no frame covers, the output is 0 (torch.istft raises there instead).  With out_len =
+ * H*(F-1) + N - 2*pad this is torch.istft(..., center=center, length=out_len).  Launches: per run of frames that fits
+ * the plan's scratch, those of the plan's irfft of the run plus 1.
+ * Refused with cudaErrorInvalidValue and a message: a NULL argument, hop == 0, an unknown boundary, in_len == 0,
+ * frames == 0, out_len == 0 (these also when batch == 0, which otherwise succeeds and launches nothing), in_len < N with
+ * _NONE, in_len <= N/2 with _REFLECT, the input or window overlapping the output (out of place only), and a mix of
+ * host and device buffers in the synchronous calls.  Device base pointers of input and output must be 16-byte
+ * aligned (cudaErrorMisalignedAddress).  Host memory is staged through the plan's buffers (the window once, whole
+ * rows in chunks) and gives the same bits as device memory.  The _async calls take device memory, are enqueued on
+ * `cuda_stream` and not synchronised. */
+#define FOURIER_B200_STFT_NONE 0
+#define FOURIER_B200_STFT_ZEROS 1
+#define FOURIER_B200_STFT_REFLECT 2
+int fourier_b200_stft_float(struct fourier_b200_rfft_float *plan, const float *in, size_t in_len, const float *window,
+                            size_t hop, int boundary, void *out, size_t batch);
+int fourier_b200_stft_double(struct fourier_b200_rfft_double *plan, const double *in, size_t in_len,
+                             const double *window, size_t hop, int boundary, void *out, size_t batch);
+int fourier_b200_stft_async_float(struct fourier_b200_rfft_float *plan, const float *in_dev, size_t in_len,
+                                  const float *window_dev, size_t hop, int boundary, void *out_dev, size_t batch,
+                                  void *cuda_stream);
+int fourier_b200_stft_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev, size_t in_len,
+                                   const double *window_dev, size_t hop, int boundary, void *out_dev, size_t batch,
+                                   void *cuda_stream);
+int fourier_b200_istft_float(struct fourier_b200_rfft_float *plan, const void *in, size_t frames, const float *window,
+                             size_t hop, int center, float *out, size_t out_len, size_t batch);
+int fourier_b200_istft_double(struct fourier_b200_rfft_double *plan, const void *in, size_t frames,
+                              const double *window, size_t hop, int center, double *out, size_t out_len, size_t batch);
+int fourier_b200_istft_async_float(struct fourier_b200_rfft_float *plan, const void *in_dev, size_t frames,
+                                   const float *window_dev, size_t hop, int center, float *out_dev, size_t out_len,
+                                   size_t batch, void *cuda_stream);
+int fourier_b200_istft_async_double(struct fourier_b200_rfft_double *plan, const void *in_dev, size_t frames,
+                                    const double *window_dev, size_t hop, int center, double *out_dev, size_t out_len,
+                                    size_t batch, void *cuda_stream);
+
 const char *fourier_b200_last_error(void);
 const char *fourier_b200_version(void);
 
