@@ -25,21 +25,23 @@ template <typename T> struct ColumnOps {
                         cudaStream_t s);
 };
 
-// register tile Shape (twopass_kernels.cuh) of the outer pass, C columns per CTA
-template <typename T, class S, int MINB> struct ColumnImpl {
-  template <bool FWD> using Tile = TileFFT<T, S::RA, S::RB, S::E, S::C, FWD>;
-  using Lay = ExLayout<S::RA * S::C + S::PAD, S::C, 1>;
-  static constexpr size_t smem = sizeof(cpx<T>) * Tile<true>::template smem_elems<Lay>();
+// the launcher of one outer pass Col (outer::ColumnCfg)
+template <class Col> struct ColumnImpl {
+  using T = typename Col::T;
+  using S = typename Col::Shape;
+  using Lay = typename Col::Lay;
+  static constexpr size_t smem = sizeof(cpx<T>) * Col::template Tile<true>::template smem_elems<Lay>();
   template <bool FWD>
   static cudaError_t run(const cpx<T>* in, cpx<T>* out, const void* twa, size_t nb, size_t batch, T scale, cudaStream_t s) {
-    using Body = outer::ColumnBody<Tile<FWD>, Lay>;
-    auto kernel = &outer::column_kernel<Body, Tile<FWD>, MINB>;
+    using Tile = typename Col::template Tile<FWD>;
+    using Body = typename Col::template Body<FWD>;
+    auto kernel = &outer::column_kernel<Body, Tile, Col::MINB>;
     static std::atomic<unsigned long long> prepared{0};
     if (cudaError_t e = ensure_dynamic_smem(kernel, smem, prepared)) return e;
     typename Body::Args a;
     a.in = in; a.out = out; a.twa = (const TwPair<T>*)twa;
     a.nb = nb; a.n_total = (unsigned long long)S::L * nb; a.tiles = (unsigned)(nb / S::C); a.scale = scale;
-    kernel<<<(unsigned)(batch * (nb / S::C)), Tile<FWD>::THREADS, smem, s>>>(a);
+    kernel<<<(unsigned)(batch * (nb / S::C)), Tile::THREADS, smem, s>>>(a);
     return cudaGetLastError();
   }
   static cudaError_t launch(const cpx<T>* in, cpx<T>* out, const void* twa, size_t nb, size_t batch, T scale, bool fwd,
@@ -52,28 +54,11 @@ template <typename T, class S, int MINB> struct ColumnImpl {
   }
 };
 
-using twopass::Shape;
-template <typename T> const ColumnOps<T>* column_lookup(int log2_na);
-template <> const ColumnOps<float>* column_lookup<float>(int a) {
-  switch (a) {   // the pass-1 shapes of the two-pass configurations (bank-conflict-free paddings checked by the emulator)
-    case 5: return ColumnImpl<float, Shape<4, 8, 8, 32, 0>, 4>::ops();
-    case 6: return ColumnImpl<float, Shape<8, 8, 8, 32, 0>, 4>::ops();
-    case 7: return ColumnImpl<float, Shape<8, 16, 16, 16, 0>, 4>::ops();
-    case 8: return ColumnImpl<float, Shape<16, 16, 16, 16, 0>, 2>::ops();
-    case 9: return ColumnImpl<float, Shape<16, 32, 32, 8, 8>, 2>::ops();
-    case 10: return ColumnImpl<float, Shape<32, 32, 32, 8, 8>, 2>::ops();
-    default: return nullptr;
-  }
-}
-template <> const ColumnOps<double>* column_lookup<double>(int a) {
-  switch (a) {
-    case 4: return ColumnImpl<double, Shape<4, 4, 4, 16, 0>, 4>::ops();
-    case 5: return ColumnImpl<double, Shape<4, 8, 8, 16, 0>, 4>::ops();
-    case 6: return ColumnImpl<double, Shape<8, 8, 8, 16, 0>, 4>::ops();
-    case 7: return ColumnImpl<double, Shape<8, 16, 16, 8, 4>, 2>::ops();
-    case 8: return ColumnImpl<double, Shape<16, 16, 16, 8, 4>, 2>::ops();
-    default: return nullptr;
-  }
+// the outer pass of length 2^log2_na (outer::visit_column), nullptr when there is none
+template <typename T> const ColumnOps<T>* column_lookup(int log2_na) {
+  const ColumnOps<T>* o = nullptr;
+  outer::visit_column<T>(log2_na, [&](auto col) { o = ColumnImpl<decltype(col)>::ops(); });
+  return o;
 }
 
 // outer radix-3 / 9 / 27 pass: one thread per column

@@ -5,7 +5,6 @@
 // traffic) runs beside pass 2 of another (NVLink stores).
 #include <algorithm>
 #include <cstdlib>
-#include <type_traits>
 
 #include "dist_kernels.cuh"
 #include "plan.h"
@@ -21,17 +20,10 @@ template <typename T> struct RowsExchangeCall {
   size_t r0, out_bs; int rb_shift; size_t rpb, rows_valid;
 };
 
-// Tiles of twice as many transforms where the configuration's pass-2 tile has 16 (f32) / 8 (f64): a warp's store is then
-// one 256-byte run instead of two 128-byte pieces.
-// Paddings are the bank-conflict-free ones (tools/emulate.cu).  FOURIER_B200_DIST_WIDE=0 selects the narrow tiles.
-template <class S, typename T> struct WideShape { using type = S; };
-template <> struct WideShape<twopass::Shape<8, 16, 16, 16, 2>, float> { using type = twopass::Shape<8, 16, 16, 32, 2>; };
-template <> struct WideShape<twopass::Shape<16, 16, 16, 16, 1>, float> { using type = twopass::Shape<16, 16, 16, 32, 1>; };
-template <> struct WideShape<twopass::Shape<8, 16, 16, 8, 1>, double> { using type = twopass::Shape<8, 16, 16, 16, 1>; };
-template <> struct WideShape<twopass::Shape<16, 16, 16, 8, 1>, double> { using type = twopass::Shape<16, 16, 16, 16, 1>; };
-
+// The pass-2 tile of configuration G, or its wide tile (dist::ExchangeShape); FOURIER_B200_DIST_WIDE=0 selects the
+// narrow tiles.
 template <class G, bool WIDE, typename T> struct ExchangeTile {
-  using S = typename std::conditional<WIDE, typename WideShape<typename G::Shape2, T>::type, typename G::Shape2>::type;
+  using S = dist::ExchangeShape<G, WIDE, T>;
   template <bool FWD> using Tile = TileFFT<T, S::RA, S::RB, S::E, S::C, FWD>;
   using Lay = ExLayout<S::RA * S::C + S::PAD, S::C, 1>;
   static constexpr int C = S::C;

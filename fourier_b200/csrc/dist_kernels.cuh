@@ -18,9 +18,11 @@
 #pragma once
 
 #include <cmath>
+#include <type_traits>
 
 #include "plan.h"
 #include "tilefft.cuh"
+#include "twopass_kernels.cuh"
 
 namespace fb200 {
 namespace dist {
@@ -124,6 +126,18 @@ template <class Body, class Tile, int MINB>
 __global__ void __launch_bounds__(Tile::THREADS, MINB) rows_exchange_kernel(const typename Body::Args a) {
   run_cta_tile<Tile, Body>(a);
 }
+
+// Tiles of twice as many transforms where the configuration's pass-2 tile has 16 (f32) / 8 (f64): a warp's store is then
+// one 256-byte run instead of two 128-byte pieces.  WideShape<S, T>::type is the wide tile of pass-2 shape S (S itself
+// where there is none); the paddings are the bank-conflict-free ones (tools/emulate.cu).
+template <class S, typename T> struct WideShape { using type = S; };
+template <> struct WideShape<twopass::Shape<8, 16, 16, 16, 2>, float> { using type = twopass::Shape<8, 16, 16, 32, 2>; };
+template <> struct WideShape<twopass::Shape<16, 16, 16, 16, 1>, float> { using type = twopass::Shape<16, 16, 16, 32, 1>; };
+template <> struct WideShape<twopass::Shape<8, 16, 16, 8, 1>, double> { using type = twopass::Shape<8, 16, 16, 16, 1>; };
+template <> struct WideShape<twopass::Shape<16, 16, 16, 8, 1>, double> { using type = twopass::Shape<16, 16, 16, 16, 1>; };
+// the tile shape of the exchange for two-pass configuration G: its wide tile (WIDE) or its pass-2 tile
+template <class G, bool WIDE, typename T>
+using ExchangeShape = typename std::conditional<WIDE, typename WideShape<typename G::Shape2, T>::type, typename G::Shape2>::type;
 
 }  // namespace dist
 }  // namespace fb200

@@ -65,5 +65,13 @@ FB_FUSED_CONFIG(double, 12, true, FusedCfg<double, 8, 8, 8, 4, 8, false>)
 
 #undef FB_FUSED_CONFIG
 
+// for_each_fused_size<T>(f) calls f(std::integral_constant<int, LOG2N>{}) for every N = 2^LOG2N with a configuration
+// above, smallest first: the size list of the library's fused_lookup and of the emulator.
+template <typename T, class F> void for_each_fused_size(F&& f) {
+  static_for<1, 31>([&](auto k) {
+    if constexpr (FusedConfig<T, decltype(k)::value>::HAS) f(k);
+  });
+}
+
 }  // namespace fused
 }  // namespace fb200

@@ -5,17 +5,14 @@
 // Bluesteins::transform_in_place / apply (bluesteins.rs:193-259).
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 
-#include "onchip_kernels.cuh"
+#include "onchip_configs.cuh"
 #include "plan.h"
 #include "tables.cuh"  // make_twa
 
 namespace fb200 {
 
 namespace {
-
-using onchip::OnChipCfg;
 
 template <typename T> struct OnChipOps {
   int ra, rb;
@@ -29,14 +26,19 @@ template <typename T> struct OnChipOps {
   const RealOnChipOps<T>* real;   // real-input transforms of length 2L on the same tiles
 };
 
-template <typename T, int RA, int RB, int E, int WARPS, int MINB, int BWARPS, bool LOCAL_STASH = false>
+// the launchers of one size class K (onchip_configs.cuh)
+template <class K>
 struct OnChipImpl {
-  template <bool FWD> using Cfg = OnChipCfg<T, RA, RB, E, WARPS, FWD>;
-  using BCfg = OnChipCfg<T, RA, RB, E, BWARPS, true>;
+  using T = typename K::T;
+  static constexpr int RA = K::RA, RB = K::RB, MINB = K::MINB;
+  static constexpr bool kHasBluestein = K::kHasBluestein;
+  template <bool FWD> using Cfg = typename K::template Cfg<FWD>;
+  using BCfg = typename K::BCfg;
   static constexpr size_t smem_fft = Cfg<true>::EX_BYTES + Cfg<true>::TWA_BYTES;
-  static constexpr size_t smem_blue =
-      BCfg::EX_BYTES + BCfg::TWA_BYTES + sizeof(cpx<T>) * (4 * (size_t)BCfg::L + (LOCAL_STASH ? 0 : (size_t)E * BCfg::THREADS));
-  static constexpr bool kHasBluestein = (RA == RB) && (E == RA);
+  static constexpr size_t smem_blue() {
+    return BCfg::EX_BYTES + BCfg::TWA_BYTES +
+           sizeof(cpx<T>) * (4 * (size_t)BCfg::L + (K::LOCAL_STASH ? 0 : (size_t)K::E * BCfg::THREADS));
+  }
 
   // the fft / real / conv kernels: the exchange and the stage twiddles in shared memory, groups of C transforms
   // grid-stride over at most sms * MINB * 4 CTAs
@@ -56,8 +58,8 @@ struct OnChipImpl {
     if ((e = allow_smem(onchip::onchip_fft_kernel<Cfg<true>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_fft_kernel<Cfg<false>, MINB>))) return e;
     if constexpr (kHasBluestein) {
-      if ((e = cudaFuncSetAttribute(onchip::bluestein_fused_kernel<BCfg, 1, LOCAL_STASH>,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_blue))) return e;
+      if ((e = cudaFuncSetAttribute(onchip::bluestein_fused_kernel<BCfg, 1, K::LOCAL_STASH>,
+                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_blue()))) return e;
     }
     return cudaSuccess;
   }
@@ -77,7 +79,7 @@ struct OnChipImpl {
       const unsigned grid = (unsigned)std::min<size_t>(groups, (size_t)sms * 2);
       typename onchip::BluesteinBody<BCfg>::Args a = {in, out, (const TwPair<T>*)twa, chirp, wm, wce, wco,
                                                       (long)n, (long)batch, scale};
-      onchip::bluestein_fused_kernel<BCfg, 1, LOCAL_STASH><<<grid, BCfg::THREADS, smem_blue, s>>>(a);
+      onchip::bluestein_fused_kernel<BCfg, 1, K::LOCAL_STASH><<<grid, BCfg::THREADS, smem_blue(), s>>>(a);
       return cudaGetLastError();
     } else {
       return cudaErrorNotSupported;
@@ -133,30 +135,11 @@ struct OnChipImpl {
   }
 };
 
-// size classes: L -> (RA, RB, E, warps per CTA, CTAs per SM, warps per CTA of the Bluestein kernel)
-template <typename T> const OnChipOps<T>* onchip_lookup(size_t l);
-template <> const OnChipOps<float>* onchip_lookup<float>(size_t l) {
-  switch (l) {
-    case 64: return OnChipImpl<float, 8, 8, 8, 8, 4, 8>::ops();
-    case 128: return OnChipImpl<float, 8, 16, 16, 8, 4, 8>::ops();
-    case 256: return OnChipImpl<float, 16, 16, 16, 8, 3, 8>::ops();
-    case 512: return OnChipImpl<float, 16, 32, 32, 8, 2, 8>::ops();
-    case 1024:
-      // The fused Bluestein kernel parks the even half in thread-local memory (16 warps per SM);
-      // FOURIER_B200_BLUESTEIN_LOCAL=0 selects the shared-memory stash (11 warps per SM).
-      if (const char* e = std::getenv("FOURIER_B200_BLUESTEIN_LOCAL"); e && atoi(e) == 0)
-        return OnChipImpl<float, 32, 32, 32, 8, 2, 11>::ops();
-      return OnChipImpl<float, 32, 32, 32, 8, 2, 16, true>::ops();
-    default: return nullptr;
-  }
-}
-template <> const OnChipOps<double>* onchip_lookup<double>(size_t l) {
-  switch (l) {
-    case 64: return OnChipImpl<double, 8, 8, 8, 8, 3, 8>::ops();
-    case 128: return OnChipImpl<double, 8, 16, 16, 8, 2, 8>::ops();
-    case 256: return OnChipImpl<double, 16, 16, 16, 8, 1, 8>::ops();
-    default: return nullptr;
-  }
+// the size class of length l (onchip_configs.cuh), nullptr when there is none
+template <typename T> const OnChipOps<T>* onchip_lookup(size_t l) {
+  const OnChipOps<T>* o = nullptr;
+  onchip::visit_onchip<T>(l, [&](auto k) { o = OnChipImpl<decltype(k)>::ops(); });
+  return o;
 }
 
 }  // namespace

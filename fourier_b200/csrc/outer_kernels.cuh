@@ -16,6 +16,7 @@
 
 #include "dist_kernels.cuh"
 #include "tilefft.cuh"
+#include "twopass_kernels.cuh"
 
 namespace fb200 {
 namespace outer {
@@ -79,6 +80,47 @@ struct ColumnBody {
 template <class Body, class Tile, int MINB>
 __global__ void __launch_bounds__(Tile::THREADS, MINB) column_kernel(const typename Body::Args a) {
   run_cta_tile<Tile, Body>(a);
+}
+
+// The outer pass of length Na = S::L: register tile Shape S (twopass_kernels.cuh) over C = S::C columns per CTA, at
+// least MINB CTAs per SM.
+template <typename T_, class S, int MINB_> struct ColumnCfg {
+  using T = T_;
+  using Shape = S;
+  static constexpr int MINB = MINB_;
+  template <bool FWD> using Tile = TileFFT<T, S::RA, S::RB, S::E, S::C, FWD>;
+  using Lay = ExLayout<S::RA * S::C + S::PAD, S::C, 1>;
+  template <bool FWD> using Body = ColumnBody<Tile<FWD>, Lay>;
+};
+
+// visit_column<T>(log2_na, f) calls f with a value of the outer pass of length 2^log2_na (false when there is none):
+// the pass-1 shapes of the two-pass configurations, whose paddings keep the exchange bank-conflict free.
+template <class F> bool visit_column_f32(int log2_na, F&& f) {
+  using twopass::Shape;
+  switch (log2_na) {
+    case 5: f(ColumnCfg<float, Shape<4, 8, 8, 32, 0>, 4>{}); return true;
+    case 6: f(ColumnCfg<float, Shape<8, 8, 8, 32, 0>, 4>{}); return true;
+    case 7: f(ColumnCfg<float, Shape<8, 16, 16, 16, 0>, 4>{}); return true;
+    case 8: f(ColumnCfg<float, Shape<16, 16, 16, 16, 0>, 2>{}); return true;
+    case 9: f(ColumnCfg<float, Shape<16, 32, 32, 8, 8>, 2>{}); return true;
+    case 10: f(ColumnCfg<float, Shape<32, 32, 32, 8, 8>, 2>{}); return true;
+    default: return false;
+  }
+}
+template <class F> bool visit_column_f64(int log2_na, F&& f) {
+  using twopass::Shape;
+  switch (log2_na) {
+    case 4: f(ColumnCfg<double, Shape<4, 4, 4, 16, 0>, 4>{}); return true;
+    case 5: f(ColumnCfg<double, Shape<4, 8, 8, 16, 0>, 4>{}); return true;
+    case 6: f(ColumnCfg<double, Shape<8, 8, 8, 16, 0>, 4>{}); return true;
+    case 7: f(ColumnCfg<double, Shape<8, 16, 16, 8, 4>, 2>{}); return true;
+    case 8: f(ColumnCfg<double, Shape<16, 16, 16, 8, 4>, 2>{}); return true;
+    default: return false;
+  }
+}
+template <typename T, class F> bool visit_column(int log2_na, F&& f) {
+  if constexpr (sizeof(T) == 4) return visit_column_f32(log2_na, f);
+  else return visit_column_f64(log2_na, f);
 }
 
 // Outer pass of length B = 3, 9 or 27 for N = B * Nb (Nb a two-pass power of two): the radix-3 stages of the

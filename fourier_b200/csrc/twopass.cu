@@ -110,28 +110,12 @@ template <typename T, int LOG2N> const FusedOps<T>* fused_pick() {
   return FusedImpl<typename D::Cfg>::ops(D::RING, D::LAG);
 }
 
-template <typename T> const FusedOps<T>* fused_lookup(size_t n);
-template <> const FusedOps<float>* fused_lookup<float>(size_t n) {
-  switch (n) {
-    case (size_t)1 << 13: return fused_pick<float, 13>();
-    case (size_t)1 << 14: return fused_pick<float, 14>();
-    case (size_t)1 << 15: return fused_pick<float, 15>();
-    case (size_t)1 << 16: return fused_pick<float, 16>();
-    case (size_t)1 << 17: return fused_pick<float, 17>();
-    case (size_t)1 << 18: return fused_pick<float, 18>();
-    case (size_t)1 << 19: return fused_pick<float, 19>();
-    case (size_t)1 << 20: return fused_pick<float, 20>();
-  }
-  return nullptr;
-}
-template <> const FusedOps<double>* fused_lookup<double>(size_t n) {
-  switch (n) {
-    case (size_t)1 << 12: return fused_pick<double, 12>();
-    case (size_t)1 << 13: return fused_pick<double, 13>();
-    case (size_t)1 << 14: return fused_pick<double, 14>();
-    case (size_t)1 << 16: return fused_pick<double, 16>();
-  }
-  return nullptr;
+template <typename T> const FusedOps<T>* fused_lookup(size_t n) {
+  const FusedOps<T>* o = nullptr;
+  fused::for_each_fused_size<T>([&](auto k) {
+    if (n == (size_t)1 << decltype(k)::value) o = fused_pick<T, decltype(k)::value>();
+  });
+  return o;
 }
 
 }  // namespace

@@ -2,7 +2,6 @@
 // path.  Shared by twopass.cu (the product) and tools/emulate.cu (CPU emulation of the same code).
 #pragma once
 
-#include <cstdlib>
 #include <vector>
 
 #include "plan.h"
@@ -141,15 +140,10 @@ using TwoPass = TwoPassG<T, Shape<R1, R1, R1, C1, PAD1>, Shape<R2, R2, R2, C2, 1
 
 // Supported sizes.  f32: 32x32 register stages (1024-point tiles); f64: 16x16 (256-point tiles).
 // visit_config<T>(n, f) calls f with a value of the configuration type of size n (false when there is none): the one
-// list of sizes behind lookup() here and behind the distributed variant of pass 2 (dist_fft.cu).
+// list of sizes behind lookup() here, the distributed variant of pass 2 (dist_fft.cu) and the CPU emulator.
 template <class F> bool visit_config_f32(size_t n, F&& f) {
   switch (n) {
-    case (size_t)1 << 20: {
-      const char* env = std::getenv("FOURIER_B200_TILE");  // experiment knob: columns per tile
-      if (env && atoi(env) == 16) f(TwoPass<float, 32, 32, 16, 16, 0, 1, 1>{});
-      else f(TwoPass<float, 32, 32, 8, 8, 8, 2, 2>{});
-      return true;
-    }
+    case (size_t)1 << 20: f(TwoPass<float, 32, 32, 8, 8, 8, 2, 2>{}); return true;
     case (size_t)1 << 11: f(TwoPassG<float, Shape<4, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>{}); return true;
     case (size_t)1 << 12: f(TwoPassG<float, Shape<8, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>{}); return true;
     case (size_t)1 << 13: f(TwoPassG<float, Shape<8, 8, 8, 32, 0>, Shape<8, 16, 16, 16, 2>, 4, 4>{}); return true;

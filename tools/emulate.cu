@@ -14,13 +14,9 @@
 #include "outer_kernels.cuh"
 #include "twopass_kernels.cuh"
 
-#ifndef FB_PAD16
-#define FB_PAD16 8
-#endif
-#ifndef FB_PADX
-#define FB_PADX 8
-#endif
 using namespace fb200::twopass;
+
+template <typename T> static const char* prec() { return sizeof(T) == 4 ? "f32" : "f64"; }
 
 // Bank-conflict report for the exchange of a tile: scatter with mapping UF_A, gather with col-fast.
 template <class Tile, class LAY, int UF_A, int UF_B = 0>
@@ -107,8 +103,11 @@ static int check(const char* name, double tol) {
 }
 
 // ---- on-chip kernels (onchip_kernels.cuh) -------------------------------------------------------------------------
-template <typename T, int RA, int RB, int E, int WARPS>
+// size class K of onchip_configs.cuh
+template <class K>
 static int check_onchip(const char* name, double tol) {
+  using T = typename K::T;
+  constexpr int RA = K::RA, RB = K::RB;
   int bad = 0;
   for (int fwd = 1; fwd >= 0; --fwd) {
     const long L = RA * RB, batch = 5;   // 5 is not a multiple of the transforms per CTA: exercises the tail
@@ -122,7 +121,7 @@ static int check_onchip(const char* name, double tol) {
                                                             (batch + Cfg::C - 1) / Cfg::C, twa.data());
       report_conflicts<typename Cfg::Tile, typename Cfg::Lay, true, true>("exchange");
     };
-    if (fwd) run(onchip::OnChipCfg<T, RA, RB, E, WARPS, true>{}); else run(onchip::OnChipCfg<T, RA, RB, E, WARPS, false>{});
+    if (fwd) run(typename K::template Cfg<true>{}); else run(typename K::template Cfg<false>{});
     double worst = 0;
     for (long b = 0; b < batch; ++b) {
       std::vector<double> re(L), im(L);
@@ -141,11 +140,15 @@ static int check_onchip(const char* name, double tol) {
   return bad;
 }
 
-template <typename T, int R, int WARPS>
+// the fused Bluestein kernel of size class K (onchip_configs.cuh), at its warps per CTA and with its stash of the even
+// half: shared memory (stash_even, combine_store) or, with LOCAL_STASH, a per-thread array (combine_store_local)
+template <class K>
 static int check_bluestein(const char* name, long n, double tol) {
-  using Cfg = onchip::OnChipCfg<T, R, R, R, WARPS, true>;
+  using T = typename K::T;
+  using Cfg = typename K::BCfg;
   using Body = onchip::BluesteinBody<Cfg>;
   using V = cpx<T>;
+  constexpr int R = K::RA, E = K::E;
   const long L = R * R, M = 2 * L, batch = 3;
   int bad = 0;
   for (int inverse = 0; inverse < 2; ++inverse) {
@@ -174,7 +177,9 @@ static int check_bluestein(const char* name, long n, double tol) {
     typename Body::Args a = {x.data(), out.data(), twa.data(), chirp.data(), wm.data(), wce.data(), wco.data(), n, batch,
                              (T)(1.0 / M)};
     std::vector<V> exch(Cfg::Tile::template smem_elems<typename Cfg::Lay>());
-    std::vector<V> stash((size_t)R * Cfg::THREADS);
+    std::vector<V> stash((size_t)E * Cfg::THREADS);
+    struct Keep { V v[E]; };
+    std::vector<Keep> keep(Cfg::THREADS);
     std::vector<typename Cfg::Tile> thr(Cfg::THREADS);
     const long groups = (batch + Cfg::C - 1) / Cfg::C;
     auto all = [&](auto fn) { for (int t = 0; t < Cfg::THREADS; ++t) fn(t); };
@@ -187,9 +192,16 @@ static int check_bluestein(const char* name, long n, double tol) {
         all([&](int t) { Body::middle(thr[t], t, exch.data(), odd ? wco.data() : wce.data()); });
         all([&](int t) { Body::second_fft_start(thr[t], t, exch.data(), twa.data()); });
         all([&](int t) { Body::second_fft_finish(thr[t], t, exch.data()); });
-        if (!odd) all([&](int t) { Body::stash_even(thr[t], t, stash.data()); });
+        if (!odd) all([&](int t) {
+          if constexpr (K::LOCAL_STASH) { for (int i = 0; i < E; ++i) keep[t].v[i] = thr[t].v[i]; }
+          else Body::stash_even(thr[t], t, stash.data());
+        });
       }
-      all([&](int t) { if (bidx(t) < batch) Body::combine_store(stash.data(), thr[t], a, bcl(t), t, chirp.data(), wm.data()); });
+      all([&](int t) {
+        if (bidx(t) >= batch) return;
+        if constexpr (K::LOCAL_STASH) Body::combine_store_local(keep[t].v, thr[t], a, bcl(t), t, chirp.data(), wm.data());
+        else Body::combine_store(stash.data(), thr[t], a, bcl(t), t, chirp.data(), wm.data());
+      });
     }
     double worst = 0;
     for (long b = 0; b < batch; ++b) {
@@ -208,7 +220,8 @@ static int check_bluestein(const char* name, long n, double tol) {
       }
       worst = std::max(worst, me / mr);
     }
-    printf("%s N=%ld (L=%ld) %s: max rel err vs naive f64 DFT %.3e %s\n", name, n, L, inverse ? "inverse" : "forward", worst,
+    printf("%s N=%ld (L=%ld) %s: %d warps, %s stash, max rel err vs naive f64 DFT %.3e %s\n", name, n, L,
+           inverse ? "inverse" : "forward", Cfg::THREADS / 32, K::LOCAL_STASH ? "per-thread" : "shared", worst,
            worst < tol ? "OK" : "FAIL");
     bad += !(worst < tol);
   }
@@ -495,10 +508,11 @@ static int check_cta(const char* name, int n, bool chirp_mode, double tol) {
 // ---- row FFTs with the exchange folded into the store of pass 2 (dist_kernels.cuh) -----------------------------
 // pass 1 of the configuration as it is, then RowsExchangeBody with P destination buffers in host memory; reference:
 // dst_q[c * out_ld + out_off + r] = FFT(row r)[q * cb + c] * w_Ntot^{(row0 + r) * (q * cb + c)}
-// SW: shape of the tile (default: the configuration's pass-2 shape; dist_fft.cu also uses tiles of twice as many
-// transforms, WideShape)
-template <typename T, class Cfg, int TW, class SW = typename Cfg::Shape2>
+// WIDE: the tile of twice as many transforms that dist_fft.cu also uses, else the configuration's pass-2 tile
+// (dist::ExchangeShape)
+template <typename T, class Cfg, int TW, bool WIDE>
 static int check_rows_exchange(const char* name, int P, double tol) {
+  using SW = dist::ExchangeShape<Cfg, WIDE, T>;
   constexpr bool FWD = TW != 2;
   const long N = Cfg::N, N1 = Cfg::N1, N2 = Cfg::N2;
   using Tile = TileFFT<T, SW::RA, SW::RB, SW::E, SW::C, FWD>;
@@ -560,12 +574,14 @@ static int check_rows_exchange(const char* name, int P, double tol) {
 }
 
 // ---- three-pass path (bigpow2.cu): outer column pass + two-pass rows with the transposed store ---------------------
-template <typename T, class SO, class Cfg, bool FWD>
+// Col: the outer pass (outer::visit_column), Cfg: the two-pass configuration of the rows
+template <typename T, class Col, class Cfg, bool FWD>
 static int check_threepass(const char* name, double tol) {
+  using SO = typename Col::Shape;
   const long Na = SO::L, Nb = Cfg::N, N = Na * Nb;
-  using TileO = TileFFT<T, SO::RA, SO::RB, SO::E, SO::C, FWD>;
-  using LayO = ExLayout<SO::RA * SO::C + SO::PAD, SO::C, 1>;
-  using BodyO = outer::ColumnBody<TileO, LayO>;
+  using TileO = typename Col::template Tile<FWD>;
+  using LayO = typename Col::Lay;
+  using BodyO = typename Col::template Body<FWD>;
   const long B = 2;   // two long transforms in one call
   std::vector<cpx<T>> x(B * N), work(B * N), scratch(B * N), out(B * N);
   fill<T>(x, 31 + FWD);
@@ -665,37 +681,122 @@ static int check_threepass_radix3(const char* name, double tol) {
   return !(maxerr / maxref < tol && untouched == 0 && nans == 0);
 }
 
+// ---- the configurations of the library's tables -------------------------------------------------------------------
+// f with the two-pass configuration of N = 2^log2n (twopass::visit_config); a size without one is a failure
+template <typename T, class F> static int with_config(int log2n, F&& f) {
+  int bad = -1;
+  visit_config<T>((size_t)1 << log2n, [&](auto g) { bad = f(g); });
+  if (bad < 0) printf("%s 2^%d: no two-pass configuration FAIL\n", prec<T>(), log2n);
+  return bad < 0 ? 1 : bad;
+}
+
+// every two-pass configuration
+template <typename T> static int check_twopass(double tol) {
+  int bad = 0;
+  for (int k = 1; k <= 30; ++k)
+    visit_config<T>((size_t)1 << k, [&](auto g) {
+      char name[32];
+      snprintf(name, sizeof name, "%s 2^%d", prec<T>(), k);
+      bad += check<T, decltype(g)>(name, tol);
+    });
+  return bad;
+}
+
+template <typename T, int TW, bool WIDE = false> static int rows_exchange(int log2n, int P, double tol) {
+  char name[32];
+  snprintf(name, sizeof name, "%s 2^%d%s", prec<T>(), log2n, WIDE ? " wide" : "");
+  return with_config<T>(log2n, [&](auto g) { return check_rows_exchange<T, decltype(g), TW, WIDE>(name, P, tol); });
+}
+
+// the outer pass of every length (outer::visit_column), both directions, before rows of N = 2^log2nb
+template <typename T> static int threepass(int log2nb, double tol) {
+  int bad = 0;
+  for (int a = 1; a <= 30; ++a)
+    outer::visit_column<T>(a, [&](auto col) {
+      char name[32];
+      snprintf(name, sizeof name, "%s 2^%d", prec<T>(), a + log2nb);
+      bad += with_config<T>(log2nb, [&](auto g) {
+        return check_threepass<T, decltype(col), decltype(g), true>(name, tol) +
+               check_threepass<T, decltype(col), decltype(g), false>(name, tol);
+      });
+    });
+  return bad;
+}
+
+template <typename T, int B, bool FWD> static int threepass_radix3(int log2nb, double tol) {
+  char name[32];
+  snprintf(name, sizeof name, "%s %d*2^%d", prec<T>(), B, log2nb);
+  return with_config<T>(log2nb, [&](auto g) { return check_threepass_radix3<T, B, decltype(g), FWD>(name, tol); });
+}
+
+// the fused Bluestein kernel of the size class of M = next_pow2(2N - 1) = 2L; a class without one is a failure
+template <typename T> static int bluestein(long n, double tol) {
+  size_t m = 1;
+  while (m < (size_t)(2 * n - 1)) m *= 2;
+  int bad = -1;
+  onchip::visit_onchip<T>(m / 2, [&](auto k) {
+    if constexpr (decltype(k)::kHasBluestein) {
+      char name[32];
+      snprintf(name, sizeof name, "bluestein %s", prec<T>());
+      bad = check_bluestein<decltype(k)>(name, n, tol);
+    }
+  });
+  if (bad < 0) printf("bluestein %s N=%ld: no fused Bluestein class FAIL\n", prec<T>(), n);
+  return bad < 0 ? 1 : bad;
+}
+
+// the persistent kernel of N = 2^LOG2N (fused_configs.cuh): the default configuration and the alternative
+// (FOURIER_B200_CFG=1) where there is one; pair items (PairCfg) change only which tiles a group claims, so the default
+// runs as its Unpaired configuration
+template <typename T, int LOG2N> static int check_persistent(double tol) {
+  using D = fused::FusedConfig<T, LOG2N>;
+  using A = fused::FusedConfig<T, LOG2N, true>;
+  char name[64];
+  snprintf(name, sizeof name, "fused %s 2^%d", prec<T>(), LOG2N);
+  int bad = check_fused<typename D::Cfg::Unpaired>(name, tol);
+  if constexpr (A::HAS) {
+    snprintf(name, sizeof name, "fused %s 2^%d (FOURIER_B200_CFG=1)", prec<T>(), LOG2N);
+    bad += check_fused<typename A::Cfg>(name, tol);
+  }
+  return bad;
+}
+
+// the work queue of the default configuration of N = 2^LOG2N, and with pair items also the one item per group that
+// FOURIER_B200_PAIR=0 selects
+template <typename T, int LOG2N> static int check_queues() {
+  using D = fused::FusedConfig<T, LOG2N>;
+  char name[64];
+  snprintf(name, sizeof name, "%s 2^%d", prec<T>(), LOG2N);
+  int bad = check_queue<D>(name);
+  if constexpr (D::Cfg::PAIR) {
+    struct Single : D { using Cfg = typename D::Cfg::Unpaired; };
+    snprintf(name, sizeof name, "%s 2^%d (FOURIER_B200_PAIR=0)", prec<T>(), LOG2N);
+    bad += check_queue<Single>(name);
+  }
+  return bad;
+}
+
 int main() {
   int bad = 0;
-  bad += check_threepass_radix3<float, 3, TwoPassG<float, Shape<4, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>, true>("f32 3*2^11", 2e-6);
-  bad += check_threepass_radix3<float, 9, TwoPassG<float, Shape<4, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>, false>("f32 9*2^11", 2e-6);
-  bad += check_threepass_radix3<float, 27, TwoPassG<float, Shape<4, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>, true>("f32 27*2^11", 2e-6);
-  bad += check_threepass_radix3<double, 27, TwoPassG<double, Shape<4, 4, 4, 16, 0>, Shape<4, 8, 8, 16, 2>, 4, 4>, false>("f64 27*2^9", 1e-14);
-  bad += check_threepass_radix3<double, 3, TwoPassG<double, Shape<4, 4, 4, 16, 0>, Shape<4, 8, 8, 16, 2>, 4, 4>, true>("f64 3*2^9", 1e-14);
-  bad += check_threepass<float, Shape<4, 8, 8, 32, 0>, TwoPassG<float, Shape<4, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>, true>("f32 2^16", 2e-6);
-  bad += check_threepass<float, Shape<8, 16, 16, 16, 0>, TwoPassG<float, Shape<4, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>, false>("f32 2^18", 2e-6);
-  bad += check_threepass<double, Shape<4, 4, 4, 16, 0>, TwoPassG<double, Shape<4, 4, 4, 16, 0>, Shape<4, 8, 8, 16, 2>, 4, 4>, true>("f64 2^13", 5e-15);
-  bad += check_threepass<double, Shape<8, 16, 16, 8, 4>, TwoPassG<double, Shape<4, 4, 4, 16, 0>, Shape<4, 8, 8, 16, 2>, 4, 4>, false>("f64 2^16", 5e-15);
-  // the remaining outer-pass shapes of bigpow2.cu's column_lookup
-  bad += check_threepass<float, Shape<8, 8, 8, 32, 0>, TwoPassG<float, Shape<4, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>, true>("f32 2^17", 2e-6);
-  bad += check_threepass<float, Shape<16, 16, 16, 16, 0>, TwoPassG<float, Shape<4, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>, true>("f32 2^19", 2e-6);
-  bad += check_threepass<float, Shape<16, 32, 32, 8, 8>, TwoPassG<float, Shape<4, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>, false>("f32 2^20", 2e-6);
-  bad += check_threepass<float, Shape<32, 32, 32, 8, 8>, TwoPassG<float, Shape<4, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>, true>("f32 2^21", 2e-6);
-  bad += check_threepass<double, Shape<4, 8, 8, 16, 0>, TwoPassG<double, Shape<4, 4, 4, 16, 0>, Shape<4, 8, 8, 16, 2>, 4, 4>, true>("f64 2^14", 5e-15);
-  bad += check_threepass<double, Shape<8, 8, 8, 16, 0>, TwoPassG<double, Shape<4, 4, 4, 16, 0>, Shape<4, 8, 8, 16, 2>, 4, 4>, false>("f64 2^15", 5e-15);
-  bad += check_threepass<double, Shape<16, 16, 16, 8, 4>, TwoPassG<double, Shape<4, 4, 4, 16, 0>, Shape<4, 8, 8, 16, 2>, 4, 4>, true>("f64 2^17", 5e-15);
-  bad += check_rows_exchange<float, TwoPassG<float, Shape<4, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>, 1>("f32 2^11", 4, 2e-6);
-  bad += check_rows_exchange<float, TwoPassG<float, Shape<8, 16, 16, 16, 0>, Shape<8, 16, 16, 16, 2>, 4, 4>, 1>("f32 2^14", 8, 2e-6);
-  bad += check_rows_exchange<float, TwoPassG<float, Shape<8, 16, 16, 16, 0>, Shape<8, 16, 16, 16, 2>, 4, 4>, 2>("f32 2^14", 2, 2e-6);
-  bad += check_rows_exchange<float, TwoPassG<float, Shape<8, 16, 16, 16, 0>, Shape<16, 16, 16, 16, 1>, 4, 2>, 0>("f32 2^15", 8, 2e-6);
-  bad += check_rows_exchange<float, TwoPass<float, 16, 16, 16, 16, 0, 2, 2>, 1>("f32 2^16", 1, 2e-6);
-  bad += check_rows_exchange<double, TwoPassG<double, Shape<4, 4, 4, 16, 0>, Shape<4, 8, 8, 16, 2>, 4, 4>, 1>("f64 2^9", 4, 5e-15);
-  bad += check_rows_exchange<double, TwoPass<double, 8, 8, 16, 16, 0, 4, 4>, 2>("f64 2^12", 16, 5e-15);
-  // tiles of twice as many transforms (256-byte store runs), as dist_fft.cu's WideShape selects them
-  bad += check_rows_exchange<float, TwoPassG<float, Shape<8, 16, 16, 16, 0>, Shape<8, 16, 16, 16, 2>, 4, 4>, 1, Shape<8, 16, 16, 32, 2>>("f32 2^14 wide", 8, 2e-6);
-  bad += check_rows_exchange<float, TwoPass<float, 16, 16, 16, 16, 0, 2, 2>, 2, Shape<16, 16, 16, 32, 1>>("f32 2^16 wide", 4, 2e-6);
-  bad += check_rows_exchange<double, TwoPassG<double, Shape<8, 8, 8, 16, 0>, Shape<8, 16, 16, 8, 1>, 4, 2>, 1, Shape<8, 16, 16, 16, 1>>("f64 2^13 wide", 2, 5e-15);
-  bad += check_rows_exchange<double, TwoPass<double, 16, 16, 8, 8, 4, 2, 2>, 0, Shape<16, 16, 16, 16, 1>>("f64 2^16 wide", 8, 5e-15);
+  bad += threepass_radix3<float, 3, true>(11, 2e-6);
+  bad += threepass_radix3<float, 9, false>(11, 2e-6);
+  bad += threepass_radix3<float, 27, true>(11, 2e-6);
+  bad += threepass_radix3<double, 27, false>(9, 1e-14);
+  bad += threepass_radix3<double, 3, true>(9, 1e-14);
+  bad += threepass<float>(11, 2e-6);
+  bad += threepass<double>(9, 5e-15);
+  bad += rows_exchange<float, 1>(11, 4, 2e-6);
+  bad += rows_exchange<float, 1>(14, 8, 2e-6);
+  bad += rows_exchange<float, 2>(14, 2, 2e-6);
+  bad += rows_exchange<float, 0>(15, 8, 2e-6);
+  bad += rows_exchange<float, 1>(16, 1, 2e-6);
+  bad += rows_exchange<double, 1>(9, 4, 5e-15);
+  bad += rows_exchange<double, 2>(12, 16, 5e-15);
+  // tiles of twice as many transforms (256-byte store runs)
+  bad += rows_exchange<float, 1, true>(14, 8, 2e-6);
+  bad += rows_exchange<float, 2, true>(16, 4, 2e-6);
+  bad += rows_exchange<double, 1, true>(13, 2, 5e-15);
+  bad += rows_exchange<double, 0, true>(16, 8, 5e-15);
   bad += check_cta<float>("cta f32", 243, false, 2e-6);
   bad += check_cta<float>("cta f32", 729, false, 2e-6);
   bad += check_cta<float>("cta f32", 2187, false, 3e-6);
@@ -711,69 +812,16 @@ int main() {
   bad += check_cta<float>("cta f32", 3125, true, 4e-6);
   bad += check_cta<double>("cta f64", 1009, true, 1e-13);
   bad += check_cta<double>("cta f64", 5, true, 1e-13);
-  bad += check<float, TwoPass<float, 32, 32, 8, 8, 8, 2, 2>>("f32 2^20 (C=8)", 2e-6);
-  bad += check<float, TwoPass<float, 32, 32, 16, 16, 0, 1, 1>>("f32 2^20 (C=16)", 2e-6);
-  bad += check<float, TwoPass<float, 16, 16, 16, 16, 0, 2, 2>>("f32 2^16", 2e-6);
-  bad += check<float, TwoPass<float, 16, 32, 16, 8, 0, 2, 2>>("f32 2^18", 2e-6);
-  bad += check<float, TwoPassG<float, Shape<4, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>>("f32 2^11", 2e-6);
-  bad += check<double, TwoPassG<double, Shape<4, 4, 4, 16, 0>, Shape<4, 8, 8, 16, 2>, 4, 4>>("f64 2^9", 5e-15);
-  bad += check<double, TwoPassG<double, Shape<4, 8, 8, 16, 0>, Shape<4, 8, 8, 16, 2>, 4, 4>>("f64 2^10", 5e-15);
-  bad += check<double, TwoPassG<double, Shape<4, 8, 8, 16, 0>, Shape<8, 8, 8, 16, 1>, 4, 4>>("f64 2^11", 5e-15);
-  bad += check<float, TwoPassG<float, Shape<8, 8, 8, 32, 0>, Shape<8, 8, 8, 32, 2>, 4, 4>>("f32 2^12", 2e-6);
-  bad += check<float, TwoPassG<float, Shape<8, 8, 8, 32, 0>, Shape<8, 16, 16, 16, 2>, 4, 4>>("f32 2^13", 2e-6);
-  bad += check<float, TwoPassG<float, Shape<8, 16, 16, 16, 0>, Shape<8, 16, 16, 16, 2>, 4, 4>>("f32 2^14", 2e-6);
-  bad += check<float, TwoPassG<float, Shape<8, 16, 16, 16, 0>, Shape<16, 16, 16, 16, 1>, 4, 2>>("f32 2^15", 2e-6);
-  bad += check<float, TwoPassG<float, Shape<16, 16, 16, 16, 0>, Shape<16, 32, 32, 8, 1>, 2, 2>>("f32 2^17", 2e-6);
-  bad += check<float, TwoPassG<float, Shape<16, 32, 32, 8, 8>, Shape<32, 32, 32, 8, 1>, 2, 2>>("f32 2^19", 2e-6);
-  bad += check<double, TwoPassG<double, Shape<8, 8, 8, 16, 0>, Shape<8, 16, 16, 8, 1>, 4, 2>>("f64 2^13", 5e-15);
-  bad += check<double, TwoPassG<double, Shape<8, 16, 16, 8, 4>, Shape<16, 16, 16, 8, 1>, 2, 2>>("f64 2^15", 5e-15);
-  bad += check<double, TwoPass<double, 16, 16, 8, 8, 4, 2, 2>>("f64 2^16", 5e-15);
-  bad += check<double, TwoPass<double, 8, 8, 16, 16, 0, 4, 4>>("f64 2^12", 5e-15);
-  bad += check<double, TwoPass<double, 8, 16, 16, 8, 0, 4, 2>>("f64 2^14", 5e-15);
-  bad += check_onchip<float, 8, 8, 8, 8>("onchip f32", 2e-6);
-  bad += check_onchip<float, 8, 16, 16, 8>("onchip f32", 2e-6);
-  bad += check_onchip<float, 16, 16, 16, 8>("onchip f32", 2e-6);
-  bad += check_onchip<float, 16, 32, 32, 8>("onchip f32", 2e-6);
-  bad += check_onchip<float, 32, 32, 32, 8>("onchip f32", 2e-6);
-  bad += check_onchip<double, 8, 8, 8, 8>("onchip f64", 5e-15);
-  bad += check_onchip<double, 8, 16, 16, 8>("onchip f64", 5e-15);
-  bad += check_onchip<double, 16, 16, 16, 8>("onchip f64", 5e-15);
-  bad += check_bluestein<float, 32, 11>("bluestein f32", 1009, 3e-6);
-  bad += check_bluestein<float, 32, 11>("bluestein f32", 513, 3e-6);
-  bad += check_bluestein<float, 16, 8>("bluestein f32", 255, 3e-6);
-  bad += check_bluestein<float, 8, 8>("bluestein f32", 37, 3e-6);
-  bad += check_bluestein<double, 16, 8>("bluestein f64", 191, 1e-13);
-  bad += check_bluestein<double, 8, 8>("bluestein f64", 61, 1e-13);
-  bad += check_fused<fused::FusedCfg<float, 32, 8, 2, 8, 1>>("fused f32 2^20", 2e-6);
-  bad += check_fused<fused::FusedCfg<double, 16, 8, 3, 4, 3>>("fused f64 2^16", 5e-15);
-  bad += check_fused<fused::FusedCfg<float, 32, 8, 2, 8, 2, true>>("fused f32 2^20", 2e-6);
-  bad += check_fused<fused::FusedCfg<double, 16, 8, 4, 4, 4, true>>("fused f64 2^16", 5e-15);
-  bad += check_fused<fused::FusedCfg<double, 8, 8, 8, 4, 8, true>>("fused f64 2^12", 5e-15);
-  // <T, RA, C, G, PAD1, EXB, DIRECT, RB, RA2, RB2, E1, E2, C1>
-  bad += check_fused<fused::FusedCfg<float, 32, 8, 2, 0, 1, false, 16, 32, 32, 32, 32, 16, true>>("fused f32 2^19", 2e-6);
-  bad += check_fused<fused::FusedCfg<float, 16, 8, 6, 8, 6, false, 8, 16, 16, 16, 32>>("fused f32 2^15", 2e-6);
-  bad += check_fused<fused::FusedCfg<float, 8, 8, 8, 8, 8, false, 8, 16, 8, 8, 16>>("fused f32 2^13", 2e-6);
-  bad += check_fused<fused::FusedCfg<float, 16, 8, 3, 8, 3, false, 16, 32, 16, 16, 32>>("fused f32 2^17", 2e-6);
-  bad += check_fused<fused::FusedCfg<double, 8, 8, 8, 4, 8, true, 8, 16, 8, 8, 16>>("fused f64 2^13", 5e-15);
-  bad += check_fused<fused::FusedCfg<float, 32, 8, 3, 8, 3, false, 16>>("fused f32 2^18", 2e-6);
-  bad += check_fused<fused::FusedCfg<float, 16, 8, 8, 8, 8, false, 8>>("fused f32 2^14", 2e-6);
-  bad += check_fused<fused::FusedCfg<double, 16, 8, 4, 4, 4, false, 8>>("fused f64 2^14", 5e-15);
-  bad += check_fused<fused::FusedCfg<float, 16, 8, 4, FB_PAD16, 4, true>>("fused f32 2^16", 2e-6);
-  bad += check_fused<fused::FusedCfg<float, 16, 8, 4, FB_PAD16, 4>>("fused f32 2^16", 2e-6);
-  bad += check_queue<fused::FusedConfig<float, 13>>("f32 2^13");
-  bad += check_queue<fused::FusedConfig<float, 14>>("f32 2^14");
-  bad += check_queue<fused::FusedConfig<float, 15>>("f32 2^15");
-  bad += check_queue<fused::FusedConfig<float, 16>>("f32 2^16");
-  bad += check_queue<fused::FusedConfig<float, 17>>("f32 2^17");
-  bad += check_queue<fused::FusedConfig<float, 18>>("f32 2^18");
-  bad += check_queue<fused::FusedConfig<float, 19>>("f32 2^19");
-  bad += check_queue<fused::FusedConfig<float, 20>>("f32 2^20");
-  struct Single20 : fused::FusedConfig<float, 20> { using Cfg = fused::FusedConfig<float, 20>::Cfg::Unpaired; };
-  bad += check_queue<Single20>("f32 2^20 (FOURIER_B200_PAIR=0)");
-  bad += check_queue<fused::FusedConfig<double, 12>>("f64 2^12");
-  bad += check_queue<fused::FusedConfig<double, 13>>("f64 2^13");
-  bad += check_queue<fused::FusedConfig<double, 14>>("f64 2^14");
-  bad += check_queue<fused::FusedConfig<double, 16>>("f64 2^16");
+  bad += check_twopass<float>(2e-6);
+  bad += check_twopass<double>(5e-15);
+  for_each_onchip<float>([&](auto k) { bad += check_onchip<decltype(k)>("onchip f32", 2e-6); });
+  for_each_onchip<double>([&](auto k) { bad += check_onchip<decltype(k)>("onchip f64", 5e-15); });
+  for (long n : {1009L, 513L, 255L, 37L}) bad += bluestein<float>(n, 3e-6);
+  for (long n : {191L, 61L}) bad += bluestein<double>(n, 1e-13);
+  fused::for_each_fused_size<float>([&](auto k) { bad += check_persistent<float, decltype(k)::value>(2e-6); });
+  fused::for_each_fused_size<double>([&](auto k) { bad += check_persistent<double, decltype(k)::value>(5e-15); });
+  fused::for_each_fused_size<float>([&](auto k) { bad += check_queues<float, decltype(k)::value>(); });
+  fused::for_each_fused_size<double>([&](auto k) { bad += check_queues<double, decltype(k)::value>(); });
   printf(bad ? "EMULATION FAILED (%d)\n" : "EMULATION OK\n", bad);
   return bad ? 1 : 0;
 }

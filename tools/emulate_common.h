@@ -1,6 +1,7 @@
 // emulate_common.h -- the harness the CPU emulators (tools/emulate*.cu) share: they run the kernels' __host__ __device__
 // bodies thread by thread and phase by phase on the CPU and check them against references in double.
 //   * run_body: the CPU driver of tilefft.cuh's phase protocol, so an emulator runs exactly the phases of the kernel;
+//   * for_each_onchip: the on-chip size classes the library selects from;
 //   * the input generator, 16-byte-aligned buffers and the bank-conflict model of shared-memory accesses;
 //   * the spectrum access hook (FB_SPEC_ACCESS, defined before the kernel headers) and check_access;
 //   * the w_N^k pair table and the direct transforms of packed reals of the real-input emulators.
@@ -21,7 +22,7 @@ static void spec_record(const void* p, int bytes);
 #define FB_SPEC_ACCESS(p, bytes) spec_record((const void*)(p), (int)(bytes))
 #endif
 
-#include "onchip_kernels.cuh"
+#include "onchip_configs.cuh"
 #include "plan.h"
 #include "tables.cuh"
 
@@ -39,6 +40,11 @@ static void run_body(const typename Body::Args& a, long groups, const TwPair<typ
     static_for<0, Body::kPhases>([&](auto P) {
       for (int t = 0; t < Tile::THREADS; ++t) Body::template phase<decltype(P)::value>(thr[t], a, g, t, smem.data(), twa);
     });
+}
+
+// every on-chip size class of precision T (onchip_configs.cuh), smallest first: f(class)
+template <typename T, class F> static void for_each_onchip(F&& f) {
+  for (size_t l = 1; l <= ((size_t)1 << 16); l *= 2) onchip::visit_onchip<T>(l, f);
 }
 
 // ---- inputs -------------------------------------------------------------------------------------------------------

@@ -53,10 +53,12 @@ static double conv_err(const std::vector<double>& x, const std::vector<double>& 
 }
 
 // ---- fused on-chip conv kernel --------------------------------------------------------------------------------------
-template <typename T, int RA, int RB, int E, int WARPS>
+template <class K>
 static int check_fused(const char* name, double tol) {
+  using T = typename K::T;
+  constexpr int RA = K::RA, RB = K::RB, E = K::E;
   using V = cpx<T>;
-  using Cfg = onchip::OnChipCfg<T, RA, RB, E, WARPS, true>;
+  using Cfg = typename K::template Cfg<true>;
   using Body = onchip::ConvBody<Cfg>;
   using Tile = typename Cfg::Tile;
   constexpr long L = RA * RB, N = 2 * L, rows = 3;
@@ -138,15 +140,9 @@ static int check_pair(const char* name, long m, double tol) {
 
 int main() {
   int bad = 0;
-  // the on-chip size classes of onchip_lookup (onchip.cu): L = M = N/2
-  bad += check_fused<float, 8, 8, 8, 8>("fused f32", 2e-6);
-  bad += check_fused<float, 8, 16, 16, 8>("fused f32", 2e-6);
-  bad += check_fused<float, 16, 16, 16, 8>("fused f32", 2e-6);
-  bad += check_fused<float, 16, 32, 32, 8>("fused f32", 2e-6);
-  bad += check_fused<float, 32, 32, 32, 8>("fused f32", 2e-6);
-  bad += check_fused<double, 8, 8, 8, 8>("fused f64", 1e-13);
-  bad += check_fused<double, 8, 16, 16, 8>("fused f64", 1e-13);
-  bad += check_fused<double, 16, 16, 16, 8>("fused f64", 1e-13);
+  // every on-chip size class (onchip_configs.cuh): L = M = N/2
+  for_each_onchip<float>([&](auto k) { bad += check_fused<decltype(k)>("fused f32", 2e-6); });
+  for_each_onchip<double>([&](auto k) { bad += check_fused<decltype(k)>("fused f64", 1e-13); });
   for (long m : {1L, 2L, 3L, 512L, 1000L, 1009L}) {
     bad += check_pair<float>("pair f32", m, 2e-6);
     bad += check_pair<double>("pair f64", m, 1e-13);

@@ -125,10 +125,12 @@ static int report(const char* what, double worst, double tol, long reads, long w
 }
 
 // ---- fused on-chip linear convolution kernel -----------------------------------------------------------------------
-template <typename T, int RA, int RB, int E, int WARPS>
+template <class K>
 static int check_fused(const char* name, double tol) {
+  using T = typename K::T;
+  constexpr int RA = K::RA, RB = K::RB, E = K::E;
   using V = cpx<T>;
-  using Cfg = onchip::OnChipCfg<T, RA, RB, E, WARPS, true>;
+  using Cfg = typename K::template Cfg<true>;
   using Body = onchip::LinConvBody<Cfg>;
   using Tile = typename Cfg::Tile;
   constexpr long L = RA * RB, N = 2 * L, rows = 3;
@@ -290,15 +292,9 @@ static int check_maps(long n) {
 
 int main() {
   int bad = 0;
-  // the on-chip size classes of onchip_lookup (onchip.cu): L = N/2
-  bad += check_fused<float, 8, 8, 8, 8>("fused f32", 1e-5);
-  bad += check_fused<float, 8, 16, 16, 8>("fused f32", 1e-5);
-  bad += check_fused<float, 16, 16, 16, 8>("fused f32", 1e-5);
-  bad += check_fused<float, 16, 32, 32, 8>("fused f32", 1e-5);
-  bad += check_fused<float, 32, 32, 32, 8>("fused f32", 1e-5);
-  bad += check_fused<double, 8, 8, 8, 8>("fused f64", 1e-12);
-  bad += check_fused<double, 8, 16, 16, 8>("fused f64", 1e-12);
-  bad += check_fused<double, 16, 16, 16, 8>("fused f64", 1e-12);
+  // every on-chip size class (onchip_configs.cuh): L = N/2
+  for_each_onchip<float>([&](auto k) { bad += check_fused<decltype(k)>("fused f32", 1e-5); });
+  for_each_onchip<double>([&](auto k) { bad += check_fused<decltype(k)>("fused f64", 1e-12); });
   for (long n : {96L, 97L}) bad += check_maps(n);
   printf(bad ? "EMULATION FAILED (%d)\n" : "EMULATION OK\n", bad);
   return bad ? 1 : 0;

@@ -47,8 +47,10 @@ static double rel(const std::vector<double>& got, const std::vector<double>& ref
 }
 
 // ---- fused on-chip real kernel ------------------------------------------------------------------------------------
-template <typename T, int RA, int RB, int E, int WARPS>
+template <class K>
 static int check_fused(const char* name, double tol) {
+  using T = typename K::T;
+  constexpr int RA = K::RA, RB = K::RB, E = K::E;
   using V = cpx<T>;
   constexpr long L = RA * RB, N = 2 * L, batch = 5;   // 5: not a multiple of the transforms per CTA
   const double s = 0.5;
@@ -57,7 +59,7 @@ static int check_fused(const char* name, double tol) {
   const auto tab = pair_table<T>(L);
   unsigned long long seed = 977 + L;
   {  // forward
-    using Cfg = onchip::OnChipCfg<T, RA, RB, E, WARPS, true>;
+    using Cfg = typename K::template Cfg<true>;
     using Body = onchip::RealBody<Cfg>;
     Buf<T> x(N * batch);
     for (long i = 0; i < N * batch; ++i) x[i] = (T)rnd(seed);
@@ -111,7 +113,7 @@ static int check_fused(const char* name, double tol) {
     printf("  park     threads %4d  exchange conflicts: write x%d, read x%d\n", Cfg::THREADS, worst_w, worst_r);
   }
   {  // inverse (Ifft: s = 1/N), random imaginary parts in bins 0 and N/2
-    using Cfg = onchip::OnChipCfg<T, RA, RB, E, WARPS, false>;
+    using Cfg = typename K::template Cfg<false>;
     using Body = onchip::RealBody<Cfg>;
     Buf<V> x((L + 1) * batch);
     for (long i = 0; i < (L + 1) * batch; ++i) x[i] = mk<T>((T)rnd(seed), (T)rnd(seed));
@@ -192,15 +194,9 @@ static int check_steps(const char* name, long m, double tol) {
 
 int main() {
   int bad = 0;
-  // the on-chip size classes of onchip_lookup (onchip.cu): L = M = N/2
-  bad += check_fused<float, 8, 8, 8, 8>("fused f32", 2e-6);
-  bad += check_fused<float, 8, 16, 16, 8>("fused f32", 2e-6);
-  bad += check_fused<float, 16, 16, 16, 8>("fused f32", 2e-6);
-  bad += check_fused<float, 16, 32, 32, 8>("fused f32", 2e-6);
-  bad += check_fused<float, 32, 32, 32, 8>("fused f32", 2e-6);
-  bad += check_fused<double, 8, 8, 8, 8>("fused f64", 5e-15);
-  bad += check_fused<double, 8, 16, 16, 8>("fused f64", 5e-15);
-  bad += check_fused<double, 16, 16, 16, 8>("fused f64", 5e-15);
+  // every on-chip size class (onchip_configs.cuh): L = M = N/2
+  for_each_onchip<float>([&](auto k) { bad += check_fused<decltype(k)>("fused f32", 2e-6); });
+  for_each_onchip<double>([&](auto k) { bad += check_fused<decltype(k)>("fused f64", 5e-15); });
   for (long m : {1L, 2L, 3L, 512L, 1000L, 1009L}) {
     bad += check_steps<float>("steps f32", m, 2e-6);
     bad += check_steps<double>("steps f64", m, 2e-14);   // the reference is a direct DFT in double: ~sqrt(N) eps
