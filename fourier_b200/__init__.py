@@ -21,6 +21,9 @@ reference's operator interface name for name:
     (no counterpart)                                      RealFft.stft / istft / stft_frames: short-time Fourier
                                                             transform of real rows and its overlap-add inverse
                                                             (torch.stft / istft, frames frame-major)
+    (no counterpart)                                      RealFft.mel_spectrogram: |stft|^p through a caller's
+                                                            mel filter bank (torchaudio's MelSpectrogram,
+                                                            frames frame-major), the spectrum kept on chip
 
 Buffers are numpy arrays (host memory: staged over PCIe by the library) or torch CUDA tensors
 (device memory: transformed in HBM on torch's current stream).  A leading batch dimension is
@@ -434,6 +437,62 @@ class RealFft:
             rc = getattr(L, f"fourier_b200_stft_{self._t}")(self._plan, pi, in_len, pw, hop, boundary, po, batch)
         if rc != 0:
             raise RuntimeError(f"stft failed (cuda error {rc}): {_lib.last_error()}")
+
+    def mel_spectrogram(self, input, window, hop, filters, output, power=2, center=True, pad_mode="reflect"):
+        """Mel spectrogram of every row of `input` (shape (..., L)) with stft's framing: output[..., f, m] =
+        sum_k filters[m, k] * |X_f[k]|**power, X_f the stft of frame f (same window, hop, center and pad_mode), power 1
+        or 2, no log.  `filters` has shape (n_mels, N//2+1) (librosa's and Whisper's layout; pass torchaudio's
+        melscale_fbanks(...).T.contiguous()), any n_mels >= 1 and any real weights.  `output` has shape
+        (..., F, n_mels), F = stft_frames(L, hop, center): with power 2 and torchaudio's own window and bank this is
+        torchaudio.transforms.MelSpectrogram(...)(x).transpose(-1, -2).  The spectrum stays on chip where the plan's
+        path allows.  Out of place only."""
+        self._stft_buffers((input, window, filters, output))
+        if center and pad_mode not in self.STFT_PAD_MODES:
+            raise ValueError(f"pad_mode must be one of {sorted(self.STFT_PAD_MODES)}, got {pad_mode!r}")
+        hop = int(hop)
+        if hop < 1:
+            raise ValueError(f"hop must be at least 1, got {hop}")
+        if power not in (1, 2):
+            raise ValueError(f"power must be 1 or 2, got {power!r}")
+        boundary = self.STFT_PAD_MODES[pad_mode] if center else 0
+        n = self._size
+        in_len = input.shape[-1] if getattr(input, "ndim", 0) > 0 else 0
+        if in_len < 1:
+            raise ValueError("input rows must hold at least one sample")
+        if boundary == 0 and in_len < n:
+            raise ValueError(f"center=False needs rows of at least N = {n} samples, got {in_len}")
+        if boundary == 2 and in_len <= n // 2:
+            raise ValueError(f"pad_mode 'reflect' needs rows of more than N//2 = {n // 2} samples, got {in_len}")
+        frames = self.stft_frames(in_len, hop, center)
+        pi, li, di, si = self._describe(input, "real", last=in_len)
+        pw, lw, dw, _ = self._describe(window, "real")
+        if lw != ():
+            raise ValueError(f"window must hold exactly N = {n} reals, got shape {tuple(window.shape)}")
+        if getattr(filters, "ndim", 0) != 2:
+            raise ValueError(f"filters must have shape (n_mels, {n // 2 + 1})")
+        pf, lf, df, _ = self._describe(filters, "real", last=n // 2 + 1)
+        n_mels = lf[0]
+        if n_mels < 1:
+            raise ValueError("filters must hold at least one mel row")
+        if getattr(output, "ndim", 0) < 2 or output.shape[-2] != frames:
+            raise ValueError(f"output must have shape (..., {frames}, {n_mels}) (F = {frames} frames)")
+        po, lo, do_, _ = self._describe(output, "real", last=n_mels)
+        if li != lo[:-1]:
+            raise ValueError(f"input and output leading shapes differ: {li} and {lo[:-1]}")
+        if not (di == dw == df == do_):
+            raise ValueError("input, window, filters and output must all be host or all be device buffers")
+        batch = int(np.prod(li, dtype=np.int64))
+        if batch == 0:
+            return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
+        L = _lib.load()
+        if di:
+            rc = getattr(L, f"fourier_b200_mel_spectrogram_async_{self._t}")(
+                self._plan, pi, in_len, pw, hop, boundary, int(power), pf, n_mels, po, batch, si)
+        else:
+            rc = getattr(L, f"fourier_b200_mel_spectrogram_{self._t}")(
+                self._plan, pi, in_len, pw, hop, boundary, int(power), pf, n_mels, po, batch)
+        if rc != 0:
+            raise RuntimeError(f"mel spectrogram failed (cuda error {rc}): {_lib.last_error()}")
 
     def istft(self, input, window, hop, output, center=True):
         """Inverse of stft: `input` (shape (..., F, N//2+1), stft's frame-major layout) -> `output` (shape

@@ -305,6 +305,59 @@ int stft_exec(void* plan, const T* in, size_t in_len, const T* window, size_t ho
   }
 }
 
+// Mel spectrogram of real rows: stft_exec's rules, plus power and n_mels checked before the plan is touched and the
+// filters kept apart from the output.
+template <typename T>
+int mel_exec(void* plan, const T* in, size_t in_len, const T* window, size_t hop, int boundary, int power,
+             const T* filters, size_t n_mels, T* out, size_t batch, bool async, void* stream) {
+  if (!plan || !in || !window || !filters || !out) {
+    fb200::set_last_error("null argument");
+    return (int)cudaErrorInvalidValue;
+  }
+  const char* bad = hop == 0                          ? "hop must be at least 1"
+                    : boundary < 0 || boundary > 2    ? "unknown boundary (FOURIER_B200_STFT_NONE, _ZEROS or _REFLECT)"
+                    : in_len == 0                     ? "in_len must be at least 1"
+                    : power != 1 && power != 2        ? "power must be 1 or 2"
+                    : n_mels == 0                     ? "n_mels must be at least 1"
+                                                      : nullptr;
+  if (bad) { fb200::set_last_error(bad); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  const size_t n = p->size();
+  if (boundary == fb200::real::kStftNone && in_len < n) {
+    fb200::set_last_error("boundary none needs in_len >= N");
+    return (int)cudaErrorInvalidValue;
+  }
+  if (boundary == fb200::real::kStftReflect && in_len <= n / 2) {
+    fb200::set_last_error("boundary reflect needs in_len > N/2");
+    return (int)cudaErrorInvalidValue;
+  }
+  try {
+    if (batch == 0)
+      return (int)p->mel_device(in, in_len, window, hop, boundary, filters, n_mels, power, out, 0, nullptr);
+    const size_t frames = (size_t)fb200::real::frame_map((long)n, (long)in_len, (long)hop, boundary).frames;
+    const size_t in_bytes = batch * in_len * sizeof(T), out_bytes = batch * frames * n_mels * sizeof(T);
+    if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, n * sizeof(T), out, out_bytes) ||
+        ranges_meet(filters, n_mels * (n / 2 + 1) * sizeof(T), out, out_bytes)) {
+      fb200::set_last_error("input, window or filters and output overlap (the mel spectrogram is out of place only)");
+      return (int)cudaErrorInvalidValue;
+    }
+    if (!async) {
+      const int dev = residence({in, window, filters, out},
+                                "input, window, filters and output must all be host or all be device memory");
+      if (dev < 0) return (int)cudaErrorInvalidValue;
+      if (!dev) return (int)p->mel_host(in, in_len, window, hop, boundary, filters, n_mels, power, out, batch);
+    }
+    if (!device_pointers_aligned(in, out)) return (int)cudaErrorMisalignedAddress;
+    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
+    cudaError_t e = p->mel_device(in, in_len, window, hop, boundary, filters, n_mels, power, out, batch, s);
+    if (e != cudaSuccess || async) return (int)e;
+    return (int)cudaStreamSynchronize(s);
+  } catch (...) {
+    fb200::set_last_error("mel spectrogram threw");
+    return (int)cudaErrorUnknown;
+  }
+}
+
 template <typename T>
 int istft_exec(void* plan, const void* in, size_t frames, const T* window, size_t hop, int center, T* out,
                size_t out_len, size_t batch, bool async, void* stream) {
@@ -637,6 +690,31 @@ int fourier_b200_istft_async_double(fourier_b200_rfft_double* plan, const void* 
                                     const double* window_dev, size_t hop, int center, double* out_dev, size_t out_len,
                                     size_t batch, void* stream) {
   return istft_exec<double>(plan, in_dev, frames, window_dev, hop, center, out_dev, out_len, batch, true, stream);
+}
+
+int fourier_b200_mel_spectrogram_float(fourier_b200_rfft_float* plan, const float* in, size_t in_len,
+                                       const float* window, size_t hop, int boundary, int power, const float* filters,
+                                       size_t n_mels, float* out, size_t batch) {
+  return mel_exec<float>(plan, in, in_len, window, hop, boundary, power, filters, n_mels, out, batch, false, nullptr);
+}
+int fourier_b200_mel_spectrogram_double(fourier_b200_rfft_double* plan, const double* in, size_t in_len,
+                                        const double* window, size_t hop, int boundary, int power,
+                                        const double* filters, size_t n_mels, double* out, size_t batch) {
+  return mel_exec<double>(plan, in, in_len, window, hop, boundary, power, filters, n_mels, out, batch, false, nullptr);
+}
+int fourier_b200_mel_spectrogram_async_float(fourier_b200_rfft_float* plan, const float* in_dev, size_t in_len,
+                                             const float* window_dev, size_t hop, int boundary, int power,
+                                             const float* filters_dev, size_t n_mels, float* out_dev, size_t batch,
+                                             void* stream) {
+  return mel_exec<float>(plan, in_dev, in_len, window_dev, hop, boundary, power, filters_dev, n_mels, out_dev, batch,
+                         true, stream);
+}
+int fourier_b200_mel_spectrogram_async_double(fourier_b200_rfft_double* plan, const double* in_dev, size_t in_len,
+                                              const double* window_dev, size_t hop, int boundary, int power,
+                                              const double* filters_dev, size_t n_mels, double* out_dev, size_t batch,
+                                              void* stream) {
+  return mel_exec<double>(plan, in_dev, in_len, window_dev, hop, boundary, power, filters_dev, n_mels, out_dev, batch,
+                          true, stream);
 }
 
 const char* fourier_b200_last_error(void) { return fb200::last_error(); }

@@ -91,7 +91,24 @@ struct OnChipImpl {
     if ((e = allow_smem(onchip::onchip_real_kernel<Cfg<false>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_conv_kernel<Cfg<true>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_lconv_kernel<Cfg<true>, MINB>))) return e;
-    return allow_smem(onchip::onchip_stft_kernel<Cfg<true>, MINB>);
+    if ((e = allow_smem(onchip::onchip_stft_kernel<Cfg<true>, MINB>))) return e;
+    return allow_smem(onchip::onchip_mel_kernel<Cfg<true>, MINB>);
+  }
+  static cudaError_t mel(const T* in, const T* win, const T* filters, const real::Band* bands, size_t n_mels, int power,
+                         T* out, const real::FrameMap& m, size_t nframes, const void* twa, const cpx<T>* tab, int sms,
+                         cudaStream_t s) {
+    typename onchip::MelBody<Cfg<true>>::Args a;
+    static_cast<typename onchip::RealBody<Cfg<true>>::Args&>(a) = {
+        nullptr, nullptr, (const TwPair<T>*)twa, tab, (long)nframes, (T)0.5};
+    a.x = in;
+    a.win = win;
+    a.m = m;
+    a.mel = out;
+    a.filters = filters;
+    a.bands = bands;
+    a.n_mels = (long)n_mels;
+    a.power = power;
+    return launch(onchip::onchip_mel_kernel<Cfg<true>, MINB>, a, nframes, sms, s);
   }
   static cudaError_t stft(const T* in, const T* win, void* out, const real::FrameMap& m, size_t nframes,
                           const void* twa, const cpx<T>* tab, int sms, cudaStream_t s) {
@@ -129,7 +146,7 @@ struct OnChipImpl {
                   {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab, (long)batch, h}, batch, sms, s);
   }
   static const OnChipOps<T>* ops() {
-    static const RealOnChipOps<T> r = {RA, RB, &real_prepare, &real, &conv, &lconv, &stft};
+    static const RealOnChipOps<T> r = {RA, RB, &real_prepare, &real, &conv, &lconv, &stft, &mel};
     static const OnChipOps<T> o = {RA, RB, &prepare, &fft, kHasBluestein ? &bluestein : nullptr, &r};
     return &o;
   }

@@ -8,8 +8,9 @@
 //   * onchip_conv_kernel:     y = irfft(rfft(x) . H) of real rows of length 2L, both transforms in one kernel.
 //   * onchip_lconv_kernel:    linear convolution of real rows of any length by overlap-save on the same phases.
 //   * onchip_stft_kernel:     windowed frames of real rows of any length through the forward real-input phases.
-//     (these five run the phases of FftBody / RealBody / ConvBody / LinConvBody / StftBody through run_onchip_groups,
-//     tilefft.cuh)
+//   * onchip_mel_kernel:      the stft's frames to mel energies: power and filter bank on chip.
+//     (these six run the phases of FftBody / RealBody / ConvBody / LinConvBody / StftBody / MelBody through
+//     run_onchip_groups, tilefft.cuh)
 //   * bluestein_fused_kernel: the whole chirp-z transform of the reference (bluesteins.rs:218-259) for
 //                             N <= L, M = 2L, in one kernel and without touching HBM in between.
 //
@@ -395,6 +396,76 @@ template <class Cfg> struct StftBody {
 template <class Cfg, int MINB>
 __global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_stft_kernel(const typename StftBody<Cfg>::Args a) {
   run_onchip_groups<Cfg, StftBody<Cfg>>(a);
+}
+
+// ---- fused mel spectrogram of real rows, N = 2L (real::band_scan / mel_dot, DESIGN.md §4.14) ---------------------
+// StftBody's phases 0-4 as they are (the windowed frame through stage A, the scatter, RealBody's gather + stage B and
+// park), then:
+//   * powers (phase 5): each lane untangles the pairs it owns, k = u + TP*j (lane u = 0 also k = L/2), and keeps
+//     |X[k]|^p and |X[L-k]|^p in its own tile registers;
+//   * park powers (phase 6): the L+1 powers go into the FFT's park as reals (it holds 2L; no lane reads Z any more);
+//   * mels (phase 7): lane u of the FFT sums mels m = u, u + TP, ... over their bands of the parked powers and stores
+//     them to row q of `mel`, consecutive lanes writing consecutive mels.
+// Only the mel energies reach HBM: n_mels reals per frame instead of N/2+1 complex bins.
+template <class Cfg> struct MelBody {
+  using Stft = StftBody<Cfg>;
+  using Real = RealBody<Cfg>;
+  using Tile = typename Cfg::Tile;   // FWD = true
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  static constexpr int L = Cfg::L, TP = Tile::TP, E = Tile::E;
+  // Stft::Args with out = nullptr; frame q of the launch writes mel[q * n_mels ..]
+  struct Args : Stft::Args { T* mel; const T* filters; const real::Band* bands; long n_mels; int power; };
+
+  static FB_HD void powers(Tile& f, const Args& a, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const V* z = smem + Real::park(t);
+#pragma unroll
+    for (int j = 0; j < E / 2; ++j) f.v[j] = real::power_pair(z, L, u + TP * j, a.tab, a.h, a.power);
+    if (u == 0) f.v[E / 2] = real::power_pair(z, L, L / 2, a.tab, a.h, a.power);
+  }
+  static FB_HD void park_powers(const Tile& f, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    T* pw = reinterpret_cast<T*>(smem + Real::park(t));
+#pragma unroll
+    for (int j = 0; j < E / 2; ++j) {
+      pw[u + TP * j] = f.v[j].x;
+      pw[L - (u + TP * j)] = f.v[j].y;
+    }
+    if (u == 0) pw[L / 2] = f.v[E / 2].x;
+  }
+  static FB_HD void mels(const Args& a, long grp, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const long q = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (q >= a.batch) return;
+    const T* pw = reinterpret_cast<const T*>(smem + Real::park(t));
+    T* y = a.mel + q * a.n_mels;
+    const long g = a.m.g0 + q;
+    // The empty asm makes these three pointers opaque here, so the lane's first weight, band and power addresses are
+    // formed in this phase: hoisted out of the group loop they stayed live through stage A, and ptxas spilled 24 bytes
+    // at the f32 L = 128 register cap.
+    const T* filters = a.filters;
+    const real::Band* bands = a.bands;
+#ifdef __CUDA_ARCH__
+    asm volatile("" : "+l"(filters), "+l"(bands), "+l"(pw));
+#endif
+    for (long m = u; m < a.n_mels; m += TP)
+      real::lin_st(y + m, real::mel_dot(filters, bands, (long)(L + 1), m, [&](long k) { return pw[k]; }), g);
+  }
+
+  // phase protocol (tilefft.cuh): StftBody's load, stage A, scatter, gather + stage B and park; powers, park powers, mels
+  static constexpr int kPhases = 8;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    if constexpr (P <= 4) Stft::template phase<P>(f, a, grp, t, smem, twa);
+    else if constexpr (P == 5) powers(f, a, t, smem);
+    else if constexpr (P == 6) park_powers(f, t, smem);
+    else mels(a, grp, t, smem);
+  }
+};
+
+template <class Cfg, int MINB>
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_mel_kernel(const typename MelBody<Cfg>::Args a) {
+  run_onchip_groups<Cfg, MelBody<Cfg>>(a);
 }
 
 // ---- fused Bluestein -------------------------------------------------------------------------------------------

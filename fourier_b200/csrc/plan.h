@@ -310,6 +310,10 @@ template <typename T> struct RealOnChipOps {
                        const cpx<T>* spec, size_t rows, T h, int sms, cudaStream_t);
   cudaError_t (*stft)(const T* in, const T* win, void* out, const real::FrameMap& m, size_t nframes, const void* twa,
                       const cpx<T>* tab, int sms, cudaStream_t);
+  // mel(): the mel energies of the same frames (DESIGN.md §4.14), n_mels reals per frame from `out` on
+  cudaError_t (*mel)(const T* in, const T* win, const T* filters, const real::Band* bands, size_t n_mels, int power,
+                     T* out, const real::FrameMap& m, size_t nframes, const void* twa, const cpx<T>* tab, int sms,
+                     cudaStream_t);
 };
 template <typename T> const RealOnChipOps<T>* real_onchip_lookup(size_t l);
 
@@ -374,6 +378,15 @@ class RealPlan {
   cudaError_t istft_host(const C* in, size_t frames, const T* win, size_t hop, bool center, T* out, size_t out_len,
                          size_t batch);
 
+  // Mel spectrogram (DESIGN.md §4.14): the frames of stft_device -> n_mels reals each, frame-major,
+  // out[b][f][m] = sum_k filters[m][k] |X_{b,f}[k]|^power, filters a row-major (n_mels, N/2+1) matrix, power 1 or 2,
+  // n_mels >= 1; checked by the caller with the stft's arguments.  Out of place only.  Device pointers, on `stream`.
+  cudaError_t mel_device(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
+                         size_t n_mels, int power, T* out, size_t batch, cudaStream_t stream);
+  // Host pointers: the window and the filters are staged once, whole rows through stage_rows; the same bits.
+  cudaError_t mel_host(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
+                       size_t n_mels, int power, T* out, size_t batch);
+
   unsigned long long launches() const { return launches_; }
   const char* kernel_name() const { return kernel_desc_.c_str(); }
 
@@ -397,6 +410,12 @@ class RealPlan {
   // scatter through seg_; adds its kernels to launches_
   cudaError_t linear_segments(const T* in, T* out, const real::SegMap& m, size_t nseg, const C* spec, size_t rows,
                               cudaStream_t s);
+  // the band of every filter row into bands_ (one launch, added to launches_)
+  cudaError_t mel_bands(const T* filters, size_t n_mels, cudaStream_t s);
+  // mel_device after mel_bands: the fused kernel, or chunks of gathered frames and their spectra through seg_; sets
+  // launches_
+  cudaError_t mel_frames(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
+                         size_t n_mels, int power, T* out, size_t batch, cudaStream_t s);
   // The host-pointer loop of exec_host and convolve_host (real.cu): chunks of rows of in_row / out_row bytes go H2D,
   // through step(dev_in, dev_out, first_row, rows) on host_stream_, and D2H; launches() then counts all chunks.
   template <class Step>
@@ -413,9 +432,11 @@ class RealPlan {
   DeviceBuffer work_;                // one chunk of inner-plan rows
   DeviceBuffer stage_in_, stage_out_;
   DeviceBuffer stage_spec_;          // the spectra of convolve_host and linear_convolve_host, the window of stft_host
-                                     // and istft_host
+                                     // and istft_host, the window and filters of mel_host
   DeviceBuffer seg_;                 // one chunk of N-real segments of a linear convolution (real_half, real_full), of
-                                     // windowed frames (stft) or of inverted frames (istft)
+                                     // windowed frames (stft) or of inverted frames (istft); of windowed frames and
+                                     // their spectra (mel, real_half and real_full)
+  DeviceBuffer bands_;               // the filter bands of the last mel call (real::Band per filter row)
   cudaStream_t host_stream_ = nullptr;
   std::string kernel_desc_;
 };

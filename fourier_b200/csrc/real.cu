@@ -13,6 +13,9 @@
 // Short-time Fourier transform (DESIGN.md §4.13): onchip_stft_kernel on the fused path; otherwise chunks of windowed
 // frames gathered into seg_ and transformed from there by the plan's own rfft.  The inverse inverts runs of frames into
 // seg_ with the plan's own irfft and overlap-adds them on every path.
+// Mel spectrogram (DESIGN.md §4.14): mel_bands_kernel, then onchip_mel_kernel on the fused path; otherwise chunks of
+// windowed frames gathered into seg_, their spectra by the plan's own rfft into seg_ behind them, and
+// mel_spectra_kernel from there into the output rows.
 #include <algorithm>
 #include <string>
 #include <vector>
@@ -133,6 +136,35 @@ overlap_add_kernel(const T* __restrict__ seg, const T* __restrict__ win, T* __re
   for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
     const long r = g / cnt;
     real::overlap_add_one(m, seg, win, gs, out + r * out_ld, b0 + r, i0 + (g - r * cnt));
+  }
+}
+
+// Mel spectrogram (real::band_scan / mel_dot).  bands: one CTA per filter row, each thread scanning every kThreads-th
+// weight, merged in shared memory.  spectra: one thread per mel m of frame q of the chunk, consecutive threads on
+// consecutive mels of a frame, from the chunk's spectra into the output rows (frame g0 + q).
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+mel_bands_kernel(const T* __restrict__ filters, long bins, long n_mels, real::Band* __restrict__ bands) {
+  __shared__ real::Band part[kThreads];
+  for (long m = blockIdx.x; m < n_mels; m += gridDim.x) {
+    part[threadIdx.x] = real::band_scan(filters + m * bins, bins, (long)threadIdx.x, (long)kThreads);
+    __syncthreads();
+    for (int w = kThreads / 2; w > 0; w /= 2) {
+      if ((int)threadIdx.x < w) part[threadIdx.x] = real::band_merge(part[threadIdx.x], part[threadIdx.x + w]);
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) bands[m] = part[0];
+    __syncthreads();
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+mel_spectra_kernel(const cpx<T>* __restrict__ spec, const T* __restrict__ filters, const real::Band* __restrict__ bands,
+                   long bins, long n_mels, int power, T* __restrict__ out, long nframes, long g0) {
+  const long total = nframes * n_mels;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long q = g / n_mels;
+    real::mel_spectrum_one(spec, filters, bands, bins, n_mels, power, out, q, g - q * n_mels, g0 + q);
   }
 }
 
@@ -563,6 +595,92 @@ cudaError_t RealPlan<T>::istft_host(const C* in, size_t frames, const T* win, si
                       return istft_device((const C*)din, frames, (const T*)stage_spec_.data(), hop, center, (T*)dout,
                                           out_len, nb, host_stream_);
                     });
+}
+
+// The bands are recomputed on every call: the caller may change the filter matrix between calls.
+template <typename T>
+cudaError_t RealPlan<T>::mel_bands(const T* filters, size_t n_mels, cudaStream_t s) {
+  FB_CHECK(bands_.reserve(n_mels * sizeof(real::Band)));
+  mel_bands_kernel<T><<<(unsigned)std::min<size_t>(n_mels, 4096), kThreads, 0, s>>>(
+      filters, (long)(n_ / 2 + 1), (long)n_mels, (real::Band*)bands_.data());
+  FB_CHECK(cudaGetLastError());
+  launches_ += 1;
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::mel_frames(const T* in, size_t in_len, const T* win, size_t hop, int boundary,
+                                    const T* filters, size_t n_mels, int power, T* out, size_t batch, cudaStream_t s) {
+  const real::FrameMap m = real::frame_map((long)n_, (long)in_len, (long)hop, boundary);
+  const size_t total = batch * (size_t)m.frames, bins = n_ / 2 + 1;
+  const real::Band* bands = (const real::Band*)bands_.data();
+  if (path_ == Path::kRealFused) {
+    FB_CHECK(fused_->mel(in, win, filters, bands, n_mels, power, out, m, total, twa_.data(), (const C*)tab_.data(),
+                         sm_count_, s));
+    launches_ = 1;
+    return cudaSuccess;
+  }
+  // chunks of frames through seg_: the windowed frames, then their spectra from the plan's own rfft behind them, then
+  // the mels of those spectra straight into the output rows
+  const size_t chunk = std::min(total, std::max<size_t>(1, kScratchTargetBytes / (n_ * sizeof(T) + bins * sizeof(C))));
+  const size_t spec_off = (chunk * n_ * sizeof(T) + 255) / 256 * 256;
+  FB_CHECK(seg_.reserve(spec_off + chunk * bins * sizeof(C)));
+  T* seg = (T*)seg_.data();
+  C* spec = (C*)((char*)seg_.data() + spec_off);
+  unsigned long long count = 0;
+  for (size_t q0 = 0; q0 < total; q0 += chunk) {
+    const size_t nq = std::min(chunk, total - q0);
+    real::FrameMap mc = m;
+    mc.g0 = (long)q0;
+    gather_frames_kernel<T><<<grid_for(nq * n_), kThreads, 0, s>>>(in, win, seg, mc, (long)nq);
+    FB_CHECK(cudaGetLastError());
+    FB_CHECK(exec_device(true, seg, spec, nq, kFft, s));
+    count += 2 + launches_;
+    mel_spectra_kernel<T><<<grid_for(nq * n_mels), kThreads, 0, s>>>(spec, filters, bands, (long)bins, (long)n_mels,
+                                                                      power, out + q0 * n_mels, (long)nq, (long)q0);
+    FB_CHECK(cudaGetLastError());
+  }
+  launches_ = count;
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::mel_device(const T* in, size_t in_len, const T* win, size_t hop, int boundary,
+                                    const T* filters, size_t n_mels, int power, T* out, size_t batch, cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  FB_CHECK(mel_bands(filters, n_mels, s));
+  FB_CHECK(mel_frames(in, in_len, win, hop, boundary, filters, n_mels, power, out, batch, s));
+  launches_ += 1;
+  return cudaSuccess;
+}
+
+// Host pointers, on the plan's own stream: the window and the filters are staged once into stage_spec_ and their bands
+// computed once; whole rows go through stage_rows.
+template <typename T>
+cudaError_t RealPlan<T>::mel_host(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
+                                  size_t n_mels, int power, T* out, size_t batch) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
+  const size_t filt_off = (n_ * sizeof(T) + 255) / 256 * 256, filt_bytes = n_mels * (n_ / 2 + 1) * sizeof(T);
+  FB_CHECK(stage_spec_.reserve(filt_off + filt_bytes));
+  const T* dwin = (const T*)stage_spec_.data();
+  const T* dfilt = (const T*)((const char*)stage_spec_.data() + filt_off);
+  FB_CHECK(cudaMemcpyAsync(stage_spec_.data(), win, n_ * sizeof(T), cudaMemcpyHostToDevice, host_stream_));
+  FB_CHECK(cudaMemcpyAsync((char*)stage_spec_.data() + filt_off, filters, filt_bytes, cudaMemcpyHostToDevice,
+                           host_stream_));
+  FB_CHECK(mel_bands(dfilt, n_mels, host_stream_));
+  const size_t frames = (size_t)real::frame_map((long)n_, (long)in_len, (long)hop, boundary).frames;
+  FB_CHECK(stage_rows(in, out, batch, in_len * sizeof(T), frames * n_mels * sizeof(T),
+                      [&](const void* din, void* dout, size_t, size_t nb) {
+                        return mel_frames((const T*)din, in_len, dwin, hop, boundary, dfilt, n_mels, power, (T*)dout,
+                                          nb, host_stream_);
+                      }));
+  launches_ += 1;
+  return cudaSuccess;
 }
 
 template class RealPlan<float>;

@@ -306,6 +306,39 @@ int fourier_b200_istft_async_double(struct fourier_b200_rfft_double *plan, const
                                     const double *window_dev, size_t hop, int center, double *out_dev, size_t out_len,
                                     size_t batch, void *cuda_stream);
 
+/* ---- Mel spectrogram of real rows ----
+ * On a real plan of length N, with the stft's framing above (in_len, window, hop, boundary and the frame count F
+ * unchanged): out[b][f][m] = sum_{k <= N/2} filters[m][k] * |X_{b,f}[k]|^power, where X_{b,f} is the stft of frame f
+ * of row b, power is 1 or 2 and `filters` is a dense row-major (n_mels, N/2+1) matrix of any real weights, n_mels >= 1
+ * (librosa's and Whisper's layout; torchaudio's melscale_fbanks returns the transpose).  The output is frame-major,
+ * row b starting at element b*F*n_mels, frame f at b*F*n_mels + f*n_mels: with power 2 and torchaudio's own window
+ * and bank this is torchaudio.transforms.MelSpectrogram(...)(x).transpose(-1, -2).  No log is taken.
+ * Row m of the matrix is read only from its first to its last non-zero weight (its band, recomputed on every call), so
+ * a triangular bank touches about 2(N/2+1) weights per frame; zeros inside a band are multiplied like any weight, and
+ * an all-zero row gives exactly 0.  Launches: 2 on the real_fused path; on the others 1, plus per scratch chunk of
+ * frames 2 + those of the plan's rfft of that many rows.
+ * Refused with cudaErrorInvalidValue and a message: a NULL argument, hop == 0, an unknown boundary, in_len == 0, power
+ * other than 1 and 2, n_mels == 0 (these also when batch == 0, which otherwise succeeds and launches nothing), in_len < N
+ * with _NONE, in_len <= N/2 with _REFLECT, the input, window or filters overlapping the output (out of place only), and
+ * a mix of host and device buffers in the synchronous calls.  Device base pointers of input and output must be
+ * 16-byte aligned (cudaErrorMisalignedAddress).  Host memory is staged through the plan's buffers (the window and
+ * filters once, whole rows in chunks) and gives the same bits as device memory.  The _async calls take device memory,
+ * are enqueued on `cuda_stream` and not synchronised. */
+int fourier_b200_mel_spectrogram_float(struct fourier_b200_rfft_float *plan, const float *in, size_t in_len,
+                                       const float *window, size_t hop, int boundary, int power,
+                                       const float *filters, size_t n_mels, float *out, size_t batch);
+int fourier_b200_mel_spectrogram_double(struct fourier_b200_rfft_double *plan, const double *in, size_t in_len,
+                                        const double *window, size_t hop, int boundary, int power,
+                                        const double *filters, size_t n_mels, double *out, size_t batch);
+int fourier_b200_mel_spectrogram_async_float(struct fourier_b200_rfft_float *plan, const float *in_dev, size_t in_len,
+                                             const float *window_dev, size_t hop, int boundary, int power,
+                                             const float *filters_dev, size_t n_mels, float *out_dev, size_t batch,
+                                             void *cuda_stream);
+int fourier_b200_mel_spectrogram_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev,
+                                              size_t in_len, const double *window_dev, size_t hop, int boundary,
+                                              int power, const double *filters_dev, size_t n_mels, double *out_dev,
+                                              size_t batch, void *cuda_stream);
+
 const char *fourier_b200_last_error(void);
 const char *fourier_b200_version(void);
 
