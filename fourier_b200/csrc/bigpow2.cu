@@ -9,7 +9,6 @@
 //   direction at N = 2^24; the general per-stage path of this library needs one too).
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 
 #include "outer_kernels.cuh"
 #include "plan.h"
@@ -109,7 +108,6 @@ cudaError_t Plan<T>::init_bigpow2() {
   if (((size_t)1 << k) != n_ || k < k_min || k > k_max) return cudaErrorNotSupported;
   // rows of 2^14 where possible (the best tile-kernel size with 16-row tiles), the outer pass takes the rest
   int a = std::min(a_max, std::max(a_min, k - 14));
-  if (const char* env = std::getenv("FOURIER_B200_BIG_NA")) a = std::min(a_max, std::max(a_min, atoi(env)));
   const ColumnOps<T>* col = column_lookup<T>(a);
   if (!col) return cudaErrorNotSupported;
   inner_.reset(Plan<T>::create((size_t)1 << (k - a), device_, true));

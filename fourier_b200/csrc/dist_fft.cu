@@ -20,8 +20,7 @@ template <typename T> struct RowsExchangeCall {
   size_t r0, out_bs; int rb_shift; size_t rpb, rows_valid;
 };
 
-// The pass-2 tile of configuration G, or its wide tile (dist::ExchangeShape); FOURIER_B200_DIST_WIDE=0 selects the
-// narrow tiles.
+// The pass-2 tile of configuration G, or its wide tile (dist::ExchangeShape).
 template <class G, bool WIDE, typename T> struct ExchangeTile {
   using S = dist::ExchangeShape<G, WIDE, T>;
   template <bool FWD> using Tile = TileFFT<T, S::RA, S::RB, S::E, S::C, FWD>;
@@ -57,10 +56,6 @@ template <class G, bool WIDE, typename T> cudaError_t dispatch_rows_exchange(con
   constexpr int MORE = 2;
   if (c.fwd) return c.twiddle ? launch_rows_exchange<G, true, 1, MORE, WIDE>(c) : launch_rows_exchange<G, true, 0, MORE, WIDE>(c);
   return c.twiddle ? launch_rows_exchange<G, false, 2, MORE, WIDE>(c) : launch_rows_exchange<G, false, 0, MORE, WIDE>(c);
-}
-bool wide_wanted() {
-  static const bool w = [] { const char* e = std::getenv("FOURIER_B200_DIST_WIDE"); return !e || atoi(e) != 0; }();
-  return w;
 }
 
 }  // namespace
@@ -98,7 +93,7 @@ cudaError_t Plan<T>::exec_rows_exchange(const C* in, size_t rows, bool forward, 
     c2 = decltype(g)::C2;
     c2w = ExchangeTile<decltype(g), true, T>::C;
   });
-  const bool wide = wide_wanted() && c2w != c2 && rows % (size_t)c2w == 0;
+  const bool wide = c2w != c2 && rows % (size_t)c2w == 0;
   if (wide) c2 = c2w;
   if (c2 == 0 || rows % (size_t)c2) {
     set_last_error("rows_exchange: the number of rows must be a multiple of " + std::to_string(c2));
@@ -114,13 +109,12 @@ cudaError_t Plan<T>::exec_rows_exchange(const C* in, size_t rows, bool forward, 
   else if (const char* e2 = std::getenv("FOURIER_B200_CHUNK_MB")) mb = (size_t)std::max(1, atoi(e2));
   const size_t want = std::max<size_t>(1, (mb << 20) / (n_ * sizeof(C)));
   size_t chunk = std::max<size_t>((size_t)c2, std::min(want, rows) / (size_t)c2 * (size_t)c2);
-  // lanes: chunks rotate over the caller's stream and up to three plan-owned ones, each with its own intermediate
+  // lanes: chunks alternate between the caller's stream and a plan-owned one, each with its own intermediate
   int nlanes = 2;
-  if (const char* env = std::getenv("FOURIER_B200_DIST_LANES")) nlanes = std::min(4, std::max(1, atoi(env)));
   if (const char* env = std::getenv("FOURIER_B200_DIST_OVERLAP")) { if (atoi(env) == 0) nlanes = 1; }
   nlanes = (int)std::min<size_t>((size_t)nlanes, (rows + chunk - 1) / chunk);
   FB_CHECK(work_.reserve((size_t)nlanes * chunk * n_ * sizeof(C)));
-  cudaStream_t lanes[4] = {s, s, s, s};
+  cudaStream_t lanes[2] = {s, s};
   if (nlanes > 1) {
     FB_CHECK(host_resources());
     FB_CHECK(cudaEventRecord(events_[0], s));

@@ -10,7 +10,6 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 
 namespace fb200 {
@@ -119,18 +118,14 @@ cudaError_t Plan<T>::init(size_t n, int device, bool allow_fast_paths) {
     const bool pow2 = (n & (n - 1)) == 0;
     if (allow_fast_paths && pow2) {
       if (init_onchip() == cudaSuccess) { path_ = Path::kOnChip; return cudaSuccess; }
-      // FOURIER_B200_TWOPASS=0 (experiment knob): skip the two-pass kernels, so that sizes the CTA kernel also
-      // covers can be measured on it
-      const char* tp = std::getenv("FOURIER_B200_TWOPASS");
-      if (!(tp && atoi(tp) == 0) && init_twopass() == cudaSuccess) { path_ = Path::kTwoPass; return cudaSuccess; }
+      if (init_twopass() == cudaSuccess) { path_ = Path::kTwoPass; return cudaSuccess; }
       // beyond the two-pass sizes: an outer column pass around two-pass rows (bigpow2.cu)
-      if (!(tp && atoi(tp) == 0) && init_bigpow2() == cudaSuccess) { path_ = Path::kThreePass; return cudaSuccess; }
+      if (init_bigpow2() == cudaSuccess) { path_ = Path::kThreePass; return cudaSuccess; }
     }
     // everything else that fits two shared-memory buffers: one kernel, one HBM round trip
     if (allow_fast_paths && init_cta(n) == cudaSuccess) { path_ = Path::kCta; return cudaSuccess; }
     // 3^b * 2^k (b <= 3) with a two-pass power of two: outer radix-3^b pass + two-pass rows (bigpow2.cu)
-    const char* tp3 = std::getenv("FOURIER_B200_TWOPASS");   // =0 (experiment knob): measure the per-stage path instead
-    if (allow_fast_paths && !pow2 && !(tp3 && atoi(tp3) == 0) && init_threepass_radix3() == cudaSuccess) {
+    if (allow_fast_paths && !pow2 && init_threepass_radix3() == cudaSuccess) {
       path_ = Path::kThreePass;
       return cudaSuccess;
     }
@@ -332,7 +327,7 @@ cudaError_t Plan<T>::exec_host(const C* in, C* out, size_t batch, int code) {
     // Latency path (the reference ABI's single small transform, fourier-ffi/src/lib.rs:46-59): nothing to
     // pipeline, so one stream, no events, one synchronisation: H2D, kernel(s), D2H back to back.
     cudaStream_t s = streams_[1];
-    if (batch * bytes_per <= kHostZeroCopyBytes && !std::getenv("FOURIER_B200_NO_ZEROCOPY")) {
+    if (batch * bytes_per <= kHostZeroCopyBytes) {
       // Smallest calls: the two DMA copies cost more than the transform.  The kernels read the input from and write
       // the result to a pinned, device-mapped bounce buffer over PCIe themselves (one launch, one synchronisation;
       // the CPU copies 2 x <= 64 KB).

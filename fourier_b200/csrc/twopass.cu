@@ -96,14 +96,10 @@ template <class Cfg> struct FusedImpl {
   }
 };
 
-// The configuration of N = 2^LOG2N (fused_configs.cuh); FOURIER_B200_CFG=1 selects the other load strategy,
-// FOURIER_B200_PAIR=0 one item per group where the default claims pairs (experiments).
+// The configuration of N = 2^LOG2N (fused_configs.cuh); FOURIER_B200_PAIR=0 one item per group where it claims pairs
+// (the bit-identity reference of the pair items).
 template <typename T, int LOG2N> const FusedOps<T>* fused_pick() {
   using D = fused::FusedConfig<T, LOG2N>;
-  using A = fused::FusedConfig<T, LOG2N, true>;
-  if constexpr (A::HAS) {
-    if (env_int("FOURIER_B200_CFG", 0) == 1) return FusedImpl<typename A::Cfg>::ops(A::RING, A::LAG);
-  }
   if constexpr (D::Cfg::PAIR) {
     if (env_int("FOURIER_B200_PAIR", 1) == 0) return FusedImpl<typename D::Cfg::Unpaired>::ops(D::RING, D::LAG);
   }

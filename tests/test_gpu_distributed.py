@@ -88,12 +88,6 @@ def test_peer_exchange_kernel_layout(real, forward):
         assert rel_err(outs[q].cpu().numpy(), want) < (5e-7 if real == "f32" else 4e-15)
 
 
-def test_peer_exchange_kernel_persistent_variant(monkeypatch):
-    monkeypatch.setenv("FOURIER_B200_EXCHANGE_BLOCKS", "7")      # 7 blocks walk 4 * 2 * 1 = 8+ tiles each
-    test_peer_exchange_kernel_layout("f32", True)
-    test_peer_exchange_kernel_layout("f64", None)
-
-
 @pytest.mark.parametrize("real,n,P,rows_loc", [("f32", 1 << 14, 4, 64), ("f32", 1 << 11, 2, 96), ("f32", 1 << 16, 8, 48),
                                                ("f32", 1 << 20, 2, 16), ("f64", 1 << 12, 4, 32), ("f64", 1 << 16, 2, 24),
                                                # 64 / 32 rows: tiles of 32 (f32) / 16 (f64) transforms, 256-byte store runs

@@ -2,7 +2,8 @@
 
 A race in its work queue, ring or readiness counters does not change the arithmetic: it makes a few transforms of a
 long batch wrong (stale data from transform b - RING, a tile read before it was stored, a slot overwritten early, a tile
-never stored).  So every configuration runs a batch that wraps its ring at least twice under full load, and every
+never stored).  So every configuration runs a batch that wraps its ring at least twice under full load, and the same
+batch on the smallest ring (RING=2, LAG=1: every pass-1 tile waits for the slot of transform b - 2), and every
 transform of it is checked
 
   1. against numpy's FFT in long double, per transform, within the bounds tools/emulate.cu enforces on the same tile
@@ -33,17 +34,17 @@ TDT = {"f32": torch.complex64, "f64": torch.complex128}
 BITS = {"f32": torch.int32, "f64": torch.int64}
 TOL = {"f32": 2e-6, "f64": 5e-15}
 FIRST, DECOY = 5, 100003          # first_transform of the checked input and of the decoy input
-KNOBS = ("FOURIER_B200_CFG", "FOURIER_B200_FUSED", "FOURIER_B200_CHUNK_MB", "FOURIER_B200_RING", "FOURIER_B200_LAG")
+KNOBS = ("FOURIER_B200_FUSED", "FOURIER_B200_CHUNK_MB", "FOURIER_B200_RING", "FOURIER_B200_LAG")
 
-DEFAULTS = [("f32", 1 << k) for k in range(13, 21)] + [("f64", 1 << k) for k in (12, 13, 14, 16)]
-ALTERNATIVES = [c for c in DEFAULTS if c != ("f32", 1 << 19)]    # FOURIER_B200_CFG=1: the other load strategy
-CONFIGS = [(r, n, False) for r, n in DEFAULTS] + [(r, n, True) for r, n in ALTERNATIVES]
+SIZES = [("f32", 1 << k) for k in range(13, 21)] + [("f64", 1 << k) for k in (12, 13, 14, 16)]
+CONFIGS = [(r, n, False) for r, n in SIZES] + [(r, n, True) for r, n in SIZES]   # True: RING=2, LAG=1
+SMALLEST_RING = {"FOURIER_B200_RING": 2, "FOURIER_B200_LAG": 1}
 DESC = re.compile(r"^fused::fused_twopass_kernel \[(\d+)x(\d+), (\d+) groups x (\d+), (TMA staging|direct loads), "
                   r"ring (\d+), lag (\d+)\]$")
 
 
 def _id(c):
-    return f"{c[0]}-2^{c[1].bit_length() - 1}-{'cfg1' if c[2] else 'default'}"
+    return f"{c[0]}-2^{c[1].bit_length() - 1}-{'ring2' if c[2] else 'default'}"
 
 
 def make_plan(monkeypatch, real, n, **env):
@@ -58,9 +59,9 @@ def make_plan(monkeypatch, real, n, **env):
     return p
 
 
-def persistent_plan(monkeypatch, real, n, alt):
+def persistent_plan(monkeypatch, real, n, **env):
     """-> plan, its configuration parsed from kernel_name()"""
-    p = make_plan(monkeypatch, real, n, **({"FOURIER_B200_CFG": 1} if alt else {}))
+    p = make_plan(monkeypatch, real, n, **env)
     name = p.kernel_name()
     m = DESC.match(name)
     assert m, f"not a persistent-kernel description: {name!r}"
@@ -136,21 +137,20 @@ def check_bits(got, want, real, ring, what):
 
 # ---- 1. every persistent configuration, at a batch that wraps its ring under full load ---------------------------
 
-@pytest.mark.parametrize("real,n,alt", CONFIGS, ids=[_id(c) for c in CONFIGS])
-def test_every_transform_of_a_ring_wrapping_batch(monkeypatch, real, n, alt):
-    p, cfg = persistent_plan(monkeypatch, real, n, alt)
-    if alt:
-        d, default = persistent_plan(monkeypatch, real, n, False)
-        d.close()
-        default = default["name"]
-        assert cfg["name"] != default, f"FOURIER_B200_CFG=1 chose the default configuration {default!r}"
-    ring, lag = cfg["ring"], cfg["lag"]
-    batch = 2 * ring + lag + 3     # wraps the ring at least twice; prologue and epilogue of the queue both run
+@pytest.mark.parametrize("real,n,smallest", CONFIGS, ids=[_id(c) for c in CONFIGS])
+def test_every_transform_of_a_ring_wrapping_batch(monkeypatch, real, n, smallest):
+    p, cfg = persistent_plan(monkeypatch, real, n)
+    batch = 2 * cfg["ring"] + cfg["lag"] + 3     # wraps the default ring at least twice; prologue and epilogue run
+    if smallest:
+        p.close()
+        p, cfg = persistent_plan(monkeypatch, real, n, **SMALLEST_RING)
+        assert (cfg["ring"], cfg["lag"]) == (2, 1), cfg["name"]
+    ring = cfg["ring"]
     window = 2 * cfg["groups"] * torch.cuda.get_device_properties(0).multi_processor_count
     x = device_input(real, batch, n, FIRST)
     decoy = device_input(real, batch, n, DECOY)
     xh = host_input(real, batch, n, FIRST, x)
-    codes = list(T) if not alt else [T.Fft, T.SqrtScaledIfft]
+    codes = list(T) if not smallest else [T.Fft, T.SqrtScaledIfft]
     bit_codes = (T.Fft, T.SqrtScaledIfft)
     failures, worst = [], {}
     unscaled, direction = None, None
@@ -170,7 +170,7 @@ def test_every_transform_of_a_ring_wrapping_batch(monkeypatch, real, n, alt):
             single = one_by_one(p, x, code)
             failures += [m for m in [check_bits(out, single, real, ring, f"{code.name} batch {batch} vs batch 1")] if m]
     torch.cuda.synchronize()
-    print(f"\n{real} N=2^{n.bit_length() - 1} {'CFG=1  ' if alt else 'default'} {cfg['name']}: B={batch} "
+    print(f"\n{real} N=2^{n.bit_length() - 1} {cfg['name']}: B={batch} "
           f"({batch / ring:.2f} rings), ~{window} work items in flight; worst per-transform error "
           + " ".join(f"{c} {e:.2e}" for c, e in worst.items()))
     p.close()
@@ -185,7 +185,7 @@ def _sweep(ring, lag):
 
 @pytest.mark.parametrize("real,n", [("f32", 1 << 13), ("f32", 1 << 20), ("f64", 1 << 16)])
 def test_batches_across_the_ring_shrink_rule(monkeypatch, real, n):
-    p, cfg = persistent_plan(monkeypatch, real, n, False)
+    p, cfg = persistent_plan(monkeypatch, real, n)
     ring, lag = cfg["ring"], cfg["lag"]
     if ring <= 8:
         batches = list(range(1, 2 * ring + 2))

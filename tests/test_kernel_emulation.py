@@ -15,9 +15,8 @@ from helpers import run_emulator
 ONCHIP = {"f32": (64, 128, 256, 512, 1024), "f64": (64, 128, 256)}
 BLUESTEIN = {"f32": (64, 256, 1024), "f64": (64, 256)}
 TWOPASS = {"f32": range(11, 21), "f64": range(9, 17)}
-# persistent kernel: the default configuration of every size, and the sizes with an alternative (FOURIER_B200_CFG=1)
+# persistent kernel: the configuration of every size
 FUSED = {"f32": range(13, 21), "f64": (12, 13, 14, 16)}
-FUSED_ALT = {"f32": (13, 14, 15, 16, 17, 18, 20), "f64": (12, 13, 14, 16)}
 
 
 @pytest.fixture(scope="module")
@@ -71,7 +70,6 @@ def test_every_two_pass_size_ran(emulation):
 def test_every_persistent_configuration_ran(emulation):
     b = blocks(emulation.stdout)
     labels = [f"fused {p} 2^{k}" for p, ks in FUSED.items() for k in ks]
-    labels += [f"fused {p} 2^{k} (FOURIER_B200_CFG=1)" for p, ks in FUSED_ALT.items() for k in ks]
     for label in labels:
         assert label in b and both_directions_ok(b[label]), (label, b.get(label))
 

@@ -1,6 +1,5 @@
-"""Round-2 sweep of BASELINE configs[4] (one N = 2^30 transform over all ranks, peer-memory exchange): number of
-persistent exchange blocks (FOURIER_B200_EXCHANGE_BLOCKS; 0 = one block per tile) x pipelined row-block chunks,
-natural and transposed output, and the N1 x N2 split.  torchrun, one rank per GPU:
+"""Round-2 sweep of BASELINE configs[4] (one N = 2^30 transform over all ranks, peer-memory exchange): pipelined
+row-block chunks, natural and transposed output, and the N1 x N2 split.  torchrun, one rank per GPU:
     PYTHONPATH=. python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 tools/c5_sweep.py [log2 N]
 Prints one JSON line "C5SWEEP {...}" (ms per transform, max over ranks, CUDA events)."""
 import json
@@ -55,19 +54,10 @@ for k1 in (k // 2, k // 2 - 1):
         out = plan.transform(state[0], state[1], natural_order=natural)
         state[0], state[1] = out, (state[0] if out is state[1] else state[1])
 
-    for blocks in (0, 32, 64, 128, 256):
-        if blocks:
-            os.environ["FOURIER_B200_EXCHANGE_BLOCKS"] = str(blocks)
-        else:
-            os.environ.pop("FOURIER_B200_EXCHANGE_BLOCKS", None)
-        for chunks in (1, 4, 8):
-            if blocks == 0 and chunks == 8:
-                continue
-            plan.chunks = chunks
-            res["ms"][f"{n1}x{n2} blocks={blocks} chunks={chunks} natural"] = timed(step)
-            if chunks in (1, 4):
-                res["ms"][f"{n1}x{n2} blocks={blocks} chunks={chunks} transposed"] = timed(lambda: step(False))
-    os.environ.pop("FOURIER_B200_EXCHANGE_BLOCKS", None)
+    for chunks in (1, 4):
+        plan.chunks = chunks
+        res["ms"][f"{n1}x{n2} chunks={chunks} natural"] = timed(step)
+        res["ms"][f"{n1}x{n2} chunks={chunks} transposed"] = timed(lambda: step(False))
     plan.chunks = 1
     r1 = n1 // world
     res["ms"][f"{n1}x{n2} exchange only"] = timed(lambda: plan._fft_then_exchange(a, b, r1, n2, 0, True, None))

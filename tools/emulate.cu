@@ -745,20 +745,12 @@ template <typename T> static int bluestein(long n, double tol) {
   return bad < 0 ? 1 : bad;
 }
 
-// the persistent kernel of N = 2^LOG2N (fused_configs.cuh): the default configuration and the alternative
-// (FOURIER_B200_CFG=1) where there is one; pair items (PairCfg) change only which tiles a group claims, so the default
-// runs as its Unpaired configuration
+// the persistent kernel of N = 2^LOG2N (fused_configs.cuh); pair items (PairCfg) change only which tiles a group
+// claims, so a paired configuration runs as its Unpaired one
 template <typename T, int LOG2N> static int check_persistent(double tol) {
-  using D = fused::FusedConfig<T, LOG2N>;
-  using A = fused::FusedConfig<T, LOG2N, true>;
   char name[64];
   snprintf(name, sizeof name, "fused %s 2^%d", prec<T>(), LOG2N);
-  int bad = check_fused<typename D::Cfg::Unpaired>(name, tol);
-  if constexpr (A::HAS) {
-    snprintf(name, sizeof name, "fused %s 2^%d (FOURIER_B200_CFG=1)", prec<T>(), LOG2N);
-    bad += check_fused<typename A::Cfg>(name, tol);
-  }
-  return bad;
+  return check_fused<typename fused::FusedConfig<T, LOG2N>::Cfg::Unpaired>(name, tol);
 }
 
 // the work queue of the default configuration of N = 2^LOG2N, and with pair items also the one item per group that
