@@ -293,13 +293,25 @@ class RealFft:
         if di != do_:
             raise ValueError("input and output must both be host or both be device buffers")
         batch = int(np.prod(li, dtype=np.int64))
+        self._call(f"rfft_{direction}", f"real {direction} transform", di, si, pi, po, batch, code)
+
+    def _call(self, symbol, what, on_device, stream, *args):
+        """fourier_b200_<symbol>_<t>(plan, *args), or on device buffers fourier_b200_<symbol>_async_<t>(plan, *args,
+        stream); RuntimeError naming `what` if it fails."""
         L = _lib.load()
-        if di:
-            rc = getattr(L, f"fourier_b200_rfft_{direction}_async_{self._t}")(self._plan, pi, po, batch, code, si)
+        if on_device:
+            rc = getattr(L, f"fourier_b200_{symbol}_async_{self._t}")(self._plan, *args, stream)
         else:
-            rc = getattr(L, f"fourier_b200_rfft_{direction}_{self._t}")(self._plan, pi, po, batch, code)
+            rc = getattr(L, f"fourier_b200_{symbol}_{self._t}")(self._plan, *args)
         if rc != 0:
-            raise RuntimeError(f"real {direction} transform failed (cuda error {rc}): {_lib.last_error()}")
+            raise RuntimeError(f"{what} failed (cuda error {rc}): {_lib.last_error()}")
+
+    @staticmethod
+    def _check_resolved(*buffers):
+        for x in buffers:
+            if _is_torch(x) and (x.is_conj() or x.is_neg()):
+                raise ValueError("torch tensors with the conj or neg bit set hold unconjugated data: "
+                                 "pass x.resolve_conj() (and resolve_neg()) instead")
 
     def convolve(self, input, spectrum, output):
         """output = numpy.fft.irfft(numpy.fft.rfft(input) * spectrum, n=N): circular convolution of every row of
@@ -308,10 +320,7 @@ class RealFft:
         broadcast over the rest: () means one filter for all rows, (C,) one per channel for input (B, C, N), the
         input's whole leading shape one per row.  `output` has the input's shape and may be `input`
         itself.  Correlation: pass conj(H), resolved (spectrum.conj().resolve_conj() for torch)."""
-        for x in (input, spectrum, output):
-            if _is_torch(x) and (x.is_conj() or x.is_neg()):
-                raise ValueError("torch tensors with the conj or neg bit set hold unconjugated data: "
-                                 "pass x.resolve_conj() (and resolve_neg()) instead")
+        self._check_resolved(input, spectrum, output)
         pi, li, di, si = self._describe(input, "real")
         ps, ls, ds, _ = self._describe(spectrum, "spec")
         po, lo, do_, _ = self._describe(output, "real")
@@ -323,13 +332,7 @@ class RealFft:
             raise ValueError("input, spectrum and output must all be host or all be device buffers")
         batch = int(np.prod(li, dtype=np.int64))
         rows = int(np.prod(ls, dtype=np.int64))
-        L = _lib.load()
-        if di:
-            rc = getattr(L, f"fourier_b200_convolve_real_async_{self._t}")(self._plan, pi, ps, rows, po, batch, si)
-        else:
-            rc = getattr(L, f"fourier_b200_convolve_real_{self._t}")(self._plan, pi, ps, rows, po, batch)
-        if rc != 0:
-            raise RuntimeError(f"real convolution failed (cuda error {rc}): {_lib.last_error()}")
+        self._call("convolve_real", "real convolution", di, si, pi, ps, rows, po, batch)
 
     LINEAR_MODES = {"full": 0, "same": 1, "valid": 2}
 
@@ -340,10 +343,7 @@ class RealFft:
         spectrum broadcasts over the input's leading shape as in convolve.  Rows are filtered by overlap-save in
         segments of N - K + 1 outputs, so N should be a few times K.  If irfft(spectrum) has non-zero samples beyond
         the first K, the result is unspecified.  Out of place only; correlation: pass conj(H), resolved."""
-        for x in (input, spectrum, output):
-            if _is_torch(x) and (x.is_conj() or x.is_neg()):
-                raise ValueError("torch tensors with the conj or neg bit set hold unconjugated data: "
-                                 "pass x.resolve_conj() (and resolve_neg()) instead")
+        self._check_resolved(input, spectrum, output)
         if mode not in self.LINEAR_MODES:
             raise ValueError(f"mode must be one of {sorted(self.LINEAR_MODES)}, got {mode!r}")
         taps = int(taps)
@@ -369,16 +369,8 @@ class RealFft:
             raise ValueError("input, spectrum and output must all be host or all be device buffers")
         batch = int(np.prod(li, dtype=np.int64))
         rows = int(np.prod(ls, dtype=np.int64))
-        code = self.LINEAR_MODES[mode]
-        L = _lib.load()
-        if di:
-            rc = getattr(L, f"fourier_b200_linear_convolve_real_async_{self._t}")(
-                self._plan, pi, in_len, ps, rows, taps, code, po, batch, si)
-        else:
-            rc = getattr(L, f"fourier_b200_linear_convolve_real_{self._t}")(
-                self._plan, pi, in_len, ps, rows, taps, code, po, batch)
-        if rc != 0:
-            raise RuntimeError(f"linear convolution failed (cuda error {rc}): {_lib.last_error()}")
+        self._call("linear_convolve_real", "linear convolution", di, si, pi, in_len, ps, rows, taps,
+                   self.LINEAR_MODES[mode], po, batch)
 
     STFT_PAD_MODES = {"constant": 1, "reflect": 2}
 
@@ -388,20 +380,10 @@ class RealFft:
         pad = self._size // 2 if center else 0
         return 1 + (int(in_len) + 2 * pad - self._size) // int(hop)
 
-    def _stft_buffers(self, buffers):
-        for x in buffers:
-            if _is_torch(x) and (x.is_conj() or x.is_neg()):
-                raise ValueError("torch tensors with the conj or neg bit set hold unconjugated data: "
-                                 "pass x.resolve_conj() (and resolve_neg()) instead")
-
-    def stft(self, input, window, hop, output, center=True, pad_mode="reflect"):
-        """Short-time Fourier transform of every row of `input` (shape (..., L)): frames of N = size() samples every
-        `hop`, times `window` (N reals; zero-pad a shorter one), through rfft.  `output` has shape (..., F, N//2+1),
-        F = stft_frames(L, hop, center), frame-major: this is torch.stft(x, N, hop, window=window, center=center,
-        pad_mode=pad_mode, return_complex=True).transpose(-1, -2).  With center the rows are padded by N//2 on both
-        sides, with zeros (pad_mode "constant") or mirrored without repeating the edge ("reflect", needs L > N//2);
-        pad_mode is ignored without center, which needs L >= N.  Out of place only."""
-        self._stft_buffers((input, window, output))
+    def _framing(self, input, window, hop, center, pad_mode):
+        """The framing of stft and mel_spectrogram: checks pad_mode, hop and the row length against N, and describes
+        the input and the window -> (hop, boundary, in_len, frames, (pointer, leading shape, is_device, stream) of the
+        input, (pointer, is_device) of the window)"""
         if center and pad_mode not in self.STFT_PAD_MODES:
             raise ValueError(f"pad_mode must be one of {sorted(self.STFT_PAD_MODES)}, got {pad_mode!r}")
         hop = int(hop)
@@ -417,10 +399,22 @@ class RealFft:
         if boundary == 2 and in_len <= n // 2:
             raise ValueError(f"pad_mode 'reflect' needs rows of more than N//2 = {n // 2} samples, got {in_len}")
         frames = self.stft_frames(in_len, hop, center)
-        pi, li, di, si = self._describe(input, "real", last=in_len)
+        src = self._describe(input, "real", last=in_len)
         pw, lw, dw, _ = self._describe(window, "real")
         if lw != ():
             raise ValueError(f"window must hold exactly N = {n} reals, got shape {tuple(window.shape)}")
+        return hop, boundary, in_len, frames, src, (pw, dw)
+
+    def stft(self, input, window, hop, output, center=True, pad_mode="reflect"):
+        """Short-time Fourier transform of every row of `input` (shape (..., L)): frames of N = size() samples every
+        `hop`, times `window` (N reals; zero-pad a shorter one), through rfft.  `output` has shape (..., F, N//2+1),
+        F = stft_frames(L, hop, center), frame-major: this is torch.stft(x, N, hop, window=window, center=center,
+        pad_mode=pad_mode, return_complex=True).transpose(-1, -2).  With center the rows are padded by N//2 on both
+        sides, with zeros (pad_mode "constant") or mirrored without repeating the edge ("reflect", needs L > N//2);
+        pad_mode is ignored without center, which needs L >= N.  Out of place only."""
+        self._check_resolved(input, window, output)
+        hop, boundary, in_len, frames, (pi, li, di, si), (pw, dw) = self._framing(input, window, hop, center, pad_mode)
+        n = self._size
         if getattr(output, "ndim", 0) < 2 or output.shape[-2] != frames:
             raise ValueError(f"output must have shape (..., {frames}, {n // 2 + 1}) (F = {frames} frames)")
         po, lo, do_, _ = self._describe(output, "spec")
@@ -429,14 +423,7 @@ class RealFft:
         if not (di == dw == do_):
             raise ValueError("input, window and output must all be host or all be device buffers")
         batch = int(np.prod(li, dtype=np.int64))
-        L = _lib.load()
-        if di:
-            rc = getattr(L, f"fourier_b200_stft_async_{self._t}")(self._plan, pi, in_len, pw, hop, boundary, po, batch,
-                                                                   si)
-        else:
-            rc = getattr(L, f"fourier_b200_stft_{self._t}")(self._plan, pi, in_len, pw, hop, boundary, po, batch)
-        if rc != 0:
-            raise RuntimeError(f"stft failed (cuda error {rc}): {_lib.last_error()}")
+        self._call("stft", "stft", di, si, pi, in_len, pw, hop, boundary, po, batch)
 
     def mel_spectrogram(self, input, window, hop, filters, output, power=2, center=True, pad_mode="reflect"):
         """Mel spectrogram of every row of `input` (shape (..., L)) with stft's framing: output[..., f, m] =
@@ -446,28 +433,11 @@ class RealFft:
         (..., F, n_mels), F = stft_frames(L, hop, center): with power 2 and torchaudio's own window and bank this is
         torchaudio.transforms.MelSpectrogram(...)(x).transpose(-1, -2).  The spectrum stays on chip where the plan's
         path allows.  Out of place only."""
-        self._stft_buffers((input, window, filters, output))
-        if center and pad_mode not in self.STFT_PAD_MODES:
-            raise ValueError(f"pad_mode must be one of {sorted(self.STFT_PAD_MODES)}, got {pad_mode!r}")
-        hop = int(hop)
-        if hop < 1:
-            raise ValueError(f"hop must be at least 1, got {hop}")
+        self._check_resolved(input, window, filters, output)
         if power not in (1, 2):
             raise ValueError(f"power must be 1 or 2, got {power!r}")
-        boundary = self.STFT_PAD_MODES[pad_mode] if center else 0
+        hop, boundary, in_len, frames, (pi, li, di, si), (pw, dw) = self._framing(input, window, hop, center, pad_mode)
         n = self._size
-        in_len = input.shape[-1] if getattr(input, "ndim", 0) > 0 else 0
-        if in_len < 1:
-            raise ValueError("input rows must hold at least one sample")
-        if boundary == 0 and in_len < n:
-            raise ValueError(f"center=False needs rows of at least N = {n} samples, got {in_len}")
-        if boundary == 2 and in_len <= n // 2:
-            raise ValueError(f"pad_mode 'reflect' needs rows of more than N//2 = {n // 2} samples, got {in_len}")
-        frames = self.stft_frames(in_len, hop, center)
-        pi, li, di, si = self._describe(input, "real", last=in_len)
-        pw, lw, dw, _ = self._describe(window, "real")
-        if lw != ():
-            raise ValueError(f"window must hold exactly N = {n} reals, got shape {tuple(window.shape)}")
         if getattr(filters, "ndim", 0) != 2:
             raise ValueError(f"filters must have shape (n_mels, {n // 2 + 1})")
         pf, lf, df, _ = self._describe(filters, "real", last=n // 2 + 1)
@@ -484,15 +454,8 @@ class RealFft:
         batch = int(np.prod(li, dtype=np.int64))
         if batch == 0:
             return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
-        L = _lib.load()
-        if di:
-            rc = getattr(L, f"fourier_b200_mel_spectrogram_async_{self._t}")(
-                self._plan, pi, in_len, pw, hop, boundary, int(power), pf, n_mels, po, batch, si)
-        else:
-            rc = getattr(L, f"fourier_b200_mel_spectrogram_{self._t}")(
-                self._plan, pi, in_len, pw, hop, boundary, int(power), pf, n_mels, po, batch)
-        if rc != 0:
-            raise RuntimeError(f"mel spectrogram failed (cuda error {rc}): {_lib.last_error()}")
+        self._call("mel_spectrogram", "mel spectrogram", di, si, pi, in_len, pw, hop, boundary, int(power), pf, n_mels,
+                   po, batch)
 
     def istft(self, input, window, hop, output, center=True):
         """Inverse of stft: `input` (shape (..., F, N//2+1), stft's frame-major layout) -> `output` (shape
@@ -501,7 +464,7 @@ class RealFft:
         sum is below 1e-11, including positions no frame covers (torch.istft raises instead).  With out_len =
         hop * (F - 1) + N - 2 pad this is torch.istft(input.transpose(-1, -2), N, hop, window=window, center=center,
         length=out_len).  Out of place only."""
-        self._stft_buffers((input, window, output))
+        self._check_resolved(input, window, output)
         hop = int(hop)
         if hop < 1:
             raise ValueError(f"hop must be at least 1, got {hop}")
@@ -522,15 +485,7 @@ class RealFft:
         if not (di == dw == do_):
             raise ValueError("input, window and output must all be host or all be device buffers")
         batch = int(np.prod(lo, dtype=np.int64))
-        L = _lib.load()
-        if di:
-            rc = getattr(L, f"fourier_b200_istft_async_{self._t}")(self._plan, pi, frames, pw, hop, int(bool(center)),
-                                                                    po, out_len, batch, si)
-        else:
-            rc = getattr(L, f"fourier_b200_istft_{self._t}")(self._plan, pi, frames, pw, hop, int(bool(center)), po,
-                                                              out_len, batch)
-        if rc != 0:
-            raise RuntimeError(f"istft failed (cuda error {rc}): {_lib.last_error()}")
+        self._call("istft", "istft", di, si, pi, frames, pw, hop, int(bool(center)), po, out_len, batch)
 
     def rfft(self, input, output, transform=Transform.Fft):
         """output[..., :N//2+1] = numpy.fft.rfft(input) (Fft) or that times 1/sqrt(N) (SqrtScaledFft)."""

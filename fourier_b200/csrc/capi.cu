@@ -41,8 +41,7 @@ bool is_device_pointer(const void* p) {
 
 // Where the buffers of a synchronous call live: 1 all in device memory, 0 all in host memory, -1 a mix, which is
 // refused (last_error set to `mix`).
-int residence(std::initializer_list<const void*> bufs,
-              const char* mix = "input and output must both be host or both be device memory") {
+int residence(std::initializer_list<const void*> bufs, const char* mix) {
   const bool dev = is_device_pointer(*bufs.begin());
   for (auto p = bufs.begin() + 1; p != bufs.end(); ++p)
     if (is_device_pointer(*p) != dev) {
@@ -56,8 +55,10 @@ int residence(std::initializer_list<const void*> bufs,
 // float4, TMA tensor maps on the input): a misaligned device pointer would fault and poison the CUDA context, so it
 // is refused up front.  (cudaMalloc and torch allocations are 256/512-byte aligned; a slice starting at an odd f32
 // sample is not.)  Host pointers are staged through the library's own buffers and may have any alignment.
-bool device_pointers_aligned(const void* in, const void* out) {
-  if ((((uintptr_t)in) | ((uintptr_t)out)) & 15) {
+bool device_pointers_aligned(std::initializer_list<const void*> bufs) {
+  uintptr_t bits = 0;
+  for (const void* p : bufs) bits |= (uintptr_t)p;
+  if (bits & 15) {
     fb200::set_last_error("device buffers must be 16-byte aligned");
     return false;
   }
@@ -80,27 +81,45 @@ void* create(size_t size, bool fast) {
   }
 }
 
-// async: device pointers on `stream`, not synchronised; otherwise host or device pointers, synchronised.
+// returned by run_call's checks() to go on with the call
+constexpr int kRun = -1;
+
+// The end of every batched entry point, after its checks that need no plan.  checks() makes the entry point's other
+// checks and returns kRun, or else the call's result.  A synchronous call then needs `bufs` all in host or all in
+// device memory (else last_error = `mix`), and runs host() on host memory.  Otherwise the device buffers `aligned`
+// must be 16-byte aligned, and device(s) runs on the caller's `stream` if async (not synchronised), else on the
+// per-thread default stream, synchronised.  An exception becomes "<what> threw".
+template <class Checks, class Host, class Device>
+int run_call(const char* what, bool async, void* stream, Checks checks, std::initializer_list<const void*> bufs,
+             const char* mix, Host host, std::initializer_list<const void*> aligned, Device device) {
+  try {
+    if (const int rc = checks(); rc != kRun) return rc;
+    if (!async) {
+      const int dev = residence(bufs, mix);
+      if (dev < 0) return (int)cudaErrorInvalidValue;
+      if (!dev) return (int)host();
+    }
+    if (!device_pointers_aligned(aligned)) return (int)cudaErrorMisalignedAddress;
+    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
+    cudaError_t e = device(s);
+    if (e != cudaSuccess || async) return (int)e;
+    return (int)cudaStreamSynchronize(s);
+  } catch (...) {
+    fb200::set_last_error(std::string(what) + " threw");
+    return (int)cudaErrorUnknown;
+  }
+}
+
 template <typename T>
 int fft_exec(const void* plan, const void* in, void* out, size_t batch, int code, bool async, void* stream) {
   if (!plan || !in || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
   auto* p = const_cast<Plan<T>*>(static_cast<const Plan<T>*>(plan));
   using C = typename Plan<T>::C;
-  try {
-    if (!async) {
-      const int dev = residence({in, out});
-      if (dev < 0) return (int)cudaErrorInvalidValue;
-      if (!dev) return (int)p->exec_host((const C*)in, (C*)out, batch, code);
-    }
-    if (!device_pointers_aligned(in, out)) return (int)cudaErrorMisalignedAddress;
-    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
-    cudaError_t e = p->exec_device((const C*)in, (C*)out, batch, code, s);
-    if (e != cudaSuccess || async) return (int)e;
-    return (int)cudaStreamSynchronize(s);
-  } catch (...) {
-    fb200::set_last_error("transform threw");
-    return (int)cudaErrorUnknown;
-  }
+  return run_call(
+      "transform", async, stream, [] { return kRun; },
+      {in, out}, "input and output must both be host or both be device memory",
+      [&] { return p->exec_host((const C*)in, (C*)out, batch, code); },
+      {in, out}, [&](cudaStream_t s) { return p->exec_device((const C*)in, (C*)out, batch, code, s); });
 }
 
 template <typename T>
@@ -111,7 +130,7 @@ int rows_exchange(const void* plan, const void* in, size_t rows, int forward, vo
   auto* p = const_cast<Plan<T>*>(static_cast<const Plan<T>*>(plan));
   using C = typename Plan<T>::C;
   try {
-    if (!device_pointers_aligned(in, in)) return (int)cudaErrorMisalignedAddress;
+    if (!device_pointers_aligned({in})) return (int)cudaErrorMisalignedAddress;
     return (int)p->exec_rows_exchange((const C*)in, rows, forward != 0, outs, nranks, out_ld, out_off, twiddle, row0,
                                       n_total, (cudaStream_t)stream);
   } catch (...) {
@@ -147,30 +166,22 @@ bool disjoint(const void* in, size_t in_bytes, const void* out, size_t out_bytes
   return true;
 }
 
-// async: device pointers on `stream`, not synchronised; otherwise host or device pointers, synchronised.
 template <typename T>
 int rfft_exec(void* plan, bool forward, const void* in, void* out, size_t batch, int code, bool async, void* stream) {
   if (!plan || !in || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
   auto* p = static_cast<RealPlan<T>*>(plan);
-  try {
-    if (cudaError_t e = p->check_code(forward, code)) return (int)e;
-    if (batch == 0) return (int)p->exec_device(forward, in, out, 0, code, nullptr);
-    if (!disjoint(in, batch * p->row_bytes(forward, true), out, batch * p->row_bytes(forward, false)))
-      return (int)cudaErrorInvalidValue;
-    if (!async) {
-      const int dev = residence({in, out});
-      if (dev < 0) return (int)cudaErrorInvalidValue;
-      if (!dev) return (int)p->exec_host(forward, in, out, batch, code);
-    }
-    if (!device_pointers_aligned(in, out)) return (int)cudaErrorMisalignedAddress;
-    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
-    cudaError_t e = p->exec_device(forward, in, out, batch, code, s);
-    if (e != cudaSuccess || async) return (int)e;
-    return (int)cudaStreamSynchronize(s);
-  } catch (...) {
-    fb200::set_last_error("real transform threw");
-    return (int)cudaErrorUnknown;
-  }
+  return run_call(
+      "real transform", async, stream,
+      [&] {
+        if (cudaError_t e = p->check_code(forward, code)) return (int)e;
+        if (batch == 0) return (int)p->exec_device(forward, in, out, 0, code, nullptr);
+        if (!disjoint(in, batch * p->row_bytes(forward, true), out, batch * p->row_bytes(forward, false)))
+          return (int)cudaErrorInvalidValue;
+        return kRun;
+      },
+      {in, out}, "input and output must both be host or both be device memory",
+      [&] { return p->exec_host(forward, in, out, batch, code); },
+      {in, out}, [&](cudaStream_t s) { return p->exec_device(forward, in, out, batch, code, s); });
 }
 
 // Convolution of real rows: in == out allowed, otherwise in, out and spectrum as for rfft_exec.
@@ -182,33 +193,24 @@ int convolve_exec(void* plan, const T* in, const void* spectrum, size_t rows, T*
   auto* p = static_cast<RealPlan<T>*>(plan);
   using C = typename RealPlan<T>::C;
   const C* spec = static_cast<const C*>(spectrum);
-  try {
-    if (batch == 0) return (int)p->convolve_device(in, spec, rows, out, 0, nullptr);
-    const size_t bytes = batch * p->size() * sizeof(T);
-    if (in != out && ranges_meet(in, bytes, out, bytes)) {
-      fb200::set_last_error("input and output overlap (they must be the same buffer or disjoint)");
-      return (int)cudaErrorInvalidValue;
-    }
-    if (ranges_meet(spectrum, p->spec_bytes(rows), out, bytes)) {
-      fb200::set_last_error("spectrum and output overlap");
-      return (int)cudaErrorInvalidValue;
-    }
-    if (!async) {
-      const int dev =
-          residence({in, spectrum, out}, "input, spectrum and output must all be host or all be device memory");
-      if (dev < 0) return (int)cudaErrorInvalidValue;
-      if (!dev) return (int)p->convolve_host(in, spec, rows, out, batch);
-    }
-    if (!device_pointers_aligned(in, out) || !device_pointers_aligned(spectrum, spectrum))
-      return (int)cudaErrorMisalignedAddress;
-    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
-    cudaError_t e = p->convolve_device(in, spec, rows, out, batch, s);
-    if (e != cudaSuccess || async) return (int)e;
-    return (int)cudaStreamSynchronize(s);
-  } catch (...) {
-    fb200::set_last_error("convolution threw");
-    return (int)cudaErrorUnknown;
-  }
+  return run_call(
+      "convolution", async, stream,
+      [&] {
+        if (batch == 0) return (int)p->convolve_device(in, spec, rows, out, 0, nullptr);
+        const size_t bytes = batch * p->size() * sizeof(T);
+        if (in != out && ranges_meet(in, bytes, out, bytes)) {
+          fb200::set_last_error("input and output overlap (they must be the same buffer or disjoint)");
+          return (int)cudaErrorInvalidValue;
+        }
+        if (ranges_meet(spectrum, p->spec_bytes(rows), out, bytes)) {
+          fb200::set_last_error("spectrum and output overlap");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {in, spectrum, out}, "input, spectrum and output must all be host or all be device memory",
+      [&] { return p->convolve_host(in, spec, rows, out, batch); },
+      {in, out, spectrum}, [&](cudaStream_t s) { return p->convolve_device(in, spec, rows, out, batch, s); });
 }
 
 // Linear convolution of real rows by overlap-save: out of place only; scalar arguments are checked before the plan is
@@ -228,34 +230,45 @@ int linear_exec(void* plan, const T* in, size_t in_len, const void* spectrum, si
   using C = typename RealPlan<T>::C;
   const C* spec = static_cast<const C*>(spectrum);
   if (taps > p->size()) { fb200::set_last_error("taps must not exceed the plan length N"); return (int)cudaErrorInvalidValue; }
-  try {
-    if (batch == 0) return (int)p->linear_convolve_device(in, in_len, spec, rows, taps, mode, out, 0, nullptr);
-    const size_t in_bytes = batch * in_len * sizeof(T);
-    const size_t out_bytes = batch * (size_t)fb200::real::linear_out_len(mode, (long)in_len, (long)taps) * sizeof(T);
-    if (ranges_meet(in, in_bytes, out, out_bytes)) {
-      fb200::set_last_error("input and output overlap (linear convolution is out of place only)");
-      return (int)cudaErrorInvalidValue;
-    }
-    if (ranges_meet(spectrum, p->spec_bytes(rows), out, out_bytes)) {
-      fb200::set_last_error("spectrum and output overlap");
-      return (int)cudaErrorInvalidValue;
-    }
-    if (!async) {
-      const int dev =
-          residence({in, spectrum, out}, "input, spectrum and output must all be host or all be device memory");
-      if (dev < 0) return (int)cudaErrorInvalidValue;
-      if (!dev) return (int)p->linear_convolve_host(in, in_len, spec, rows, taps, mode, out, batch);
-    }
-    if (!device_pointers_aligned(in, out) || !device_pointers_aligned(spectrum, spectrum))
-      return (int)cudaErrorMisalignedAddress;
-    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
-    cudaError_t e = p->linear_convolve_device(in, in_len, spec, rows, taps, mode, out, batch, s);
-    if (e != cudaSuccess || async) return (int)e;
-    return (int)cudaStreamSynchronize(s);
-  } catch (...) {
-    fb200::set_last_error("linear convolution threw");
-    return (int)cudaErrorUnknown;
+  return run_call(
+      "linear convolution", async, stream,
+      [&] {
+        if (batch == 0) return (int)p->linear_convolve_device(in, in_len, spec, rows, taps, mode, out, 0, nullptr);
+        const size_t in_bytes = batch * in_len * sizeof(T);
+        const size_t out_bytes =
+            batch * (size_t)fb200::real::linear_out_len(mode, (long)in_len, (long)taps) * sizeof(T);
+        if (ranges_meet(in, in_bytes, out, out_bytes)) {
+          fb200::set_last_error("input and output overlap (linear convolution is out of place only)");
+          return (int)cudaErrorInvalidValue;
+        }
+        if (ranges_meet(spectrum, p->spec_bytes(rows), out, out_bytes)) {
+          fb200::set_last_error("spectrum and output overlap");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {in, spectrum, out}, "input, spectrum and output must all be host or all be device memory",
+      [&] { return p->linear_convolve_host(in, in_len, spec, rows, taps, mode, out, batch); },
+      {in, out, spectrum},
+      [&](cudaStream_t s) { return p->linear_convolve_device(in, in_len, spec, rows, taps, mode, out, batch, s); });
+}
+
+// The framing checks of stft_exec and mel_exec, in this order: hop, boundary and in_len; then `bad`, the caller's
+// refusal of its other scalar arguments (nullptr: none); then in_len against N, the only check that reads the plan.
+template <typename T>
+bool check_frames(const RealPlan<T>* p, size_t in_len, size_t hop, int boundary, const char* bad) {
+  const char* why = hop == 0                          ? "hop must be at least 1"
+                    : boundary < 0 || boundary > 2    ? "unknown boundary (FOURIER_B200_STFT_NONE, _ZEROS or _REFLECT)"
+                    : in_len == 0                     ? "in_len must be at least 1"
+                                                      : bad;
+  if (!why) {
+    const size_t n = p->size();
+    why = boundary == fb200::real::kStftNone && in_len < n             ? "boundary none needs in_len >= N"
+          : boundary == fb200::real::kStftReflect && in_len <= n / 2   ? "boundary reflect needs in_len > N/2"
+                                                                       : nullptr;
   }
+  if (why) fb200::set_last_error(why);
+  return !why;
 }
 
 // Short-time Fourier transform of real rows: out of place only; the arguments are checked before the plan is touched,
@@ -264,45 +277,23 @@ template <typename T>
 int stft_exec(void* plan, const T* in, size_t in_len, const T* window, size_t hop, int boundary, void* out, size_t batch,
               bool async, void* stream) {
   if (!plan || !in || !window || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
-  const char* bad = hop == 0                          ? "hop must be at least 1"
-                    : boundary < 0 || boundary > 2    ? "unknown boundary (FOURIER_B200_STFT_NONE, _ZEROS or _REFLECT)"
-                    : in_len == 0                     ? "in_len must be at least 1"
-                                                      : nullptr;
-  if (bad) { fb200::set_last_error(bad); return (int)cudaErrorInvalidValue; }
   auto* p = static_cast<RealPlan<T>*>(plan);
   using C = typename RealPlan<T>::C;
-  const size_t n = p->size();
-  if (boundary == fb200::real::kStftNone && in_len < n) {
-    fb200::set_last_error("boundary none needs in_len >= N");
-    return (int)cudaErrorInvalidValue;
-  }
-  if (boundary == fb200::real::kStftReflect && in_len <= n / 2) {
-    fb200::set_last_error("boundary reflect needs in_len > N/2");
-    return (int)cudaErrorInvalidValue;
-  }
-  try {
-    if (batch == 0) return (int)p->stft_device(in, in_len, window, hop, boundary, (C*)out, 0, nullptr);
-    const size_t frames = (size_t)fb200::real::frame_map((long)n, (long)in_len, (long)hop, boundary).frames;
-    const size_t in_bytes = batch * in_len * sizeof(T), out_bytes = batch * frames * (n / 2 + 1) * sizeof(C);
-    if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, n * sizeof(T), out, out_bytes)) {
-      fb200::set_last_error("input or window and output overlap (the stft is out of place only)");
-      return (int)cudaErrorInvalidValue;
-    }
-    if (!async) {
-      const int dev =
-          residence({in, window, out}, "input, window and output must all be host or all be device memory");
-      if (dev < 0) return (int)cudaErrorInvalidValue;
-      if (!dev) return (int)p->stft_host(in, in_len, window, hop, boundary, (C*)out, batch);
-    }
-    if (!device_pointers_aligned(in, out)) return (int)cudaErrorMisalignedAddress;
-    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
-    cudaError_t e = p->stft_device(in, in_len, window, hop, boundary, (C*)out, batch, s);
-    if (e != cudaSuccess || async) return (int)e;
-    return (int)cudaStreamSynchronize(s);
-  } catch (...) {
-    fb200::set_last_error("stft threw");
-    return (int)cudaErrorUnknown;
-  }
+  if (!check_frames(p, in_len, hop, boundary, nullptr)) return (int)cudaErrorInvalidValue;
+  return run_call(
+      "stft", async, stream,
+      [&] {
+        if (batch == 0) return (int)p->stft_device(in, in_len, window, hop, boundary, (C*)out, 0, nullptr);
+        const size_t in_bytes = batch * in_len * sizeof(T), out_bytes = batch * p->stft_row_bytes(in_len, hop, boundary);
+        if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, p->size() * sizeof(T), out, out_bytes)) {
+          fb200::set_last_error("input or window and output overlap (the stft is out of place only)");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {in, window, out}, "input, window and output must all be host or all be device memory",
+      [&] { return p->stft_host(in, in_len, window, hop, boundary, (C*)out, batch); },
+      {in, out}, [&](cudaStream_t s) { return p->stft_device(in, in_len, window, hop, boundary, (C*)out, batch, s); });
 }
 
 // Mel spectrogram of real rows: stft_exec's rules, plus power and n_mels checked before the plan is touched and the
@@ -314,48 +305,34 @@ int mel_exec(void* plan, const T* in, size_t in_len, const T* window, size_t hop
     fb200::set_last_error("null argument");
     return (int)cudaErrorInvalidValue;
   }
-  const char* bad = hop == 0                          ? "hop must be at least 1"
-                    : boundary < 0 || boundary > 2    ? "unknown boundary (FOURIER_B200_STFT_NONE, _ZEROS or _REFLECT)"
-                    : in_len == 0                     ? "in_len must be at least 1"
-                    : power != 1 && power != 2        ? "power must be 1 or 2"
-                    : n_mels == 0                     ? "n_mels must be at least 1"
-                                                      : nullptr;
-  if (bad) { fb200::set_last_error(bad); return (int)cudaErrorInvalidValue; }
   auto* p = static_cast<RealPlan<T>*>(plan);
+  if (!check_frames(p, in_len, hop, boundary,
+                    power != 1 && power != 2 ? "power must be 1 or 2"
+                    : n_mels == 0            ? "n_mels must be at least 1"
+                                             : nullptr))
+    return (int)cudaErrorInvalidValue;
   const size_t n = p->size();
-  if (boundary == fb200::real::kStftNone && in_len < n) {
-    fb200::set_last_error("boundary none needs in_len >= N");
-    return (int)cudaErrorInvalidValue;
-  }
-  if (boundary == fb200::real::kStftReflect && in_len <= n / 2) {
-    fb200::set_last_error("boundary reflect needs in_len > N/2");
-    return (int)cudaErrorInvalidValue;
-  }
-  try {
-    if (batch == 0)
-      return (int)p->mel_device(in, in_len, window, hop, boundary, filters, n_mels, power, out, 0, nullptr);
-    const size_t frames = (size_t)fb200::real::frame_map((long)n, (long)in_len, (long)hop, boundary).frames;
-    const size_t in_bytes = batch * in_len * sizeof(T), out_bytes = batch * frames * n_mels * sizeof(T);
-    if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, n * sizeof(T), out, out_bytes) ||
-        ranges_meet(filters, n_mels * (n / 2 + 1) * sizeof(T), out, out_bytes)) {
-      fb200::set_last_error("input, window or filters and output overlap (the mel spectrogram is out of place only)");
-      return (int)cudaErrorInvalidValue;
-    }
-    if (!async) {
-      const int dev = residence({in, window, filters, out},
-                                "input, window, filters and output must all be host or all be device memory");
-      if (dev < 0) return (int)cudaErrorInvalidValue;
-      if (!dev) return (int)p->mel_host(in, in_len, window, hop, boundary, filters, n_mels, power, out, batch);
-    }
-    if (!device_pointers_aligned(in, out)) return (int)cudaErrorMisalignedAddress;
-    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
-    cudaError_t e = p->mel_device(in, in_len, window, hop, boundary, filters, n_mels, power, out, batch, s);
-    if (e != cudaSuccess || async) return (int)e;
-    return (int)cudaStreamSynchronize(s);
-  } catch (...) {
-    fb200::set_last_error("mel spectrogram threw");
-    return (int)cudaErrorUnknown;
-  }
+  return run_call(
+      "mel spectrogram", async, stream,
+      [&] {
+        if (batch == 0)
+          return (int)p->mel_device(in, in_len, window, hop, boundary, filters, n_mels, power, out, 0, nullptr);
+        const size_t in_bytes = batch * in_len * sizeof(T);
+        const size_t out_bytes = batch * p->mel_row_bytes(in_len, hop, boundary, n_mels);
+        if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, n * sizeof(T), out, out_bytes) ||
+            ranges_meet(filters, n_mels * (n / 2 + 1) * sizeof(T), out, out_bytes)) {
+          fb200::set_last_error(
+              "input, window or filters and output overlap (the mel spectrogram is out of place only)");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {in, window, filters, out}, "input, window, filters and output must all be host or all be device memory",
+      [&] { return p->mel_host(in, in_len, window, hop, boundary, filters, n_mels, power, out, batch); },
+      {in, out},
+      [&](cudaStream_t s) {
+        return p->mel_device(in, in_len, window, hop, boundary, filters, n_mels, power, out, batch, s);
+      });
 }
 
 template <typename T>
@@ -370,29 +347,21 @@ int istft_exec(void* plan, const void* in, size_t frames, const T* window, size_
   auto* p = static_cast<RealPlan<T>*>(plan);
   using C = typename RealPlan<T>::C;
   const C* spec = static_cast<const C*>(in);
-  try {
-    if (batch == 0) return (int)p->istft_device(spec, frames, window, hop, center != 0, out, out_len, 0, nullptr);
-    const size_t n = p->size();
-    const size_t in_bytes = batch * frames * (n / 2 + 1) * sizeof(C), out_bytes = batch * out_len * sizeof(T);
-    if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, n * sizeof(T), out, out_bytes)) {
-      fb200::set_last_error("input or window and output overlap (the istft is out of place only)");
-      return (int)cudaErrorInvalidValue;
-    }
-    if (!async) {
-      const int dev =
-          residence({in, window, out}, "input, window and output must all be host or all be device memory");
-      if (dev < 0) return (int)cudaErrorInvalidValue;
-      if (!dev) return (int)p->istft_host(spec, frames, window, hop, center != 0, out, out_len, batch);
-    }
-    if (!device_pointers_aligned(in, out)) return (int)cudaErrorMisalignedAddress;
-    cudaStream_t s = async ? (cudaStream_t)stream : cudaStreamPerThread;
-    cudaError_t e = p->istft_device(spec, frames, window, hop, center != 0, out, out_len, batch, s);
-    if (e != cudaSuccess || async) return (int)e;
-    return (int)cudaStreamSynchronize(s);
-  } catch (...) {
-    fb200::set_last_error("istft threw");
-    return (int)cudaErrorUnknown;
-  }
+  return run_call(
+      "istft", async, stream,
+      [&] {
+        if (batch == 0) return (int)p->istft_device(spec, frames, window, hop, center != 0, out, out_len, 0, nullptr);
+        const size_t in_bytes = batch * p->spec_bytes(frames), out_bytes = batch * out_len * sizeof(T);
+        if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, p->size() * sizeof(T), out, out_bytes)) {
+          fb200::set_last_error("input or window and output overlap (the istft is out of place only)");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {in, window, out}, "input, window and output must all be host or all be device memory",
+      [&] { return p->istft_host(spec, frames, window, hop, center != 0, out, out_len, batch); },
+      {in, out},
+      [&](cudaStream_t s) { return p->istft_device(spec, frames, window, hop, center != 0, out, out_len, batch, s); });
 }
 
 }  // namespace

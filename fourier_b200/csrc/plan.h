@@ -351,7 +351,6 @@ class RealPlan {
   }
   // Host pointers: the spectra are staged once, the rows in chunks as in exec_host; returns when `out` is done.
   cudaError_t convolve_host(const T* in, const C* spec, size_t rows, T* out, size_t batch);
-  size_t spec_bytes(size_t rows) const { return rows * (n_ / 2 + 1) * sizeof(C); }
 
   // Linear convolution by overlap-save (DESIGN.md §4.12): `batch` rows of in_len reals -> rows of
   // real::linear_out_len(mode, in_len, taps) reals, out[b][i] = y_full[off + i], y_full = row b (*) c, where
@@ -398,11 +397,24 @@ class RealPlan {
     const size_t real = n_ * sizeof(T), spec = (n_ / 2 + 1) * sizeof(C);
     return forward == input ? real : spec;
   }
+  // bytes of `rows` spectra of N/2+1 bins: a convolution's spectra, or one istft input row of `rows` frames
+  size_t spec_bytes(size_t rows) const { return rows * (n_ / 2 + 1) * sizeof(C); }
+  // bytes of one stft output row (a spectrum per frame) and of one mel output row (n_mels reals per frame)
+  size_t stft_row_bytes(size_t in_len, size_t hop, int boundary) const {
+    return spec_bytes(frame_count(in_len, hop, boundary));
+  }
+  size_t mel_row_bytes(size_t in_len, size_t hop, int boundary, size_t n_mels) const {
+    return frame_count(in_len, hop, boundary) * n_mels * sizeof(T);
+  }
 
  private:
   template <class P> friend P* create_plan(size_t, int, bool);
   RealPlan() = default;
   cudaError_t init(size_t n, int device, bool allow_fast_paths);
+  // frames of one stft / mel row
+  size_t frame_count(size_t in_len, size_t hop, int boundary) const {
+    return (size_t)real::frame_map((long)n_, (long)in_len, (long)hop, boundary).frames;
+  }
   // convolve_device with row b using spectrum row ((row0 + b) / per) mod rows; adds its kernels to launches_
   cudaError_t convolve_rows(const T* in, const C* spec, size_t rows, size_t row0, size_t per, T* out, size_t batch,
                             cudaStream_t s);
@@ -416,10 +428,17 @@ class RealPlan {
   // launches_
   cudaError_t mel_frames(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
                          size_t n_mels, int power, T* out, size_t batch, cudaStream_t s);
-  // The host-pointer loop of exec_host and convolve_host (real.cu): chunks of rows of in_row / out_row bytes go H2D,
-  // through step(dev_in, dev_out, first_row, rows) on host_stream_, and D2H; launches() then counts all chunks.
+  // The host-pointer loop (real.cu): chunks of rows of in_row / out_row bytes go H2D, through
+  // step(dev_in, dev_out, first_row, rows) on host_stream_, and D2H; launches() then counts all chunks.
   template <class Step>
   cudaError_t stage_rows(const void* in, void* out, size_t batch, size_t in_row, size_t out_row, Step step);
+  // A host-pointer call's constant operands, a and optionally b, go H2D into stage_spec_ on host_stream_, each at a
+  // 256-byte-aligned offset; *da and *db are their device copies.  The caller holds the DeviceGuard.
+  template <class A, class B = A>
+  cudaError_t stage_consts(const A* a, size_t a_bytes, const A** da, const B* b = nullptr, size_t b_bytes = 0,
+                           const B** db = nullptr);
+  // creates host_stream_ on the first host-pointer call
+  cudaError_t open_host_stream();
 
   size_t n_ = 0, m_ = 0;        // m_ = N/2 (even N)
   int device_ = 0;
@@ -431,11 +450,9 @@ class RealPlan {
   DeviceBuffer tab_, twa_;           // w_N^k, k <= N/4 (even N); stage twiddles of the fused kernel
   DeviceBuffer work_;                // one chunk of inner-plan rows
   DeviceBuffer stage_in_, stage_out_;
-  DeviceBuffer stage_spec_;          // the spectra of convolve_host and linear_convolve_host, the window of stft_host
-                                     // and istft_host, the window and filters of mel_host
-  DeviceBuffer seg_;                 // one chunk of N-real segments of a linear convolution (real_half, real_full), of
-                                     // windowed frames (stft) or of inverted frames (istft); of windowed frames and
-                                     // their spectra (mel, real_half and real_full)
+  DeviceBuffer stage_spec_;          // the constant operands of a host-pointer call: spectra, window, filters
+  DeviceBuffer seg_;                 // one chunk of N-real segments or frames (for the mel spectrogram, the frames'
+                                     // spectra behind them)
   DeviceBuffer bands_;               // the filter bands of the last mel call (real::Band per filter row)
   cudaStream_t host_stream_ = nullptr;
   std::string kernel_desc_;

@@ -175,6 +175,11 @@ real_part_kernel(const cpx<T>* __restrict__ y, T* __restrict__ out, size_t count
     out[g] = y[g].x;
 }
 
+// Items of item_bytes that one chunk of plan scratch holds: as many as fit kScratchTargetBytes, at least 1, at most total.
+size_t scratch_chunk(size_t total, size_t item_bytes) {
+  return std::min(total, std::max<size_t>(1, kScratchTargetBytes / item_bytes));
+}
+
 }  // namespace
 
 template <typename T>
@@ -259,7 +264,7 @@ cudaError_t RealPlan<T>::exec_device(bool forward, const void* in, void* out, si
     return cudaSuccess;
   }
   const size_t len = inner_->size(), bins = n_ / 2 + 1;
-  const size_t chunk = std::min(batch, std::max<size_t>(1, kScratchTargetBytes / (len * sizeof(C))));
+  const size_t chunk = scratch_chunk(batch, len * sizeof(C));
   FB_CHECK(work_.reserve(chunk * len * sizeof(C)));
   C* work = (C*)work_.data();
   for (size_t b0 = 0; b0 < batch; b0 += chunk) {
@@ -302,13 +307,19 @@ cudaError_t RealPlan<T>::exec_device(bool forward, const void* in, void* out, si
   return cudaSuccess;
 }
 
+template <typename T>
+cudaError_t RealPlan<T>::open_host_stream() {
+  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
+  return cudaSuccess;
+}
+
 // Host pointers: chunks of rows go H2D into stage_in_, through `step` into stage_out_, and D2H, one chunk at a time on
 // the plan's own stream (no pipelining: the results are those of the device path, bit for bit).  The caller holds the
 // DeviceGuard.
 template <typename T>
 template <class Step>
 cudaError_t RealPlan<T>::stage_rows(const void* in, void* out, size_t batch, size_t in_row, size_t out_row, Step step) {
-  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
+  FB_CHECK(open_host_stream());
   const size_t rows = std::min(batch, std::max<size_t>(1, kHostChunkBytes / std::max(in_row, out_row)));
   FB_CHECK(stage_in_.reserve(rows * in_row));
   FB_CHECK(stage_out_.reserve(rows * out_row));
@@ -325,6 +336,23 @@ cudaError_t RealPlan<T>::stage_rows(const void* in, void* out, size_t batch, siz
     FB_CHECK(cudaStreamSynchronize(host_stream_));
   }
   launches_ = total;
+  return cudaSuccess;
+}
+
+template <typename T>
+template <class A, class B>
+cudaError_t RealPlan<T>::stage_consts(const A* a, size_t a_bytes, const A** da, const B* b, size_t b_bytes,
+                                      const B** db) {
+  FB_CHECK(open_host_stream());
+  const size_t b_off = (a_bytes + 255) / 256 * 256;
+  FB_CHECK(stage_spec_.reserve(b ? b_off + b_bytes : a_bytes));
+  char* base = (char*)stage_spec_.data();
+  FB_CHECK(cudaMemcpyAsync(base, a, a_bytes, cudaMemcpyHostToDevice, host_stream_));
+  *da = (const A*)base;
+  if (b) {
+    FB_CHECK(cudaMemcpyAsync(base + b_off, b, b_bytes, cudaMemcpyHostToDevice, host_stream_));
+    *db = (const B*)(base + b_off);
+  }
   return cudaSuccess;
 }
 
@@ -365,7 +393,7 @@ cudaError_t RealPlan<T>::convolve_rows(const T* in, const C* spec, size_t rows, 
     launches_ += inner_->launches();
     return cudaSuccess;
   }
-  const size_t chunk = std::min(batch, std::max<size_t>(1, kScratchTargetBytes / (n_ * sizeof(C))));
+  const size_t chunk = scratch_chunk(batch, n_ * sizeof(C));
   FB_CHECK(work_.reserve(chunk * n_ * sizeof(C)));
   C* work = (C*)work_.data();
   for (size_t b0 = 0; b0 < batch; b0 += chunk) {
@@ -394,13 +422,11 @@ cudaError_t RealPlan<T>::convolve_host(const T* in, const C* spec, size_t rows, 
   launches_ = 0;
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
-  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
-  FB_CHECK(stage_spec_.reserve(spec_bytes(rows)));
-  FB_CHECK(cudaMemcpyAsync(stage_spec_.data(), spec, spec_bytes(rows), cudaMemcpyHostToDevice, host_stream_));
+  const C* dspec;
+  FB_CHECK(stage_consts(spec, spec_bytes(rows), &dspec));
   return stage_rows(in, out, batch, n_ * sizeof(T), n_ * sizeof(T),
                     [&](const void* din, void* dout, size_t b0, size_t nb) {
-                      return convolve_rows((const T*)din, (const C*)stage_spec_.data(), rows, b0, 1, (T*)dout, nb,
-                                           host_stream_);
+                      return convolve_rows((const T*)din, dspec, rows, b0, 1, (T*)dout, nb, host_stream_);
                     });
 }
 
@@ -416,7 +442,7 @@ cudaError_t RealPlan<T>::linear_segments(const T* in, T* out, const real::SegMap
   }
   // chunks of segments through seg_: gather, the circular convolution in place (segment q of the chunk uses spectrum
   // row ((g0 + q) / per) mod rows), scatter
-  const size_t chunk = std::min(nseg, std::max<size_t>(1, kScratchTargetBytes / (n_ * sizeof(T))));
+  const size_t chunk = scratch_chunk(nseg, n_ * sizeof(T));
   FB_CHECK(seg_.reserve(chunk * n_ * sizeof(T)));
   T* seg = (T*)seg_.data();
   for (size_t q0 = 0; q0 < nseg; q0 += chunk) {
@@ -450,10 +476,8 @@ cudaError_t RealPlan<T>::linear_convolve_host(const T* in, size_t in_len, const 
   launches_ = 0;
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
-  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
-  FB_CHECK(stage_spec_.reserve(spec_bytes(rows)));
-  FB_CHECK(cudaMemcpyAsync(stage_spec_.data(), spec, spec_bytes(rows), cudaMemcpyHostToDevice, host_stream_));
-  const C* dspec = (const C*)stage_spec_.data();
+  const C* dspec;
+  FB_CHECK(stage_consts(spec, spec_bytes(rows), &dspec));
   const real::SegMap m = real::linear_map((long)n_, (long)taps, mode, (long)in_len);
   const size_t out_len = (size_t)m.out_len;
   if (std::max(in_len, out_len) * sizeof(T) <= kHostChunkBytes) {
@@ -512,7 +536,7 @@ cudaError_t RealPlan<T>::stft_device(const T* in, size_t in_len, const T* win, s
     return cudaSuccess;
   }
   // chunks of frames through seg_: gather the windowed frames, then the plan's own rfft straight into the output rows
-  const size_t chunk = std::min(total, std::max<size_t>(1, kScratchTargetBytes / (n_ * sizeof(T))));
+  const size_t chunk = scratch_chunk(total, n_ * sizeof(T));
   FB_CHECK(seg_.reserve(chunk * n_ * sizeof(T)));
   T* seg = (T*)seg_.data();
   unsigned long long count = 0;
@@ -543,9 +567,9 @@ cudaError_t RealPlan<T>::istft_device(const C* in, size_t frames, const T* win, 
   m.frames = (long)frames;
   m.rcp = 1.0 / (double)frames;
   const size_t bins = n_ / 2 + 1;
-  const size_t cap = real::istft_scratch_frames(std::max<size_t>(1, kScratchTargetBytes / (n_ * sizeof(T))), n_, hop,
-                                                frames);
-  FB_CHECK(seg_.reserve(std::min(cap, batch * frames) * n_ * sizeof(T)));
+  // cap <= batch * frames: istft_scratch_frames raises the chunk to at most `frames`
+  const size_t cap = real::istft_scratch_frames(scratch_chunk(batch * frames, n_ * sizeof(T)), n_, hop, frames);
+  FB_CHECK(seg_.reserve(cap * n_ * sizeof(T)));
   T* seg = (T*)seg_.data();
   unsigned long long count = 0;
   const int e = real::istft_runs(n_, hop, (size_t)m.pad, frames, out_len, batch, cap,
@@ -563,21 +587,17 @@ cudaError_t RealPlan<T>::istft_device(const C* in, size_t frames, const T* win, 
   return cudaSuccess;
 }
 
-// Host pointers, on the plan's own stream: the window is staged once into stage_spec_, whole rows through stage_rows.
 template <typename T>
 cudaError_t RealPlan<T>::stft_host(const T* in, size_t in_len, const T* win, size_t hop, int boundary, C* out,
                                    size_t batch) {
   launches_ = 0;
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
-  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
-  FB_CHECK(stage_spec_.reserve(n_ * sizeof(T)));
-  FB_CHECK(cudaMemcpyAsync(stage_spec_.data(), win, n_ * sizeof(T), cudaMemcpyHostToDevice, host_stream_));
-  const size_t frames = (size_t)real::frame_map((long)n_, (long)in_len, (long)hop, boundary).frames;
-  return stage_rows(in, out, batch, in_len * sizeof(T), frames * (n_ / 2 + 1) * sizeof(C),
+  const T* dwin;
+  FB_CHECK(stage_consts(win, n_ * sizeof(T), &dwin));
+  return stage_rows(in, out, batch, in_len * sizeof(T), stft_row_bytes(in_len, hop, boundary),
                     [&](const void* din, void* dout, size_t, size_t nb) {
-                      return stft_device((const T*)din, in_len, (const T*)stage_spec_.data(), hop, boundary, (C*)dout,
-                                         nb, host_stream_);
+                      return stft_device((const T*)din, in_len, dwin, hop, boundary, (C*)dout, nb, host_stream_);
                     });
 }
 
@@ -587,13 +607,12 @@ cudaError_t RealPlan<T>::istft_host(const C* in, size_t frames, const T* win, si
   launches_ = 0;
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
-  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
-  FB_CHECK(stage_spec_.reserve(n_ * sizeof(T)));
-  FB_CHECK(cudaMemcpyAsync(stage_spec_.data(), win, n_ * sizeof(T), cudaMemcpyHostToDevice, host_stream_));
-  return stage_rows(in, out, batch, frames * (n_ / 2 + 1) * sizeof(C), out_len * sizeof(T),
+  const T* dwin;
+  FB_CHECK(stage_consts(win, n_ * sizeof(T), &dwin));
+  return stage_rows(in, out, batch, spec_bytes(frames), out_len * sizeof(T),
                     [&](const void* din, void* dout, size_t, size_t nb) {
-                      return istft_device((const C*)din, frames, (const T*)stage_spec_.data(), hop, center, (T*)dout,
-                                          out_len, nb, host_stream_);
+                      return istft_device((const C*)din, frames, dwin, hop, center, (T*)dout, out_len, nb,
+                                          host_stream_);
                     });
 }
 
@@ -622,7 +641,7 @@ cudaError_t RealPlan<T>::mel_frames(const T* in, size_t in_len, const T* win, si
   }
   // chunks of frames through seg_: the windowed frames, then their spectra from the plan's own rfft behind them, then
   // the mels of those spectra straight into the output rows
-  const size_t chunk = std::min(total, std::max<size_t>(1, kScratchTargetBytes / (n_ * sizeof(T) + bins * sizeof(C))));
+  const size_t chunk = scratch_chunk(total, n_ * sizeof(T) + bins * sizeof(C));
   const size_t spec_off = (chunk * n_ * sizeof(T) + 255) / 256 * 256;
   FB_CHECK(seg_.reserve(spec_off + chunk * bins * sizeof(C)));
   T* seg = (T*)seg_.data();
@@ -656,25 +675,16 @@ cudaError_t RealPlan<T>::mel_device(const T* in, size_t in_len, const T* win, si
   return cudaSuccess;
 }
 
-// Host pointers, on the plan's own stream: the window and the filters are staged once into stage_spec_ and their bands
-// computed once; whole rows go through stage_rows.
 template <typename T>
 cudaError_t RealPlan<T>::mel_host(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
                                   size_t n_mels, int power, T* out, size_t batch) {
   launches_ = 0;
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
-  if (!host_stream_) FB_CHECK(cudaStreamCreateWithFlags(&host_stream_, cudaStreamNonBlocking));
-  const size_t filt_off = (n_ * sizeof(T) + 255) / 256 * 256, filt_bytes = n_mels * (n_ / 2 + 1) * sizeof(T);
-  FB_CHECK(stage_spec_.reserve(filt_off + filt_bytes));
-  const T* dwin = (const T*)stage_spec_.data();
-  const T* dfilt = (const T*)((const char*)stage_spec_.data() + filt_off);
-  FB_CHECK(cudaMemcpyAsync(stage_spec_.data(), win, n_ * sizeof(T), cudaMemcpyHostToDevice, host_stream_));
-  FB_CHECK(cudaMemcpyAsync((char*)stage_spec_.data() + filt_off, filters, filt_bytes, cudaMemcpyHostToDevice,
-                           host_stream_));
+  const T *dwin, *dfilt;
+  FB_CHECK(stage_consts(win, n_ * sizeof(T), &dwin, filters, n_mels * (n_ / 2 + 1) * sizeof(T), &dfilt));
   FB_CHECK(mel_bands(dfilt, n_mels, host_stream_));
-  const size_t frames = (size_t)real::frame_map((long)n_, (long)in_len, (long)hop, boundary).frames;
-  FB_CHECK(stage_rows(in, out, batch, in_len * sizeof(T), frames * n_mels * sizeof(T),
+  FB_CHECK(stage_rows(in, out, batch, in_len * sizeof(T), mel_row_bytes(in_len, hop, boundary, n_mels),
                       [&](const void* din, void* dout, size_t, size_t nb) {
                         return mel_frames((const T*)din, in_len, dwin, hop, boundary, dfilt, n_mels, power, (T*)dout,
                                           nb, host_stream_);
