@@ -24,6 +24,8 @@ reference's operator interface name for name:
     (no counterpart)                                      RealFft.mel_spectrogram: |stft|^p through a caller's
                                                             mel filter bank (torchaudio's MelSpectrogram,
                                                             frames frame-major), the spectrum kept on chip
+    (no counterpart)                                      RealFft.welch: Welch's power spectral density of real
+                                                            rows (scipy.signal.welch), frames summed on chip
 
 Buffers are numpy arrays (host memory: staged over PCIe by the library) or torch CUDA tensors
 (device memory: transformed in HBM on torch's current stream).  A leading batch dimension is
@@ -456,6 +458,37 @@ class RealFft:
             return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
         self._call("mel_spectrogram", "mel spectrogram", di, si, pi, in_len, pw, hop, boundary, int(power), pf, n_mels,
                    po, batch)
+
+    WELCH_SCALINGS = {"density": 0, "spectrum": 1}
+    WELCH_DETRENDS = {False: 0, "constant": 1}
+
+    def welch(self, input, window, hop, output, fs=1.0, scaling="density", detrend="constant"):
+        """Welch's power spectral density of every row of `input` (shape (..., L), L >= N): the F = stft_frames(L, hop,
+        center=False) frames of N = size() samples every `hop`, each with its mean taken off (detrend "constant"; False
+        keeps it) and then times `window` (N reals), averaged as |rfft|**2, one-sided and scaled to a density
+        (1 / (fs * sum(window**2))) or a spectrum (1 / sum(window)**2).  `output` has shape (..., N//2+1) in the real
+        dtype: this is scipy.signal.welch(x, fs, window=window, nperseg=N, noverlap=N-hop, detrend=detrend,
+        scaling=scaling)[1], at the frequencies numpy.fft.rfftfreq(N, 1/fs).  The frames stay on chip where the plan's
+        path allows.  Out of place only."""
+        self._check_resolved(input, window, output)
+        if not isinstance(scaling, str) or scaling not in self.WELCH_SCALINGS:
+            raise ValueError(f"scaling must be 'density' or 'spectrum', got {scaling!r}")
+        if not (detrend is False or (isinstance(detrend, str) and detrend == "constant")):
+            raise ValueError(f"detrend must be 'constant' or False, got {detrend!r}")
+        fs = float(fs)
+        if not (np.isfinite(fs) and fs > 0):
+            raise ValueError(f"fs must be finite and positive, got {fs!r}")
+        hop, _, in_len, _, (pi, li, di, si), (pw, dw) = self._framing(input, window, hop, False, "reflect")
+        po, lo, do_, _ = self._describe(output, "real", last=self._size // 2 + 1)
+        if li != lo:
+            raise ValueError(f"input and output leading shapes differ: {li} and {lo}")
+        if not (di == dw == do_):
+            raise ValueError("input, window and output must all be host or all be device buffers")
+        batch = int(np.prod(li, dtype=np.int64))
+        if batch == 0:
+            return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
+        self._call("welch", "welch", di, si, pi, in_len, pw, hop, self.WELCH_DETRENDS[detrend],
+                   self.WELCH_SCALINGS[scaling], fs, po, batch)
 
     def istft(self, input, window, hop, output, center=True):
         """Inverse of stft: `input` (shape (..., F, N//2+1), stft's frame-major layout) -> `output` (shape

@@ -9,6 +9,7 @@
 #include "../../include/fourier_b200.h"
 #pragma GCC visibility pop
 
+#include <cmath>
 #include <cstdint>
 #include <initializer_list>
 #include <new>
@@ -333,6 +334,37 @@ int mel_exec(void* plan, const T* in, size_t in_len, const T* window, size_t hop
       [&](cudaStream_t s) {
         return p->mel_device(in, in_len, window, hop, boundary, filters, n_mels, power, out, batch, s);
       });
+}
+
+// Welch power spectral density of real rows: stft_exec's rules with boundary none, plus detrend, scaling and fs checked
+// before the plan is touched.
+template <typename T>
+int welch_exec(void* plan, const T* in, size_t in_len, const T* window, size_t hop, int detrend, int scaling, double fs,
+               T* out, size_t batch, bool async, void* stream) {
+  if (!plan || !in || !window || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  if (!check_frames(p, in_len, hop, fb200::real::kStftNone,
+                    detrend != 0 && detrend != 1    ? "unknown detrend (FOURIER_B200_DETREND_NONE or _CONSTANT)"
+                    : scaling != 0 && scaling != 1  ? "unknown scaling (FOURIER_B200_WELCH_DENSITY or _SPECTRUM)"
+                    : !(std::isfinite(fs) && fs > 0) ? "fs must be finite and positive"
+                                                     : nullptr))
+    return (int)cudaErrorInvalidValue;
+  const size_t n = p->size();
+  return run_call(
+      "welch", async, stream,
+      [&] {
+        if (batch == 0) return (int)p->welch_device(in, in_len, window, hop, detrend, scaling, fs, out, 0, nullptr);
+        const size_t in_bytes = batch * in_len * sizeof(T), out_bytes = batch * (n / 2 + 1) * sizeof(T);
+        if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, n * sizeof(T), out, out_bytes)) {
+          fb200::set_last_error("input or window and output overlap (welch is out of place only)");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {in, window, out}, "input, window and output must all be host or all be device memory",
+      [&] { return p->welch_host(in, in_len, window, hop, detrend, scaling, fs, out, batch); },
+      {in, out},
+      [&](cudaStream_t s) { return p->welch_device(in, in_len, window, hop, detrend, scaling, fs, out, batch, s); });
 }
 
 template <typename T>
@@ -684,6 +716,25 @@ int fourier_b200_mel_spectrogram_async_double(fourier_b200_rfft_double* plan, co
                                               void* stream) {
   return mel_exec<double>(plan, in_dev, in_len, window_dev, hop, boundary, power, filters_dev, n_mels, out_dev, batch,
                           true, stream);
+}
+
+int fourier_b200_welch_float(fourier_b200_rfft_float* plan, const float* in, size_t in_len, const float* window,
+                             size_t hop, int detrend, int scaling, double fs, float* out, size_t batch) {
+  return welch_exec<float>(plan, in, in_len, window, hop, detrend, scaling, fs, out, batch, false, nullptr);
+}
+int fourier_b200_welch_double(fourier_b200_rfft_double* plan, const double* in, size_t in_len, const double* window,
+                              size_t hop, int detrend, int scaling, double fs, double* out, size_t batch) {
+  return welch_exec<double>(plan, in, in_len, window, hop, detrend, scaling, fs, out, batch, false, nullptr);
+}
+int fourier_b200_welch_async_float(fourier_b200_rfft_float* plan, const float* in_dev, size_t in_len,
+                                   const float* window_dev, size_t hop, int detrend, int scaling, double fs,
+                                   float* out_dev, size_t batch, void* stream) {
+  return welch_exec<float>(plan, in_dev, in_len, window_dev, hop, detrend, scaling, fs, out_dev, batch, true, stream);
+}
+int fourier_b200_welch_async_double(fourier_b200_rfft_double* plan, const double* in_dev, size_t in_len,
+                                    const double* window_dev, size_t hop, int detrend, int scaling, double fs,
+                                    double* out_dev, size_t batch, void* stream) {
+  return welch_exec<double>(plan, in_dev, in_len, window_dev, hop, detrend, scaling, fs, out_dev, batch, true, stream);
 }
 
 const char* fourier_b200_last_error(void) { return fb200::last_error(); }

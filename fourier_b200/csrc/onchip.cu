@@ -35,6 +35,11 @@ struct OnChipImpl {
   template <bool FWD> using Cfg = typename K::template Cfg<FWD>;
   using BCfg = typename K::BCfg;
   static constexpr size_t smem_fft = Cfg<true>::EX_BYTES + Cfg<true>::TWA_BYTES;
+  static constexpr size_t smem_welch = smem_fft + onchip::WelchBody<Cfg<true>>::ACC_BYTES;
+  // The Welch kernel's CTAs per SM: the class's, or fewer where its accumulators leave shared memory for fewer (228 KB
+  // per H100 SM, 1 KB of it reserved per CTA).  That is f32 L = 128 only: 3 instead of 4, which also lifts its register
+  // cap from 64 to 80, at which it does not spill.
+  static constexpr int MINB_WELCH = std::min<int>(MINB, (int)((228u << 10) / (smem_welch + 1024)));
   static constexpr size_t smem_blue() {
     return BCfg::EX_BYTES + BCfg::TWA_BYTES +
            sizeof(cpx<T>) * (4 * (size_t)BCfg::L + (K::LOCAL_STASH ? 0 : (size_t)K::E * BCfg::THREADS));
@@ -92,7 +97,28 @@ struct OnChipImpl {
     if ((e = allow_smem(onchip::onchip_conv_kernel<Cfg<true>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_lconv_kernel<Cfg<true>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_stft_kernel<Cfg<true>, MINB>))) return e;
-    return allow_smem(onchip::onchip_mel_kernel<Cfg<true>, MINB>);
+    if ((e = allow_smem(onchip::onchip_mel_kernel<Cfg<true>, MINB>))) return e;
+    return cudaFuncSetAttribute(onchip::onchip_welch_kernel<Cfg<true>, MINB_WELCH>,
+                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_welch);
+  }
+  // the items of w, groups grid-stride over at most sms * MINB_WELCH * 4 CTAs, as launch() does
+  static cudaError_t welch(const T* in, const T* win, const T* base, int detrend, T* part, T* out,
+                           const real::FrameMap& m, const real::WelchItems& w, const void* twa, const cpx<T>* tab, int sms,
+                           cudaStream_t s) {
+    typename onchip::WelchBody<Cfg<true>>::Args a;
+    static_cast<typename onchip::RealBody<Cfg<true>>::Args&>(a) = {
+        nullptr, nullptr, (const TwPair<T>*)twa, tab, 0, (T)0.5};
+    a.x = in;
+    a.win = win;
+    a.m = m;
+    a.part = part;
+    a.psd = out;
+    a.base = base;
+    a.w = w;
+    a.detrend = detrend;
+    const unsigned grid = (unsigned)std::min<size_t>((size_t)w.groups, (size_t)sms * MINB_WELCH * 4);
+    onchip::onchip_welch_kernel<Cfg<true>, MINB_WELCH><<<grid, Cfg<true>::THREADS, smem_welch, s>>>(a);
+    return cudaGetLastError();
   }
   static cudaError_t mel(const T* in, const T* win, const T* filters, const real::Band* bands, size_t n_mels, int power,
                          T* out, const real::FrameMap& m, size_t nframes, const void* twa, const cpx<T>* tab, int sms,
@@ -146,7 +172,7 @@ struct OnChipImpl {
                   {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab, (long)batch, h}, batch, sms, s);
   }
   static const OnChipOps<T>* ops() {
-    static const RealOnChipOps<T> r = {RA, RB, &real_prepare, &real, &conv, &lconv, &stft, &mel};
+    static const RealOnChipOps<T> r = {RA, RB, Cfg<true>::C, &real_prepare, &real, &conv, &lconv, &stft, &mel, &welch};
     static const OnChipOps<T> o = {RA, RB, &prepare, &fft, kHasBluestein ? &bluestein : nullptr, &r};
     return &o;
   }

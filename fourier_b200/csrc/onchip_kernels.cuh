@@ -11,6 +11,8 @@
 //   * onchip_mel_kernel:      the stft's frames to mel energies: power and filter bank on chip.
 //     (these six run the phases of FftBody / RealBody / ConvBody / LinConvBody / StftBody / MelBody through
 //     run_onchip_groups, tilefft.cuh)
+//   * onchip_welch_kernel:    detrended, windowed frames to Welch's averaged power spectrum, summed on chip
+//                             (WelchBody through run_welch_groups, below).
 //   * bluestein_fused_kernel: the whole chirp-z transform of the reference (bluesteins.rs:218-259) for
 //                             N <= L, M = 2L, in one kernel and without touching HBM in between.
 //
@@ -466,6 +468,167 @@ template <class Cfg> struct MelBody {
 template <class Cfg, int MINB>
 __global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_mel_kernel(const typename MelBody<Cfg>::Args a) {
   run_onchip_groups<Cfg, MelBody<Cfg>>(a);
+}
+
+// ---- fused Welch power spectral density of real rows, N = 2L (real::WelchItems, DESIGN.md §4.15) -----------------
+// Groups are the items of real::WelchItems, run in rounds of C frames, frame f of an item in column f mod C.  Per frame:
+//   * load (phase 0): the TP lanes of an FFT read the frame's N raw samples as StftBody's load does (a frame always lies
+//     inside its row, L >= N), park them and put each lane's sum of its own samples, in ascending p, in `sums`;
+//   * detrend (phase 1): each lane forms the frame mean from the TP lane sums in lane order (0 with detrend none) and
+//     rewrites its own parked samples as (x - mu) w[p], so the mean is taken off before the window;
+//   * phases 2-5: StftBody's stage A, scatter, gather + stage B and park;
+//   * accumulate (phase 6): each lane forms |X[k]|^2 and |X[L-k]|^2 of the pairs it owns (real::power_pair, lane u = 0
+//     also k = L/2) and adds them to its column's row of L+1 accumulators in shared memory (stores them in round 0).
+// After the last round a CTA barrier, then the flush: thread o of the CTA sums bin k of an item over the item's columns
+// in ascending order and writes the item's partial, or, when a row is one item, the row's output through welch_out.
+// The lane sums go through shared memory rather than warp shuffles so that the CPU emulator runs these phases as they
+// are.  Shared memory behind the exchange and the stage twiddles: C rows of L+1 accumulators, then one lane sum per
+// thread.
+template <class Cfg> struct WelchBody {
+  using Stft = StftBody<Cfg>;
+  using Real = RealBody<Cfg>;
+  using Tile = typename Cfg::Tile;   // FWD = true
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  static constexpr int L = Cfg::L, TP = Tile::TP, E = Tile::E, C = Cfg::C, THREADS = Cfg::THREADS, BINS = L + 1;
+  static constexpr size_t ACC_BYTES = sizeof(T) * ((size_t)C * BINS + THREADS);
+  // Stft::Args with out = nullptr (m: the frames of the launch's rows, rows in_ld apart from x); part: a partial of
+  // BINS reals per item of the launch, psd: BINS reals per row, base: s / F (welch_base) in device memory
+  struct Args : Stft::Args { T* part; T* psd; const T* base; real::WelchItems w; int detrend; };
+
+  // The empty asm makes a 64-bit value (the group, the round, a pointer) opaque where a phase uses it, so that what the
+  // phase derives from it (the item, row and frame of real::WelchItems::slot, addresses) is not hoisted out of the round
+  // loop and kept live through the FFT phases: that spilled 16-84 bytes at the register caps.
+  template <typename U> static FB_HD void opaque(U& v) {
+    static_assert(sizeof(U) == 8, "64-bit values only");
+#ifdef __CUDA_ARCH__
+    asm volatile("" : "+l"(v));
+#endif
+    (void)v;
+  }
+  static FB_HD bool slot(const Args& a, long g, long r, int t, long& i, long& b, long& f) {
+    opaque(g);
+    return a.w.slot(g, Tile::template col_of<true>(t), r, i, b, f);
+  }
+
+  static FB_HD void load(const Args& a, long g, long r, int t, V* smem, T* acc) {
+    const int u = Tile::template u_of<true>(t);
+    long i, b, f;
+    slot(a, g, r, t, i, b, f);
+    const long fg = b * a.w.frames + f;
+    const T* src = a.x + b * a.m.in_ld + f * a.m.hop;
+    T* z = reinterpret_cast<T*>(smem + Real::park(t));
+    opaque(z);
+    T s = 0;
+#pragma unroll 2
+    for (int p = u; p < 2 * L; p += TP) {
+      const T x = real::lin_ld(src + p, fg);
+      z[p] = x;
+      s += x;
+    }
+    acc[C * BINS + t] = s;
+  }
+  static FB_HD void detrend(const Args& a, int t, V* smem, const T* acc) {
+    const int u = Tile::template u_of<true>(t), col = Tile::template col_of<true>(t);
+    T mu = 0;
+    if (a.detrend == real::kDetrendConstant) {
+      const T* sums = acc + C * BINS + col * TP;
+      T s = 0;
+      for (int v = 0; v < TP; ++v) s += sums[v];
+      mu = s / (T)(2 * L);
+    }
+    T* z = reinterpret_cast<T*>(smem + Real::park(t));
+    const T* win = a.win;
+    opaque(z);
+    opaque(win);
+#pragma unroll 2
+    for (int p = u; p < 2 * L; p += TP) z[p] = (z[p] - mu) * win[p];
+  }
+  static FB_HD void accumulate(const Args& a, long g, long r, int t, const V* smem, T* acc) {
+    const int u = Tile::template u_of<true>(t), col = Tile::template col_of<true>(t);
+    long i, b, f;
+    if (!slot(a, g, r, t, i, b, f)) return;
+    const V* z = smem + Real::park(t);
+    const V* tab = a.tab;
+    T* y = acc + col * BINS;
+    opaque(z);
+    opaque(tab);
+    opaque(y);
+#pragma unroll 4
+    for (int j = 0; j < E / 2; ++j) {
+      const int k = u + TP * j;
+      const V p = real::power_pair(z, L, k, tab, a.h, 2);
+      y[k] = r == 0 ? p.x : y[k] + p.x;
+      y[L - k] = r == 0 ? p.y : y[L - k] + p.y;
+    }
+    if (u == 0) {
+      const V p = real::power_pair(z, L, L / 2, tab, a.h, 2);
+      y[L / 2] = r == 0 ? p.x : y[L / 2] + p.x;
+    }
+  }
+  // the item sums of group g, after a CTA barrier; thread t takes outputs t, t + THREADS, ...
+  static FB_HD void flush(const Args& a, long g, int t, const T* acc) {
+    const int outs = (int)a.w.per_group * BINS;
+    for (int o = t; o < outs; o += THREADS) {
+      const int q = o / BINS, k = o - q * BINS;
+      const long i = g * a.w.per_group + q;
+      if (i >= a.w.total()) return;
+      const long cnt = a.w.count(i), used = cnt < C ? cnt : C;
+      const T* y = acc + q * a.w.block * BINS + k;
+      T s = 0;
+      for (long c = 0; c < used; ++c) s += y[c * BINS];
+      if (a.w.items == 1) real::lin_st(a.psd + i * BINS + k, real::welch_out(s, *a.base, 2L * L, (long)k), i);
+      else real::lin_st(a.part + i * BINS + k, s, i);
+    }
+  }
+
+  // phase protocol of run_welch_groups: load, detrend, StftBody's stage A, scatter, gather + stage B, park; accumulate
+  static constexpr int kPhases = 7;
+  template <int P>
+  static FB_HD void phase(Tile& f, const Args& a, long g, long r, int t, V* smem, T* acc, const TwPair<T>* twa) {
+    if constexpr (P == 0) load(a, g, r, t, smem, acc);
+    else if constexpr (P == 1) detrend(a, t, smem, acc);
+    else if constexpr (P <= 5) Stft::template phase<P - 1>(f, a, 0, t, smem, twa);
+    else accumulate(a, g, r, t, smem, acc);
+  }
+};
+
+// The device driver of WelchBody: run_onchip_groups' set-up, then per group its rounds, each phase followed by
+// __syncwarp, and the flush between two CTA barriers (the accumulators of every column are complete before it, and it
+// has read them before the next group's round 0 stores).  tools/emulate_common.h has the CPU driver.
+template <class Cfg, class Body> __device__ __forceinline__ void run_welch_groups(const typename Body::Args& a) {
+  using Tile = typename Cfg::Tile;
+  using T = typename Body::T;
+  extern __shared__ __align__(128) unsigned char onchip_smem[];
+  typename Tile::V* exch = reinterpret_cast<typename Tile::V*>(onchip_smem);
+  TwPair<T>* twa = reinterpret_cast<TwPair<T>*>(onchip_smem + Cfg::EX_BYTES);
+  T* acc = reinterpret_cast<T*>(onchip_smem + Cfg::EX_BYTES + Cfg::TWA_BYTES);
+  for (int i = threadIdx.x; i < (Tile::RA / 2) * Tile::RB; i += Cfg::THREADS) twa[i] = a.twa[i];
+  __syncthreads();
+  Tile f;
+  // One loop over (group, round), carrying only g and r: whatever a phase derives from g is formed again where it is
+  // used (g is opaque at the top of every iteration), so the FFT phases have the registers the stft kernel has.
+  long g = blockIdx.x;
+  int r = 0;
+  while (g < a.w.groups) {
+    Body::opaque(g);
+    static_for<0, Body::kPhases>([&](auto P) FB_LAMBDA {
+      Body::template phase<decltype(P)::value>(f, a, g, r, threadIdx.x, exch, acc, twa);
+      __syncwarp();
+    });
+    if (++r == a.w.rounds(g)) {
+      __syncthreads();
+      Body::flush(a, g, threadIdx.x, acc);
+      __syncthreads();
+      g += gridDim.x;
+      r = 0;
+    }
+  }
+}
+
+template <class Cfg, int MINB>
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_welch_kernel(const typename WelchBody<Cfg>::Args a) {
+  run_welch_groups<Cfg, WelchBody<Cfg>>(a);
 }
 
 // ---- fused Bluestein -------------------------------------------------------------------------------------------

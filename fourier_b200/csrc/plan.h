@@ -301,6 +301,7 @@ class Plan {
 // §4.13) into consecutive spectrum rows from `out` on.
 template <typename T> struct RealOnChipOps {
   int ra, rb;
+  int cols;   // FFTs per CTA (the C of real::welch_items)
   cudaError_t (*prepare)();
   cudaError_t (*run)(const void* in, void* out, const void* twa, const cpx<T>* tab, size_t batch, bool fwd, T h,
                      int sms, cudaStream_t);
@@ -314,6 +315,10 @@ template <typename T> struct RealOnChipOps {
   cudaError_t (*mel)(const T* in, const T* win, const T* filters, const real::Band* bands, size_t n_mels, int power,
                      T* out, const real::FrameMap& m, size_t nframes, const void* twa, const cpx<T>* tab, int sms,
                      cudaStream_t);
+  // welch(): the Welch items w (DESIGN.md §4.15) of the rows of m, from `in` on: each item's partial into part, or, when
+  // a row is one item, the row's output into out; base = s / F in device memory, detrend real::kDetrend*
+  cudaError_t (*welch)(const T* in, const T* win, const T* base, int detrend, T* part, T* out, const real::FrameMap& m,
+                       const real::WelchItems& w, const void* twa, const cpx<T>* tab, int sms, cudaStream_t);
 };
 template <typename T> const RealOnChipOps<T>* real_onchip_lookup(size_t l);
 
@@ -386,6 +391,16 @@ class RealPlan {
   cudaError_t mel_host(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
                        size_t n_mels, int power, T* out, size_t batch);
 
+  // Welch power spectral density (DESIGN.md §4.15): `batch` rows of in_len >= N reals -> N/2+1 reals each, out[b][k] =
+  // c_k s / F sum_f |rfft(win . (frame f - its mean))[k]|^2 over the F frames of hop `hop` (no padding), the mean only
+  // with detrend real::kDetrendConstant, s from scaling real::kWelch* and fs.  Arguments checked by the caller.  Out of
+  // place only.  Device pointers, on `stream`, never synchronised: the window sums are formed on the device.
+  cudaError_t welch_device(const T* in, size_t in_len, const T* win, size_t hop, int detrend, int scaling, double fs,
+                           T* out, size_t batch, cudaStream_t stream);
+  // Host pointers: the window is staged once, whole rows through stage_rows; the same bits.
+  cudaError_t welch_host(const T* in, size_t in_len, const T* win, size_t hop, int detrend, int scaling, double fs,
+                         T* out, size_t batch);
+
   unsigned long long launches() const { return launches_; }
   const char* kernel_name() const { return kernel_desc_.c_str(); }
 
@@ -428,6 +443,12 @@ class RealPlan {
   // launches_
   cudaError_t mel_frames(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
                          size_t n_mels, int power, T* out, size_t batch, cudaStream_t s);
+  // s / F of a Welch call from the window into welch_base_ (one launch, added to launches_)
+  cudaError_t welch_scale(const T* win, int scaling, double fs, size_t frames, cudaStream_t s);
+  // welch_device after welch_scale: chunks of rows whose partials fit part_, each through the fused kernel or chunks of
+  // frames through seg_, then the finish; adds its kernels to launches_
+  cudaError_t welch_rows(const T* in, size_t in_len, const T* win, size_t hop, int detrend, T* out, size_t batch,
+                         cudaStream_t s);
   // The host-pointer loop (real.cu): chunks of rows of in_row / out_row bytes go H2D, through
   // step(dev_in, dev_out, first_row, rows) on host_stream_, and D2H; launches() then counts all chunks.
   template <class Step>
@@ -454,6 +475,8 @@ class RealPlan {
   DeviceBuffer seg_;                 // one chunk of N-real segments or frames (for the mel spectrogram, the frames'
                                      // spectra behind them)
   DeviceBuffer bands_;               // the filter bands of the last mel call (real::Band per filter row)
+  DeviceBuffer welch_base_;          // s / F of the last Welch call (one T)
+  DeviceBuffer part_;                // one chunk of rows of Welch partials (N/2+1 reals per item)
   cudaStream_t host_stream_ = nullptr;
   std::string kernel_desc_;
 };

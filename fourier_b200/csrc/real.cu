@@ -16,6 +16,9 @@
 // Mel spectrogram (DESIGN.md §4.14): mel_bands_kernel, then onchip_mel_kernel on the fused path; otherwise chunks of
 // windowed frames gathered into seg_, their spectra by the plan's own rfft into seg_ behind them, and
 // mel_spectra_kernel from there into the output rows.
+// Welch power spectral density (DESIGN.md §4.15): welch_scale_kernel, then per chunk of rows onchip_welch_kernel on the
+// fused path, or chunks of detrended windowed frames gathered into seg_, their spectra by the plan's own rfft behind
+// them and welch_accumulate_kernel into the partials; then welch_finish_kernel unless the fused kernel wrote the rows.
 #include <algorithm>
 #include <string>
 #include <vector>
@@ -165,6 +168,78 @@ mel_spectra_kernel(const cpx<T>* __restrict__ spec, const T* __restrict__ filter
   for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
     const long q = g / n_mels;
     real::mel_spectrum_one(spec, filters, bands, bins, n_mels, power, out, q, g - q * n_mels, g0 + q);
+  }
+}
+
+// Welch (real::WelchItems).  scale: one CTA, the window sums in double, each thread over every kThreads-th sample in
+// ascending order, then a tree in shared memory.  gather: one CTA per frame q of the chunk (frame g0 + q of the rows'
+// FrameMap), the frame mean by the same two steps in T, then (x - mu) w into seg.  accumulate: one thread per (item, bin)
+// of the items that have frames in the chunk.  finish: one thread per (row, bin).
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+welch_scale_kernel(const T* __restrict__ win, long n, int scaling, double fs, long frames, T* __restrict__ base) {
+  __shared__ double s1[kThreads], s2[kThreads];
+  double a = 0, b = 0;
+  for (long p = threadIdx.x; p < n; p += kThreads) {
+    const double w = win[p];
+    a += w;
+    b += w * w;
+  }
+  s1[threadIdx.x] = a;
+  s2[threadIdx.x] = b;
+  __syncthreads();
+  for (int w = kThreads / 2; w > 0; w /= 2) {
+    if ((int)threadIdx.x < w) {
+      s1[threadIdx.x] += s1[threadIdx.x + w];
+      s2[threadIdx.x] += s2[threadIdx.x + w];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *base = (T)real::welch_base(s1[0], s2[0], scaling, fs, frames);
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+welch_gather_kernel(const T* __restrict__ in, const T* __restrict__ win, T* __restrict__ seg, const real::FrameMap m,
+                    long nframes, int detrend) {
+  __shared__ T part[kThreads];
+  for (long q = blockIdx.x; q < nframes; q += gridDim.x) {
+    const long g = m.g0 + q, b = m.row_of(g);
+    const T* src = in + (b - m.r0) * m.in_ld + m.start(g, b);
+    T mu = 0;
+    if (detrend == real::kDetrendConstant) {
+      T s = 0;
+      for (long p = threadIdx.x; p < m.n; p += kThreads) s += src[p];
+      part[threadIdx.x] = s;
+      __syncthreads();
+      for (int w = kThreads / 2; w > 0; w /= 2) {
+        if ((int)threadIdx.x < w) part[threadIdx.x] += part[threadIdx.x + w];
+        __syncthreads();
+      }
+      mu = part[0] / (T)m.n;
+      __syncthreads();
+    }
+    for (long p = threadIdx.x; p < m.n; p += kThreads) seg[q * m.n + p] = (src[p] - mu) * win[p];
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+welch_accumulate_kernel(const cpx<T>* __restrict__ spec, const real::WelchItems w, long bins, long q0, long nq, long i0,
+                        long ni, T* __restrict__ part) {
+  const long total = ni * bins;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long i = i0 + g / bins, k = g - (g / bins) * bins, b = i / w.items;
+    real::welch_accumulate_one(spec, bins, q0, nq, b * w.frames + (i - b * w.items) * w.block, w.count(i), part, i, k);
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+welch_finish_kernel(const T* __restrict__ part, long items, long n, const T* __restrict__ base, T* __restrict__ out,
+                    long rows) {
+  const long bins = n / 2 + 1, total = rows * bins;
+  const T s = *base;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / bins;
+    real::welch_finish_one(part, items, n, s, out, b, g - b * bins);
   }
 }
 
@@ -688,6 +763,100 @@ cudaError_t RealPlan<T>::mel_host(const T* in, size_t in_len, const T* win, size
                       [&](const void* din, void* dout, size_t, size_t nb) {
                         return mel_frames((const T*)din, in_len, dwin, hop, boundary, dfilt, n_mels, power, (T*)dout,
                                           nb, host_stream_);
+                      }));
+  launches_ += 1;
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::welch_scale(const T* win, int scaling, double fs, size_t frames, cudaStream_t s) {
+  FB_CHECK(welch_base_.reserve(sizeof(T)));
+  welch_scale_kernel<T><<<1, kThreads, 0, s>>>(win, (long)n_, scaling, fs, (long)frames, (T*)welch_base_.data());
+  FB_CHECK(cudaGetLastError());
+  launches_ += 1;
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::welch_rows(const T* in, size_t in_len, const T* win, size_t hop, int detrend, T* out,
+                                    size_t batch, cudaStream_t s) {
+  const real::FrameMap m = real::frame_map((long)n_, (long)in_len, (long)hop, real::kStftNone);
+  const size_t bins = n_ / 2 + 1, frames = (size_t)m.frames;
+  const bool fused = path_ == Path::kRealFused;
+  const long cols = fused ? fused_->cols : 1;
+  const size_t items = (size_t)real::welch_items(m.frames, cols, 1).items;
+  // the fused kernel writes a row of one item itself; every other row goes through partials and the finish
+  const bool direct = fused && items == 1;
+  const size_t rows = direct ? batch : scratch_chunk(batch, items * bins * sizeof(T));
+  if (!direct) FB_CHECK(part_.reserve(rows * items * bins * sizeof(T)));
+  T* part = (T*)part_.data();
+  const T* base = (const T*)welch_base_.data();
+  unsigned long long count = launches_;
+  for (size_t r0 = 0; r0 < batch; r0 += rows) {
+    const size_t nr = std::min(rows, batch - r0);
+    const real::WelchItems w = real::welch_items(m.frames, cols, (long)nr);
+    const T* x = in + r0 * in_len;
+    T* y = out + r0 * bins;
+    if (fused) {
+      FB_CHECK(fused_->welch(x, win, base, detrend, part, y, m, w, twa_.data(), (const C*)tab_.data(), sm_count_, s));
+      count += 1;
+    } else {
+      // chunks of frames through seg_: the detrended windowed frames, their spectra from the plan's own rfft behind
+      // them, and the items with frames in the chunk accumulated from there
+      const size_t total = nr * frames;
+      const size_t chunk = scratch_chunk(total, n_ * sizeof(T) + bins * sizeof(C));
+      const size_t spec_off = (chunk * n_ * sizeof(T) + 255) / 256 * 256;
+      FB_CHECK(seg_.reserve(spec_off + chunk * bins * sizeof(C)));
+      T* seg = (T*)seg_.data();
+      C* spec = (C*)((char*)seg_.data() + spec_off);
+      for (size_t q0 = 0; q0 < total; q0 += chunk) {
+        const size_t nq = std::min(chunk, total - q0);
+        real::FrameMap mc = m;
+        mc.g0 = (long)q0;
+        welch_gather_kernel<T><<<(unsigned)std::min<size_t>(nq, 132u * 32u), kThreads, 0, s>>>(x, win, seg, mc, (long)nq,
+                                                                                             detrend);
+        FB_CHECK(cudaGetLastError());
+        FB_CHECK(exec_device(true, seg, spec, nq, kFft, s));
+        count += 2 + launches_;
+        auto item_of = [&](size_t q) { return (q / frames) * items + (q % frames) / (size_t)w.block; };
+        const size_t i0 = item_of(q0), ni = item_of(q0 + nq - 1) + 1 - i0;
+        welch_accumulate_kernel<T><<<grid_for(ni * bins), kThreads, 0, s>>>(spec, w, (long)bins, (long)q0, (long)nq,
+                                                                            (long)i0, (long)ni, part);
+        FB_CHECK(cudaGetLastError());
+      }
+    }
+    if (!direct) {
+      welch_finish_kernel<T><<<grid_for(nr * bins), kThreads, 0, s>>>(part, (long)items, (long)n_, base, y, (long)nr);
+      FB_CHECK(cudaGetLastError());
+      count += 1;
+    }
+  }
+  launches_ = count;
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::welch_device(const T* in, size_t in_len, const T* win, size_t hop, int detrend, int scaling,
+                                      double fs, T* out, size_t batch, cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  FB_CHECK(welch_scale(win, scaling, fs, frame_count(in_len, hop, real::kStftNone), s));
+  return welch_rows(in, in_len, win, hop, detrend, out, batch, s);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::welch_host(const T* in, size_t in_len, const T* win, size_t hop, int detrend, int scaling,
+                                    double fs, T* out, size_t batch) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  const T* dwin;
+  FB_CHECK(stage_consts(win, n_ * sizeof(T), &dwin));
+  FB_CHECK(welch_scale(dwin, scaling, fs, frame_count(in_len, hop, real::kStftNone), host_stream_));
+  FB_CHECK(stage_rows(in, out, batch, in_len * sizeof(T), (n_ / 2 + 1) * sizeof(T),
+                      [&](const void* din, void* dout, size_t, size_t nb) {
+                        return welch_rows((const T*)din, in_len, dwin, hop, detrend, (T*)dout, nb, host_stream_);
                       }));
   launches_ += 1;
   return cudaSuccess;

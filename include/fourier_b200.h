@@ -339,6 +339,46 @@ int fourier_b200_mel_spectrogram_async_double(struct fourier_b200_rfft_double *p
                                               int power, const double *filters_dev, size_t n_mels, double *out_dev,
                                               size_t batch, void *cuda_stream);
 
+/* ---- Welch power spectral density of real rows ----
+ * On a real plan of length N, for `batch` rows of in_len >= N reals (row b at element b*in_len), a window of N reals
+ * and hop >= 1: the F = 1 + (in_len - N) / hop frames x_bf[p] = in[b*in_len + f*hop + p], p < N (no padding, F =
+ * the stft's frame count with FOURIER_B200_STFT_NONE), and
+ *   out[b][k] = c_k * s / F * sum_{f < F} |X_bf[k]|^2,   X_bf = rfft(w * (x_bf - mu_bf)),   k <= N/2,
+ * where mu_bf is the frame's mean (FOURIER_B200_DETREND_CONSTANT, taken off before the window) or 0 (_NONE),
+ * s = 1 / (fs * sum w^2) (FOURIER_B200_WELCH_DENSITY) or 1 / (sum w)^2 (_SPECTRUM), and c_k = 2 for 0 < k < N/2 (N even)
+ * or 0 < k <= (N-1)/2 (N odd), else 1.  With nperseg = N and noverlap = N - hop this is
+ * scipy.signal.welch(x, fs, window=w, nperseg=N, noverlap=N-hop, detrend="constant" | False,
+ * scaling="density" | "spectrum")[1].  out holds N/2+1 reals per row.  A window with sum w^2 = 0 gives the IEEE
+ * result (inf / NaN), as scipy does.
+ * Frames are summed in items of consecutive frames whose size depends only on F and the plan, so a row's bits depend
+ * only on the row, the window, hop, detrend, scaling, fs and the plan: not on the batch, the other rows, host or device
+ * memory or the stream.  The window sums are formed on the device on every call.  Launches: at most 3 on the real_fused
+ * path while the rows' partials fit one scratch chunk (512 MB); on the others 2, plus per scratch chunk of frames 2 and
+ * those of the plan's rfft of that many rows.
+ * Refused with cudaErrorInvalidValue and a message: a NULL argument, hop == 0, in_len == 0, detrend other than 0 and 1,
+ * scaling other than 0 and 1, fs not finite and > 0 (these also when batch == 0, which otherwise succeeds and launches
+ * nothing), in_len < N, the input or window overlapping the output (out of place only), and a mix of host and device
+ * buffers in the synchronous calls.  Device base pointers of input and output must be 16-byte aligned
+ * (cudaErrorMisalignedAddress).  Host memory is staged through the plan's buffers (the window once, whole rows in
+ * chunks) and gives the same bits as device memory.  The _async calls take device memory, are enqueued on
+ * `cuda_stream` and never synchronise the host. */
+#define FOURIER_B200_DETREND_NONE 0
+#define FOURIER_B200_DETREND_CONSTANT 1
+#define FOURIER_B200_WELCH_DENSITY 0
+#define FOURIER_B200_WELCH_SPECTRUM 1
+int fourier_b200_welch_float(struct fourier_b200_rfft_float *plan, const float *in, size_t in_len,
+                             const float *window, size_t hop, int detrend, int scaling, double fs, float *out,
+                             size_t batch);
+int fourier_b200_welch_double(struct fourier_b200_rfft_double *plan, const double *in, size_t in_len,
+                              const double *window, size_t hop, int detrend, int scaling, double fs, double *out,
+                              size_t batch);
+int fourier_b200_welch_async_float(struct fourier_b200_rfft_float *plan, const float *in_dev, size_t in_len,
+                                   const float *window_dev, size_t hop, int detrend, int scaling, double fs,
+                                   float *out_dev, size_t batch, void *cuda_stream);
+int fourier_b200_welch_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev, size_t in_len,
+                                    const double *window_dev, size_t hop, int detrend, int scaling, double fs,
+                                    double *out_dev, size_t batch, void *cuda_stream);
+
 const char *fourier_b200_last_error(void);
 const char *fourier_b200_version(void);
 

@@ -42,6 +42,25 @@ static void run_body(const typename Body::Args& a, long groups, const TwPair<typ
     });
 }
 
+// The CPU driver of run_welch_groups (onchip_kernels.cuh): per group of a.w its rounds, each phase for every thread
+// before the next, then the flush for every thread, which is the CTA barrier on both sides.  acc: the accumulators
+// and lane sums the device keeps behind the exchange buffer and the stage twiddles.
+template <class Body, class Tile, class LAY>
+static void run_welch_body(const typename Body::Args& a, const TwPair<typename Body::T>* twa) {
+  using T = typename Body::T;
+  std::vector<typename Tile::V> smem(Tile::template smem_elems<LAY>());
+  std::vector<T> acc(Body::ACC_BYTES / sizeof(T));
+  std::vector<Tile> thr(Tile::THREADS);
+  for (long g = 0; g < a.w.groups; ++g) {
+    for (long r = 0; r < a.w.rounds(g); ++r)
+      static_for<0, Body::kPhases>([&](auto P) {
+        for (int t = 0; t < Tile::THREADS; ++t)
+          Body::template phase<decltype(P)::value>(thr[t], a, g, r, t, smem.data(), acc.data(), twa);
+      });
+    for (int t = 0; t < Tile::THREADS; ++t) Body::flush(a, g, t, acc.data());
+  }
+}
+
 // every on-chip size class of precision T (onchip_configs.cuh), smallest first: f(class)
 template <typename T, class F> static void for_each_onchip(F&& f) {
   for (size_t l = 1; l <= ((size_t)1 << 16); l *= 2) onchip::visit_onchip<T>(l, f);
