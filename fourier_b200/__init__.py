@@ -26,6 +26,9 @@ reference's operator interface name for name:
                                                             frames frame-major), the spectrum kept on chip
     (no counterpart)                                      RealFft.welch: Welch's power spectral density of real
                                                             rows (scipy.signal.welch), frames summed on chip
+    (no counterpart)                                      RealFft.dct / idct: discrete cosine transforms of real
+                                                            rows, types 2 and 3 (scipy.fft.dct / idct; torch has
+                                                            none)
 
 Buffers are numpy arrays (host memory: staged over PCIe by the library) or torch CUDA tensors
 (device memory: transformed in HBM on torch's current stream).  A leading batch dimension is
@@ -458,6 +461,38 @@ class RealFft:
             return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
         self._call("mel_spectrogram", "mel spectrogram", di, si, pi, in_len, pw, hop, boundary, int(power), pf, n_mels,
                    po, batch)
+
+    DCT_NORMS = {"backward": 0, "ortho": 1, "forward": 2}
+
+    def dct(self, input, output, type=2, norm="backward"):
+        """output = scipy.fft.dct(input, type=type, norm=norm) along the last axis: the discrete cosine transform of
+        type 2 or 3 of every row of `input` (shape (..., N), real dtype), with scipy's norms "backward", "ortho" and
+        "forward" (orthogonalize=True).  `output` has the input's shape and may be `input` itself."""
+        self._check_resolved(input, output)
+        if type not in (2, 3) or isinstance(type, bool):
+            raise ValueError(f"type must be 2 or 3, got {type!r}")
+        if not isinstance(norm, str) or norm not in self.DCT_NORMS:
+            raise ValueError(f"norm must be one of {sorted(self.DCT_NORMS)}, got {norm!r}")
+        pi, li, di, si = self._describe(input, "real")
+        po, lo, do_, _ = self._describe(output, "real")
+        if li != lo:
+            raise ValueError(f"input and output shapes differ: {li} and {lo}")
+        if di != do_:
+            raise ValueError("input and output must both be host or both be device buffers")
+        batch = int(np.prod(li, dtype=np.int64))
+        if batch == 0:
+            return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
+        self._call("dct", "dct", di, si, pi, po, batch, int(type), self.DCT_NORMS[norm])
+
+    def idct(self, input, output, type=2, norm="backward"):
+        """output = scipy.fft.idct(input, type=type, norm=norm): the dct of type 5 - type with the norms "backward" and
+        "forward" swapped, so that idct(dct(x, type, norm), type, norm) is x."""
+        if not isinstance(norm, str) or norm not in self.DCT_NORMS:
+            raise ValueError(f"norm must be one of {sorted(self.DCT_NORMS)}, got {norm!r}")
+        if type not in (2, 3) or isinstance(type, bool):
+            raise ValueError(f"type must be 2 or 3, got {type!r}")
+        swapped = {"backward": "forward", "forward": "backward", "ortho": "ortho"}[norm]
+        self.dct(input, output, type=5 - type, norm=swapped)
 
     WELCH_SCALINGS = {"density": 0, "spectrum": 1}
     WELCH_DETRENDS = {False: 0, "constant": 1}

@@ -367,6 +367,32 @@ int welch_exec(void* plan, const T* in, size_t in_len, const T* window, size_t h
       [&](cudaStream_t s) { return p->welch_device(in, in_len, window, hop, detrend, scaling, fs, out, batch, s); });
 }
 
+// Discrete cosine transform of real rows: type and norm checked before the plan is touched, even for batch == 0; in == out
+// allowed, otherwise disjoint.
+template <typename T>
+int dct_exec(void* plan, const T* in, T* out, size_t batch, int type, int norm, bool async, void* stream) {
+  if (!plan || !in || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
+  const char* bad = type != 2 && type != 3   ? "unknown type (the DCT types are 2 and 3)"
+                    : norm < 0 || norm > 2 ? "unknown norm (FOURIER_B200_DCT_NORM_BACKWARD, _ORTHO or _FORWARD)"
+                                           : nullptr;
+  if (bad) { fb200::set_last_error(bad); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  return run_call(
+      "dct", async, stream,
+      [&] {
+        if (batch == 0) return (int)p->dct_device(in, out, 0, type, norm, nullptr);
+        const size_t bytes = batch * p->size() * sizeof(T);
+        if (in != out && ranges_meet(in, bytes, out, bytes)) {
+          fb200::set_last_error("input and output overlap (they must be the same buffer or disjoint)");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {in, out}, "input and output must both be host or both be device memory",
+      [&] { return p->dct_host(in, out, batch, type, norm); },
+      {in, out}, [&](cudaStream_t s) { return p->dct_device(in, out, batch, type, norm, s); });
+}
+
 template <typename T>
 int istft_exec(void* plan, const void* in, size_t frames, const T* window, size_t hop, int center, T* out,
                size_t out_len, size_t batch, bool async, void* stream) {
@@ -735,6 +761,22 @@ int fourier_b200_welch_async_double(fourier_b200_rfft_double* plan, const double
                                     const double* window_dev, size_t hop, int detrend, int scaling, double fs,
                                     double* out_dev, size_t batch, void* stream) {
   return welch_exec<double>(plan, in_dev, in_len, window_dev, hop, detrend, scaling, fs, out_dev, batch, true, stream);
+}
+
+int fourier_b200_dct_float(fourier_b200_rfft_float* plan, const float* in, float* out, size_t batch, int type, int norm) {
+  return dct_exec<float>(plan, in, out, batch, type, norm, false, nullptr);
+}
+int fourier_b200_dct_double(fourier_b200_rfft_double* plan, const double* in, double* out, size_t batch, int type,
+                            int norm) {
+  return dct_exec<double>(plan, in, out, batch, type, norm, false, nullptr);
+}
+int fourier_b200_dct_async_float(fourier_b200_rfft_float* plan, const float* in_dev, float* out_dev, size_t batch,
+                                 int type, int norm, void* stream) {
+  return dct_exec<float>(plan, in_dev, out_dev, batch, type, norm, true, stream);
+}
+int fourier_b200_dct_async_double(fourier_b200_rfft_double* plan, const double* in_dev, double* out_dev, size_t batch,
+                                  int type, int norm, void* stream) {
+  return dct_exec<double>(plan, in_dev, out_dev, batch, type, norm, true, stream);
 }
 
 const char* fourier_b200_last_error(void) { return fb200::last_error(); }

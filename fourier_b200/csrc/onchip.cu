@@ -98,6 +98,8 @@ struct OnChipImpl {
     if ((e = allow_smem(onchip::onchip_lconv_kernel<Cfg<true>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_stft_kernel<Cfg<true>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_mel_kernel<Cfg<true>, MINB>))) return e;
+    if ((e = allow_smem(onchip::onchip_dct_kernel<Cfg<true>, MINB, 2>))) return e;
+    if ((e = allow_smem(onchip::onchip_dct_kernel<Cfg<true>, MINB, 3>))) return e;
     return cudaFuncSetAttribute(onchip::onchip_welch_kernel<Cfg<true>, MINB_WELCH>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_welch);
   }
@@ -119,6 +121,18 @@ struct OnChipImpl {
     const unsigned grid = (unsigned)std::min<size_t>((size_t)w.groups, (size_t)sms * MINB_WELCH * 4);
     onchip::onchip_welch_kernel<Cfg<true>, MINB_WELCH><<<grid, Cfg<true>::THREADS, smem_welch, s>>>(a);
     return cudaGetLastError();
+  }
+  static cudaError_t dct(const T* in, T* out, int type, const void* twa, const cpx<T>* tab, const cpx<T>* wq,
+                         size_t batch, T h, T h0, int sms, cudaStream_t s) {
+    typename onchip::Dct2Body<Cfg<true>>::Args a;
+    static_cast<typename onchip::RealBody<Cfg<true>>::Args&>(a) = {
+        nullptr, nullptr, (const TwPair<T>*)twa, tab, (long)batch, h};
+    a.x = in;
+    a.y = out;
+    a.wq = wq;
+    a.h0 = h0;
+    if (type == 2) return launch(onchip::onchip_dct_kernel<Cfg<true>, MINB, 2>, a, batch, sms, s);
+    return launch(onchip::onchip_dct_kernel<Cfg<true>, MINB, 3>, a, batch, sms, s);
   }
   static cudaError_t mel(const T* in, const T* win, const T* filters, const real::Band* bands, size_t n_mels, int power,
                          T* out, const real::FrameMap& m, size_t nframes, const void* twa, const cpx<T>* tab, int sms,
@@ -172,7 +186,8 @@ struct OnChipImpl {
                   {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab, (long)batch, h}, batch, sms, s);
   }
   static const OnChipOps<T>* ops() {
-    static const RealOnChipOps<T> r = {RA, RB, Cfg<true>::C, &real_prepare, &real, &conv, &lconv, &stft, &mel, &welch};
+    static const RealOnChipOps<T> r = {RA, RB, Cfg<true>::C, &real_prepare, &real, &conv, &lconv, &stft, &mel, &welch,
+                                      &dct};
     static const OnChipOps<T> o = {RA, RB, &prepare, &fft, kHasBluestein ? &bluestein : nullptr, &r};
     return &o;
   }

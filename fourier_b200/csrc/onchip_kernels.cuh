@@ -9,8 +9,9 @@
 //   * onchip_lconv_kernel:    linear convolution of real rows of any length by overlap-save on the same phases.
 //   * onchip_stft_kernel:     windowed frames of real rows of any length through the forward real-input phases.
 //   * onchip_mel_kernel:      the stft's frames to mel energies: power and filter bank on chip.
-//     (these six run the phases of FftBody / RealBody / ConvBody / LinConvBody / StftBody / MelBody through
-//     run_onchip_groups, tilefft.cuh)
+//   * onchip_dct_kernel:      discrete cosine transforms (types II and III) of real rows of length 2L.
+//     (these seven run the phases of FftBody / RealBody / ConvBody / LinConvBody / StftBody / MelBody /
+//     Dct2Body / Dct3Body through run_onchip_groups, tilefft.cuh)
 //   * onchip_welch_kernel:    detrended, windowed frames to Welch's averaged power spectrum, summed on chip
 //                             (WelchBody through run_welch_groups, below).
 //   * bluestein_fused_kernel: the whole chirp-z transform of the reference (bluesteins.rs:218-259) for
@@ -629,6 +630,199 @@ template <class Cfg, class Body> __device__ __forceinline__ void run_welch_group
 template <class Cfg, int MINB>
 __global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_welch_kernel(const typename WelchBody<Cfg>::Args a) {
   run_welch_groups<Cfg, WelchBody<Cfg>>(a);
+}
+
+// ---- fused discrete cosine transforms of real rows, N = 2L (real::dct2_pair / dct3_pair, DESIGN.md §4.16) --------
+// Type 2 (Dct2Body):
+//   * load (phase 0): lane u of the FFT reads the row as pairs (x[2j], x[2j+1]), j = u, u + TP, ..., and writes them
+//     into the FFT's park as reals in Makhoul's order, v[j] = x[2j] and v[N-1-j] = x[2j+1];
+//   * phases 1-4: StftBody's stage A from the park, the scatter, RealBody's gather + stage B and park;
+//   * pairs (phase 5): each lane forms the four outputs y[k], y[N-k], y[L-k], y[L+k] of the pairs it owns,
+//     k = u + TP*j, into tile registers 2j and 2j+1; lane u = 0's pair k = 0 gives only y[0] and y[L], so its register 1
+//     takes y[L/2] and y[3L/2] of the self-paired k = L/2;
+//   * park (phase 6): the N outputs go into the FFT's park as reals (no lane reads Z any more);
+//   * store (phase 7): consecutive lanes write consecutive outputs of the row.
+// Type 3 (Dct3Body):
+//   * load (phase 0): the row's N reals into the park, one complex value (two reals) per lane and step;
+//   * pairs (phase 1): each lane forms Z'[k] and Z'[L-k] of the pairs it owns, k = u + TP*j, from x[k], x[N-k], x[L-k]
+//     and x[L+k] in the park, into tile registers 2j and 2j+1 (lane u = 0: Z'[0] and the self-paired Z'[L/2]);
+//   * park (phase 2): Z' into the park in natural order;
+//   * phases 3-4: ConvBody's stage A on conj Z' from the park and its scatter: the inverse runs on the forward tile as
+//     conj(FFT(conj .));
+//   * phases 5-6: RealBody's gather + stage B and park: the park holds conj u as interleaved reals;
+//   * store (phase 7): lane u writes (y[2j], y[2j+1]) = (u[j], u[N-1-j]), j = u, u + TP, ..., as one complex value.
+// Forming Z'[n] straight in the stage-A registers instead, from the four inputs of each of the lane's E positions, made
+// ptxas spill 360-380 bytes at the f32 L = 512 and 1024 register caps (and 20-104 bytes at L = 128).
+// A row is read completely into the park before any of its outputs is stored, and only its own FFT reads it (a column
+// past the batch transforms zeros and stores nothing), so in == out is safe.
+template <class Cfg> struct Dct2Body {
+  using Stft = StftBody<Cfg>;
+  using Real = RealBody<Cfg>;
+  using Tile = typename Cfg::Tile;   // FWD = true
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  static constexpr int L = Cfg::L, TP = Tile::TP, E = Tile::E;
+  // Real::Args with in = out = nullptr and h the pair step's scale; x, y: rows of N = 2L reals (x == y allowed); wq: W^k,
+  // k <= L; h0: the scale of bin 0 (real::dct_scales)
+  struct Args : Real::Args { const T* x; T* y; const V* wq; T h0; };
+
+  static FB_HD long row(long grp, int t) { return grp * Cfg::C + Tile::template col_of<true>(t); }
+
+  static FB_HD void load(const Args& a, long grp, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const long b = row(grp, t);
+    T* z = reinterpret_cast<T*>(smem + Real::park(t));
+    if (b >= a.batch) {
+      for (int p = u; p < 2 * L; p += TP) z[p] = (T)0;
+      return;
+    }
+    const V* src = reinterpret_cast<const V*>(a.x + b * (2 * L));
+#pragma unroll 2
+    for (int j = u; j < L; j += TP) {
+      const V s = real::lin_ld(src + j, b);
+      z[j] = s.x;
+      z[2 * L - 1 - j] = s.y;
+    }
+  }
+  static FB_HD void pairs(Tile& f, const Args& a, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const V* z = smem + Real::park(t);
+#pragma unroll
+    for (int j = 0; j < E / 2; ++j) {
+      const int k = u + TP * j;
+      real::dct2_pair(z[k], z[(L - k) & (L - 1)], (long)L, (long)k, a.tab, a.wq, a.h, a.h0, f.v[2 * j], f.v[2 * j + 1]);
+    }
+    if (u == 0) {
+      V hi;
+      real::dct2_pair(z[L / 2], z[L / 2], (long)L, (long)(L / 2), a.tab, a.wq, a.h, a.h0, f.v[1], hi);
+    }
+  }
+  static FB_HD void park_out(const Tile& f, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    T* y = reinterpret_cast<T*>(smem + Real::park(t));
+#pragma unroll
+    for (int j = 0; j < E / 2; ++j) {
+      const int k = u + TP * j;
+      const V lo = f.v[2 * j], hi = f.v[2 * j + 1];
+      if (k == 0) {
+        y[0] = lo.x;
+        y[L] = lo.y;
+        y[L / 2] = hi.x;
+        y[3 * L / 2] = hi.y;
+      } else {
+        y[k] = lo.x;
+        y[2 * L - k] = lo.y;
+        y[L - k] = hi.x;
+        y[L + k] = hi.y;
+      }
+    }
+  }
+  static FB_HD void store(const Args& a, long grp, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const long b = row(grp, t);
+    if (b >= a.batch) return;
+    const T* y = reinterpret_cast<const T*>(smem + Real::park(t));
+    T* dst = a.y + b * (2 * L);
+#pragma unroll 2
+    for (int p = u; p < 2 * L; p += TP) real::lin_st(dst + p, y[p], b);
+  }
+
+  // phase protocol (tilefft.cuh): load into the park; StftBody's stage A and scatter; RealBody's gather + stage B and
+  // park; pairs, park, store
+  static constexpr int kPhases = 8;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    if constexpr (P == 0) load(a, grp, t, smem);
+    else if constexpr (P == 1) Stft::load_stage_a(f, t, smem, twa);
+    else if constexpr (P == 2) f.template scatter<true, typename Cfg::Lay>(t, smem);
+    else if constexpr (P == 3) Real::fwd_gather(f, t, smem);
+    else if constexpr (P == 4) Real::fwd_park(f, t, smem);
+    else if constexpr (P == 5) pairs(f, a, t, smem);
+    else if constexpr (P == 6) park_out(f, t, smem);
+    else store(a, grp, t, smem);
+  }
+};
+
+template <class Cfg> struct Dct3Body {
+  using Dct2 = Dct2Body<Cfg>;
+  using Conv = ConvBody<Cfg>;
+  using Real = RealBody<Cfg>;
+  using Tile = typename Cfg::Tile;   // FWD = true
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  static constexpr int L = Cfg::L, TP = Tile::TP, E = Tile::E;
+  using Args = typename Dct2::Args;
+
+  static FB_HD void load(const Args& a, long grp, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const long b = Dct2::row(grp, t);
+    V* z = smem + Real::park(t);
+    if (b >= a.batch) {
+      for (int j = u; j < L; j += TP) z[j] = mk<T>((T)0, (T)0);
+      return;
+    }
+    const V* src = reinterpret_cast<const V*>(a.x + b * (2 * L));
+#pragma unroll 2
+    for (int j = u; j < L; j += TP) z[j] = real::lin_ld(src + j, b);
+  }
+  // Z'[k] and Z'[L-k] of the pairs the lane owns into tile registers 2j and 2j+1 (lane u = 0: Z'[0] and Z'[L/2])
+  static FB_HD void pairs(Tile& f, const Args& a, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const T* x = reinterpret_cast<const T*>(smem + Real::park(t));
+#pragma unroll
+    for (int j = 0; j < E / 2; ++j)
+      real::dct3_pair(x, (long)L, (long)(u + TP * j), a.tab, a.wq, a.h, a.h0, f.v[2 * j], f.v[2 * j + 1]);
+    if (u == 0) {
+      V q;
+      real::dct3_pair(x, (long)L, (long)(L / 2), a.tab, a.wq, a.h, a.h0, f.v[1], q);
+    }
+  }
+  static FB_HD void park_pairs(const Tile& f, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    V* z = smem + Real::park(t);
+#pragma unroll
+    for (int j = 0; j < E / 2; ++j) {
+      const int k = u + TP * j;
+      z[k] = f.v[2 * j];
+      z[k == 0 ? L / 2 : L - k] = f.v[2 * j + 1];
+    }
+  }
+  static FB_HD void store(const Args& a, long grp, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const long b = Dct2::row(grp, t);
+    if (b >= a.batch) return;
+    const T* r = reinterpret_cast<const T*>(smem + Real::park(t));
+    V* dst = reinterpret_cast<V*>(a.y + b * (2 * L));
+    // u[p] = r[p] (p even), -r[p] (p odd); j and N-1-j have opposite parities
+#pragma unroll 2
+    for (int j = u; j < L; j += TP) {
+      const T lo = r[j], hi = r[2 * L - 1 - j];
+      real::lin_st(dst + j, (j & 1) ? mk<T>(-lo, hi) : mk<T>(lo, -hi), b);
+    }
+  }
+
+  // phase protocol (tilefft.cuh): load into the park; pairs, park Z'; ConvBody's conj stage A and scatter; RealBody's
+  // gather + stage B and park; store
+  static constexpr int kPhases = 8;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    if constexpr (P == 0) load(a, grp, t, smem);
+    else if constexpr (P == 1) pairs(f, a, t, smem);
+    else if constexpr (P == 2) park_pairs(f, t, smem);
+    else if constexpr (P == 3) Conv::inv_stage_a(f, t, smem, twa);
+    else if constexpr (P == 4) Conv::inv_scatter(f, t, smem);
+    else if constexpr (P == 5) Real::fwd_gather(f, t, smem);
+    else if constexpr (P == 6) Real::fwd_park(f, t, smem);
+    else store(a, grp, t, smem);
+  }
+};
+
+// the body of DCT type TYPE (2 or 3)
+template <class Cfg, int TYPE> struct DctBodyOf { using type = Dct2Body<Cfg>; };
+template <class Cfg> struct DctBodyOf<Cfg, 3> { using type = Dct3Body<Cfg>; };
+template <class Cfg, int TYPE> using DctBody = typename DctBodyOf<Cfg, TYPE>::type;
+
+template <class Cfg, int MINB, int TYPE>
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_dct_kernel(const typename Dct2Body<Cfg>::Args a) {
+  run_onchip_groups<Cfg, DctBody<Cfg, TYPE>>(a);
 }
 
 // ---- fused Bluestein -------------------------------------------------------------------------------------------

@@ -319,6 +319,10 @@ template <typename T> struct RealOnChipOps {
   // a row is one item, the row's output into out; base = s / F in device memory, detrend real::kDetrend*
   cudaError_t (*welch)(const T* in, const T* win, const T* base, int detrend, T* part, T* out, const real::FrameMap& m,
                        const real::WelchItems& w, const void* twa, const cpx<T>* tab, int sms, cudaStream_t);
+  // dct(): the discrete cosine transform of type 2 or 3 (DESIGN.md §4.16) of `batch` rows of N reals, in == out
+  // allowed; wq = W^k, k <= L; h, h0 from real::dct_scales
+  cudaError_t (*dct)(const T* in, T* out, int type, const void* twa, const cpx<T>* tab, const cpx<T>* wq, size_t batch,
+                     T h, T h0, int sms, cudaStream_t);
 };
 template <typename T> const RealOnChipOps<T>* real_onchip_lookup(size_t l);
 
@@ -401,6 +405,12 @@ class RealPlan {
   cudaError_t welch_host(const T* in, size_t in_len, const T* win, size_t hop, int detrend, int scaling, double fs,
                          T* out, size_t batch);
 
+  // Discrete cosine transform (DESIGN.md §4.16): `batch` rows of N reals -> rows of N reals, scipy.fft.dct(x, type,
+  // norm), type 2 or 3, norm real::kDctNorm*; checked by the caller.  in == out allowed.  Device pointers, on `stream`.
+  cudaError_t dct_device(const T* in, T* out, size_t batch, int type, int norm, cudaStream_t stream);
+  // Host pointers: whole rows through stage_rows; the same bits.
+  cudaError_t dct_host(const T* in, T* out, size_t batch, int type, int norm);
+
   unsigned long long launches() const { return launches_; }
   const char* kernel_name() const { return kernel_desc_.c_str(); }
 
@@ -469,6 +479,7 @@ class RealPlan {
   const RealOnChipOps<T>* fused_ = nullptr;
   std::unique_ptr<Plan<T>> inner_;   // length N/2 (kRealHalf) or N (kRealFull)
   DeviceBuffer tab_, twa_;           // w_N^k, k <= N/4 (even N); stage twiddles of the fused kernel
+  DeviceBuffer dct_tab_;             // W^k = exp(-i pi k / (2N)), k <= N/2: the twiddles of the DCT
   DeviceBuffer work_;                // one chunk of inner-plan rows
   DeviceBuffer stage_in_, stage_out_;
   DeviceBuffer stage_spec_;          // the constant operands of a host-pointer call: spectra, window, filters

@@ -19,6 +19,10 @@
 // Welch power spectral density (DESIGN.md §4.15): welch_scale_kernel, then per chunk of rows onchip_welch_kernel on the
 // fused path, or chunks of detrended windowed frames gathered into seg_, their spectra by the plan's own rfft behind
 // them and welch_accumulate_kernel into the partials; then welch_finish_kernel unless the fused kernel wrote the rows.
+// Discrete cosine transforms (DESIGN.md §4.16): onchip_dct_kernel on the fused path; otherwise per chunk of rows an O(N)
+// kernel into seg_, the inner plan in place there and an O(N) kernel into the output: dct_permute_kernel, Fft and
+// dct_untangle_kernel (type 2) or dct_tangle_kernel, UnscaledIfft and dct_unpermute_kernel (type 3) at half length;
+// dct_widen_kernel, Fft and dct_post_kernel or dct_pre_kernel, UnscaledIfft and dct_unpermute_kernel at full length.
 #include <algorithm>
 #include <string>
 #include <vector>
@@ -243,6 +247,85 @@ welch_finish_kernel(const T* __restrict__ part, long items, long n, const T* __r
   }
 }
 
+// Discrete cosine transforms (real::dct2_pair, dct3_pair, dct2_post, dct3_pre).  Rows of N reals in `in` / `out`, rows of the inner
+// plan's length in seg; one thread per element or pair of a row, consecutive threads along a row.
+//   permute: v into seg, N reals per row (half length) or N complex values with zero imaginary parts (full length);
+//   untangle: the pair k <= M/2 of Z in seg -> four outputs;  tangle: the pair k <= M/2 of Z' from the row into seg;
+//   post: the bin k <= N/2 of V in seg -> y[k], y[N-k];  pre: V'[k], k < N, from the row into seg;
+//   unpermute: output i from u in seg, N reals per row (half length) or the real parts of N complex values.
+template <typename T, bool WIDE>
+__global__ void __launch_bounds__(kThreads)
+dct_permute_kernel(const T* __restrict__ in, void* __restrict__ seg, long n, long batch) {
+  const long total = n * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / n, j = g - b * n;
+    const T x = real::lin_ld(in + b * n + real::dct_src(n, j), b);
+    if (WIDE) ((cpx<T>*)seg)[g] = mk<T>(x, (T)0);
+    else ((T*)seg)[g] = x;
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+dct_untangle_kernel(const cpx<T>* __restrict__ z, T* __restrict__ out, const cpx<T>* __restrict__ tab,
+                    const cpx<T>* __restrict__ wq, long m, long batch, T h, T h0) {
+  const long pairs = m / 2 + 1, total = pairs * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / pairs, k = g - b * pairs, n = 2 * m;
+    const cpx<T>* zb = z + b * m;
+    T* y = out + b * n;
+    cpx<T> lo, hi;
+    real::dct2_pair(zb[k], zb[k ? m - k : 0], m, k, tab, wq, h, h0, lo, hi);
+    real::lin_st(y + k, lo.x, b);
+    if (k == 0) { real::lin_st(y + m, lo.y, b); continue; }
+    real::lin_st(y + (n - k), lo.y, b);
+    if (m - k == k) continue;
+    real::lin_st(y + (m - k), hi.x, b);
+    real::lin_st(y + (m + k), hi.y, b);
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+dct_tangle_kernel(const T* __restrict__ in, cpx<T>* __restrict__ z, const cpx<T>* __restrict__ tab,
+                  const cpx<T>* __restrict__ wq, long m, long batch, T h, T h0) {
+  const long pairs = m / 2 + 1, total = pairs * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / pairs, k = g - b * pairs;
+    cpx<T> p, q;
+    real::dct3_pair(in + b * 2 * m, m, k, tab, wq, h, h0, p, q);
+    z[b * m + k] = p;
+    if (k > 0 && m - k != k) z[b * m + m - k] = q;
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+dct_post_kernel(const cpx<T>* __restrict__ v, T* __restrict__ out, const cpx<T>* __restrict__ wq, long n, long batch,
+                T h, T h0) {
+  const long bins = n / 2 + 1, total = bins * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / bins, k = g - b * bins;
+    real::dct2_post(v + b * n, out + b * n, n, k, wq, h, h0, b);
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+dct_pre_kernel(const T* __restrict__ in, cpx<T>* __restrict__ v, const cpx<T>* __restrict__ wq, long n, long batch, T h,
+               T h0) {
+  const long total = n * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / n;
+    v[g] = real::dct3_pre(in + b * n, n, g - b * n, wq, h, h0);
+  }
+}
+template <typename T, bool WIDE>
+__global__ void __launch_bounds__(kThreads)
+dct_unpermute_kernel(const void* __restrict__ seg, T* __restrict__ out, long n, long batch) {
+  const long total = n * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / n, s = b * n + real::dct_pos(n, g - b * n);
+    real::lin_st(out + g, WIDE ? ((const cpx<T>*)seg)[s].x : ((const T*)seg)[s], b);
+  }
+}
+
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
 real_part_kernel(const cpx<T>* __restrict__ y, T* __restrict__ out, size_t count) {
@@ -269,6 +352,13 @@ cudaError_t RealPlan<T>::init(size_t n, int device, bool allow_fast_paths) {
   device_ = device;
   DeviceGuard g(device_);
   if (!g.ok) { set_last_error("cudaSetDevice failed"); return cudaErrorInvalidDevice; }
+  std::vector<C> wq(n / 2 + 1);
+  for (size_t k = 0; k < wq.size(); ++k) {
+    double re, im;
+    host_twiddle(k, 4 * n, &re, &im);
+    wq[k] = mk<T>((T)re, (T)im);
+  }
+  FB_CHECK(upload(dct_tab_, wq));
   if (n % 2 != 0) {
     inner_.reset(Plan<T>::create(n, device, allow_fast_paths));
     if (!inner_) return cudaErrorUnknown;
@@ -309,7 +399,7 @@ PlanInfo RealPlan<T>::info() const {
   i.path = (int)path_;
   i.precision_bytes = (int)sizeof(T);
   i.device = device_;
-  i.table_bytes = tab_.bytes() + twa_.bytes() + (inner_ ? inner_->info().table_bytes : 0);
+  i.table_bytes = tab_.bytes() + twa_.bytes() + dct_tab_.bytes() + (inner_ ? inner_->info().table_bytes : 0);
   return i;
 }
 
@@ -860,6 +950,77 @@ cudaError_t RealPlan<T>::welch_host(const T* in, size_t in_len, const T* win, si
                       }));
   launches_ += 1;
   return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::dct_device(const T* in, T* out, size_t batch, int type, int norm, cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  double hd, h0d;
+  real::dct_scales(type, norm, (long)n_, hd, h0d);
+  const T h = (T)hd, h0 = (T)h0d;
+  const C* wq = (const C*)dct_tab_.data();
+  const C* tab = (const C*)tab_.data();
+  if (path_ == Path::kRealFused) {
+    FB_CHECK(fused_->dct(in, out, type, twa_.data(), tab, wq, batch, h, h0, sm_count_, s));
+    launches_ = 1;
+    return cudaSuccess;
+  }
+  // chunks of rows through seg_: N reals per row (half length) or N complex values (full length); the first kernel reads
+  // the chunk's input rows whole and only the last one writes its output rows, so in == out is safe
+  const bool half = path_ == Path::kRealHalf;
+  const size_t row = half ? n_ * sizeof(T) : n_ * sizeof(C);
+  const size_t chunk = scratch_chunk(batch, row);
+  FB_CHECK(seg_.reserve(chunk * row));
+  void* seg = seg_.data();
+  unsigned long long count = 0;
+  for (size_t b0 = 0; b0 < batch; b0 += chunk) {
+    const size_t nb = std::min(chunk, batch - b0);
+    const T* x = in + b0 * n_;
+    T* y = out + b0 * n_;
+    if (half) {
+      const unsigned pairs = grid_for((m_ / 2 + 1) * nb);
+      if (type == 2) {
+        dct_permute_kernel<T, false><<<grid_for(nb * n_), kThreads, 0, s>>>(x, seg, (long)n_, (long)nb);
+        FB_CHECK(cudaGetLastError());
+        FB_CHECK(inner_->exec_device((C*)seg, (C*)seg, nb, kFft, s));
+        dct_untangle_kernel<T><<<pairs, kThreads, 0, s>>>((const C*)seg, y, tab, wq, (long)m_, (long)nb, h, h0);
+      } else {
+        dct_tangle_kernel<T><<<pairs, kThreads, 0, s>>>(x, (C*)seg, tab, wq, (long)m_, (long)nb, h, h0);
+        FB_CHECK(cudaGetLastError());
+        FB_CHECK(inner_->exec_device((C*)seg, (C*)seg, nb, kUnscaledIfft, s));
+        dct_unpermute_kernel<T, false><<<grid_for(nb * n_), kThreads, 0, s>>>(seg, y, (long)n_, (long)nb);
+      }
+    } else {
+      if (type == 2) {
+        dct_permute_kernel<T, true><<<grid_for(nb * n_), kThreads, 0, s>>>(x, seg, (long)n_, (long)nb);
+        FB_CHECK(cudaGetLastError());
+        FB_CHECK(inner_->exec_device((C*)seg, (C*)seg, nb, kFft, s));
+        dct_post_kernel<T><<<grid_for((n_ / 2 + 1) * nb), kThreads, 0, s>>>((const C*)seg, y, wq, (long)n_, (long)nb, h,
+                                                                           h0);
+      } else {
+        dct_pre_kernel<T><<<grid_for(nb * n_), kThreads, 0, s>>>(x, (C*)seg, wq, (long)n_, (long)nb, h, h0);
+        FB_CHECK(cudaGetLastError());
+        FB_CHECK(inner_->exec_device((C*)seg, (C*)seg, nb, kUnscaledIfft, s));
+        dct_unpermute_kernel<T, true><<<grid_for(nb * n_), kThreads, 0, s>>>(seg, y, (long)n_, (long)nb);
+      }
+    }
+    FB_CHECK(cudaGetLastError());
+    count += 2 + inner_->launches();
+  }
+  launches_ = count;
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::dct_host(const T* in, T* out, size_t batch, int type, int norm) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  return stage_rows(in, out, batch, n_ * sizeof(T), n_ * sizeof(T), [&](const void* din, void* dout, size_t, size_t nb) {
+    return dct_device((const T*)din, (T*)dout, nb, type, norm, host_stream_);
+  });
 }
 
 template class RealPlan<float>;

@@ -379,6 +379,38 @@ int fourier_b200_welch_async_double(struct fourier_b200_rfft_double *plan, const
                                     const double *window_dev, size_t hop, int detrend, int scaling, double fs,
                                     double *out_dev, size_t batch, void *cuda_stream);
 
+/* ---- discrete cosine transforms of real rows (types II and III) ----
+ * On a real plan of length N >= 1, for `batch` rows of N reals (row b at element b*N), with W = exp(-i pi / (2N)) and
+ * Makhoul's reordering v[j] = x[2j] (j < ceil(N/2)), v[N-1-j] = x[2j+1] (j < floor(N/2)):
+ *   type 2:  V = FFT_N(v),  y[k] = 2 h Re(W^k V[k]) (0 <= k <= N/2),  y[N-k] = -2 h Im(W^k V[k]) (0 < k <= N/2),
+ *            i.e. y[k] = 2 h sum_n x[n] cos(pi k (2n+1) / (2N));
+ *   type 3:  V'[k] = h conj(W^k) (x[k] - i x[N-k]) (0 < k <= N/2),  V'[0] = h x[0],  u = N irfft(V', n = N),
+ *            y[2j] = u[j], y[2j+1] = u[N-1-j], i.e. y[k] = h x[0] + 2 h sum_{n>0} x[n] cos(pi (2k+1) n / (2N)).
+ * The norm sets h: 1 (FOURIER_B200_DCT_NORM_BACKWARD), 1 / (2N) (_FORWARD) or 1 / sqrt(2N) (_ORTHO, which also scales
+ * y[0] of type 2 by 1 / sqrt(2) and x[0] of type 3 by sqrt(2)).  This is scipy.fft.dct(x, type, norm) with
+ * orthogonalize=True, and FFTW's REDFT10 (type 2) and REDFT01 (type 3) with the backward norm.  scipy.fft.idct(x, type,
+ * norm) is the call with type 5 - type and norm backward and forward swapped.  torch has no DCT.
+ * Launches: 1 on the real_fused path (N = 128 .. 2048 in f32, 128 .. 512 in f64); on the others, per scratch chunk of
+ * rows (512 MB), 2 plus those of the inner plan: a reordering or twiddle kernel, the inner complex plan of length N/2
+ * (even N) or N (odd N) in place in the scratch, and a kernel that writes the output rows.
+ * Refused with cudaErrorInvalidValue and a message: a NULL argument, a type other than 2 and 3, a norm other than the
+ * three macros (these also when batch == 0, which otherwise succeeds and launches nothing), input and output
+ * overlapping without being the same buffer, and a mix of host and device buffers in the synchronous calls.  in == out
+ * transforms in place.  Device base pointers must be 16-byte aligned (cudaErrorMisalignedAddress).  Host memory is
+ * staged through the plan's buffers in whole rows and gives the same bits as device memory.  The _async calls take
+ * device memory, are enqueued on `cuda_stream` and never synchronise the host. */
+#define FOURIER_B200_DCT_NORM_BACKWARD 0
+#define FOURIER_B200_DCT_NORM_ORTHO 1
+#define FOURIER_B200_DCT_NORM_FORWARD 2
+int fourier_b200_dct_float(struct fourier_b200_rfft_float *plan, const float *in, float *out, size_t batch, int type,
+                           int norm);
+int fourier_b200_dct_double(struct fourier_b200_rfft_double *plan, const double *in, double *out, size_t batch,
+                            int type, int norm);
+int fourier_b200_dct_async_float(struct fourier_b200_rfft_float *plan, const float *in_dev, float *out_dev,
+                                 size_t batch, int type, int norm, void *cuda_stream);
+int fourier_b200_dct_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev, double *out_dev,
+                                  size_t batch, int type, int norm, void *cuda_stream);
+
 const char *fourier_b200_last_error(void);
 const char *fourier_b200_version(void);
 
