@@ -26,6 +26,9 @@ reference's operator interface name for name:
                                                             frames frame-major), the spectrum kept on chip
     (no counterpart)                                      RealFft.welch: Welch's power spectral density of real
                                                             rows (scipy.signal.welch), frames summed on chip
+    (no counterpart)                                      RealFft.csd / coherence: cross-spectral density and
+                                                            magnitude-squared coherence of real row pairs
+                                                            (scipy.signal.csd / coherence), frames summed on chip
     (no counterpart)                                      RealFft.dct / idct: discrete cosine transforms of real
                                                             rows, types 2 and 3 (scipy.fft.dct / idct; torch has
                                                             none)
@@ -524,6 +527,54 @@ class RealFft:
             return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
         self._call("welch", "welch", di, si, pi, in_len, pw, hop, self.WELCH_DETRENDS[detrend],
                    self.WELCH_SCALINGS[scaling], fs, po, batch)
+
+    def csd(self, x, y, window, hop, output, fs=1.0, scaling="density", detrend="constant"):
+        """Cross-spectral density of every row of `x` (shape (..., L), L >= N) with its row of `y`: welch's frames of
+        both, detrended and windowed alike, averaged as conj(rfft(x frame)) * rfft(y frame), one-sided and scaled as
+        welch does.  `y` has rows of the same L, and its leading shape must equal a trailing part of x's and is
+        broadcast over the rest, as convolve's spectrum is.  `output` has shape (..., N//2+1) in the complex dtype and
+        x's leading shape: this is scipy.signal.csd(x, y, fs, window=window, nperseg=N, noverlap=N-hop,
+        detrend=detrend, scaling=scaling)[1].  The frames stay on chip where the plan's path allows.  Out of place
+        only."""
+        if not isinstance(scaling, str) or scaling not in self.WELCH_SCALINGS:
+            raise ValueError(f"scaling must be 'density' or 'spectrum', got {scaling!r}")
+        fs = float(fs)
+        if not (np.isfinite(fs) and fs > 0):
+            raise ValueError(f"fs must be finite and positive, got {fs!r}")
+        self._cross("csd", x, y, window, hop, output, detrend, self.WELCH_SCALINGS[scaling], fs)
+
+    def coherence(self, x, y, window, hop, output, detrend="constant"):
+        """Magnitude-squared coherence of every row of `x` with its row of `y` (framed and broadcast as in csd):
+        |sum conj(X) Y|**2 / (sum |X|**2 * sum |Y|**2) over the frames, per bin.  `output` has shape (..., N//2+1) in
+        the real dtype: this is scipy.signal.coherence(x, y, fs, window=window, nperseg=N, noverlap=N-hop,
+        detrend=detrend)[1] for any fs.  NaN where a denominator is 0, as scipy gives.  Out of place only."""
+        self._cross("coherence", x, y, window, hop, output, detrend, None, None)
+
+    def _cross(self, kind, x, y, window, hop, output, detrend, scaling, fs):
+        self._check_resolved(x, y, window, output)
+        if not (detrend is False or (isinstance(detrend, str) and detrend == "constant")):
+            raise ValueError(f"detrend must be 'constant' or False, got {detrend!r}")
+        hop, _, in_len, _, (pi, li, di, si), (pw, dw) = self._framing(x, window, hop, False, "reflect")
+        if getattr(y, "ndim", 0) == 0 or y.shape[-1] != in_len:
+            raise ValueError(f"y rows must hold the {in_len} samples of the x rows")
+        py, ly, dy, _ = self._describe(y, "real", last=in_len)
+        po, lo, do_, _ = self._describe(output, "spec" if kind == "csd" else "real", last=self._size // 2 + 1)
+        if li != lo:
+            raise ValueError(f"x and output leading shapes differ: {li} and {lo}")
+        if len(ly) > len(li) or tuple(li[len(li) - len(ly):]) != ly:
+            raise ValueError(f"y leading shape {ly} is not a trailing part of x's {li}")
+        if not (di == dy == dw == do_):
+            raise ValueError("x, y, window and output must all be host or all be device buffers")
+        batch = int(np.prod(li, dtype=np.int64))
+        if batch == 0:
+            return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
+        y_rows = int(np.prod(ly, dtype=np.int64))
+        if kind == "csd":
+            self._call("csd", "csd", di, si, pi, py, y_rows, in_len, pw, hop, self.WELCH_DETRENDS[detrend], scaling,
+                       fs, po, batch)
+        else:
+            self._call("coherence", "coherence", di, si, pi, py, y_rows, in_len, pw, hop, self.WELCH_DETRENDS[detrend],
+                       po, batch)
 
     def istft(self, input, window, hop, output, center=True):
         """Inverse of stft: `input` (shape (..., F, N//2+1), stft's frame-major layout) -> `output` (shape

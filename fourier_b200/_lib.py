@@ -35,6 +35,7 @@ EXTENSION_SYMBOLS = (
     + [f"fourier_b200_{fn}_{op}{t}" for fn in ("stft", "istft") for t in ("float", "double") for op in ("", "async_")]
     + [f"fourier_b200_mel_spectrogram_{op}{t}" for t in ("float", "double") for op in ("", "async_")]
     + [f"fourier_b200_welch_{op}{t}" for t in ("float", "double") for op in ("", "async_")]
+    + [f"fourier_b200_{fn}_{op}{t}" for fn in ("csd", "coherence") for t in ("float", "double") for op in ("", "async_")]
     + [f"fourier_b200_dct_{op}{t}" for t in ("float", "double") for op in ("", "async_")])
 
 
@@ -96,6 +97,11 @@ def load():
         getattr(L, f"fourier_b200_mel_spectrogram_async_{t}").argtypes = [vp, vp, sz, vp, sz, ci, ci, vp, sz, vp, sz, vp]
         getattr(L, f"fourier_b200_welch_{t}").argtypes = [vp, vp, sz, vp, sz, ci, ci, ctypes.c_double, vp, sz]
         getattr(L, f"fourier_b200_welch_async_{t}").argtypes = [vp, vp, sz, vp, sz, ci, ci, ctypes.c_double, vp, sz, vp]
+        getattr(L, f"fourier_b200_csd_{t}").argtypes = [vp, vp, vp, sz, sz, vp, sz, ci, ci, ctypes.c_double, vp, sz]
+        getattr(L, f"fourier_b200_csd_async_{t}").argtypes = [vp, vp, vp, sz, sz, vp, sz, ci, ci, ctypes.c_double, vp,
+                                                              sz, vp]
+        getattr(L, f"fourier_b200_coherence_{t}").argtypes = [vp, vp, vp, sz, sz, vp, sz, ci, vp, sz]
+        getattr(L, f"fourier_b200_coherence_async_{t}").argtypes = [vp, vp, vp, sz, sz, vp, sz, ci, vp, sz, vp]
         getattr(L, f"fourier_b200_dct_{t}").argtypes = [vp, vp, vp, sz, ci, ci]
         getattr(L, f"fourier_b200_dct_async_{t}").argtypes = [vp, vp, vp, sz, ci, ci, vp]
     L.fourier_b200_peer_alloc.argtypes = [sz, ctypes.POINTER(vp), ctypes.c_char_p]

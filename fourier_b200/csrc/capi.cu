@@ -393,6 +393,45 @@ int dct_exec(void* plan, const T* in, T* out, size_t batch, int type, int norm, 
       {in, out}, [&](cudaStream_t s) { return p->dct_device(in, out, batch, type, norm, s); });
 }
 
+// Cross-spectral density (coh false) and coherence of real rows: welch_exec's rules for x, the window, hop, detrend
+// (and for the csd scaling and fs), plus y and y_rows, checked before the plan is touched; y may overlap x.
+template <typename T>
+int cross_exec(void* plan, const T* x, const T* y, size_t y_rows, size_t in_len, const T* window, size_t hop,
+               int detrend, bool coh, int scaling, double fs, void* out, size_t batch, bool async, void* stream) {
+  if (!plan || !x || !y || !window || !out) { fb200::set_last_error("null argument"); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  if (!check_frames(p, in_len, hop, fb200::real::kStftNone,
+                    y_rows == 0                              ? "y_rows must be at least 1"
+                    : detrend != 0 && detrend != 1           ? "unknown detrend (FOURIER_B200_DETREND_NONE or _CONSTANT)"
+                    : !coh && scaling != 0 && scaling != 1   ? "unknown scaling (FOURIER_B200_WELCH_DENSITY or _SPECTRUM)"
+                    : !coh && !(std::isfinite(fs) && fs > 0) ? "fs must be finite and positive"
+                                                             : nullptr))
+    return (int)cudaErrorInvalidValue;
+  const size_t n = p->size();
+  const char* what = coh ? "coherence" : "csd";
+  return run_call(
+      what, async, stream,
+      [&] {
+        if (batch == 0)
+          return (int)p->cross_device(x, y, y_rows, in_len, window, hop, detrend, coh, scaling, fs, out, 0, nullptr);
+        const size_t x_bytes = batch * in_len * sizeof(T), y_bytes = y_rows * in_len * sizeof(T);
+        const size_t out_bytes = batch * (n / 2 + 1) * (coh ? sizeof(T) : 2 * sizeof(T));
+        if (ranges_meet(x, x_bytes, out, out_bytes) || ranges_meet(y, y_bytes, out, out_bytes) ||
+            ranges_meet(window, n * sizeof(T), out, out_bytes)) {
+          fb200::set_last_error(coh ? "x, y or window and output overlap (coherence is out of place only)"
+                                    : "x, y or window and output overlap (csd is out of place only)");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {x, y, window, out}, "x, y, window and output must all be host or all be device memory",
+      [&] { return p->cross_host(x, y, y_rows, in_len, window, hop, detrend, coh, scaling, fs, out, batch); },
+      {x, y, out},
+      [&](cudaStream_t s) {
+        return p->cross_device(x, y, y_rows, in_len, window, hop, detrend, coh, scaling, fs, out, batch, s);
+      });
+}
+
 template <typename T>
 int istft_exec(void* plan, const void* in, size_t frames, const T* window, size_t hop, int center, T* out,
                size_t out_len, size_t batch, bool async, void* stream) {
@@ -777,6 +816,49 @@ int fourier_b200_dct_async_float(fourier_b200_rfft_float* plan, const float* in_
 int fourier_b200_dct_async_double(fourier_b200_rfft_double* plan, const double* in_dev, double* out_dev, size_t batch,
                                   int type, int norm, void* stream) {
   return dct_exec<double>(plan, in_dev, out_dev, batch, type, norm, true, stream);
+}
+
+int fourier_b200_csd_float(fourier_b200_rfft_float* plan, const float* x, const float* y, size_t y_rows, size_t in_len,
+                       const float* window, size_t hop, int detrend, int scaling, double fs, void* out, size_t batch) {
+  return cross_exec<float>(plan, x, y, y_rows, in_len, window, hop, detrend, false, scaling, fs, out, batch, false,
+                           nullptr);
+}
+int fourier_b200_csd_async_float(fourier_b200_rfft_float* plan, const float* x_dev, const float* y_dev, size_t y_rows,
+                             size_t in_len, const float* window_dev, size_t hop, int detrend, int scaling, double fs,
+                             void* out_dev, size_t batch, void* stream) {
+  return cross_exec<float>(plan, x_dev, y_dev, y_rows, in_len, window_dev, hop, detrend, false, scaling, fs, out_dev,
+                           batch, true, stream);
+}
+int fourier_b200_coherence_float(fourier_b200_rfft_float* plan, const float* x, const float* y, size_t y_rows,
+                             size_t in_len, const float* window, size_t hop, int detrend, float* out, size_t batch) {
+  return cross_exec<float>(plan, x, y, y_rows, in_len, window, hop, detrend, true, 0, 1.0, out, batch, false, nullptr);
+}
+int fourier_b200_coherence_async_float(fourier_b200_rfft_float* plan, const float* x_dev, const float* y_dev,
+                                   size_t y_rows, size_t in_len, const float* window_dev, size_t hop, int detrend,
+                                   float* out_dev, size_t batch, void* stream) {
+  return cross_exec<float>(plan, x_dev, y_dev, y_rows, in_len, window_dev, hop, detrend, true, 0, 1.0, out_dev, batch,
+                           true, stream);
+}
+int fourier_b200_csd_double(fourier_b200_rfft_double* plan, const double* x, const double* y, size_t y_rows, size_t in_len,
+                       const double* window, size_t hop, int detrend, int scaling, double fs, void* out, size_t batch) {
+  return cross_exec<double>(plan, x, y, y_rows, in_len, window, hop, detrend, false, scaling, fs, out, batch, false,
+                           nullptr);
+}
+int fourier_b200_csd_async_double(fourier_b200_rfft_double* plan, const double* x_dev, const double* y_dev, size_t y_rows,
+                             size_t in_len, const double* window_dev, size_t hop, int detrend, int scaling, double fs,
+                             void* out_dev, size_t batch, void* stream) {
+  return cross_exec<double>(plan, x_dev, y_dev, y_rows, in_len, window_dev, hop, detrend, false, scaling, fs, out_dev,
+                           batch, true, stream);
+}
+int fourier_b200_coherence_double(fourier_b200_rfft_double* plan, const double* x, const double* y, size_t y_rows,
+                             size_t in_len, const double* window, size_t hop, int detrend, double* out, size_t batch) {
+  return cross_exec<double>(plan, x, y, y_rows, in_len, window, hop, detrend, true, 0, 1.0, out, batch, false, nullptr);
+}
+int fourier_b200_coherence_async_double(fourier_b200_rfft_double* plan, const double* x_dev, const double* y_dev,
+                                   size_t y_rows, size_t in_len, const double* window_dev, size_t hop, int detrend,
+                                   double* out_dev, size_t batch, void* stream) {
+  return cross_exec<double>(plan, x_dev, y_dev, y_rows, in_len, window_dev, hop, detrend, true, 0, 1.0, out_dev, batch,
+                           true, stream);
 }
 
 const char* fourier_b200_last_error(void) { return fb200::last_error(); }

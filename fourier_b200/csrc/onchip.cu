@@ -40,6 +40,11 @@ struct OnChipImpl {
   // per H100 SM, 1 KB of it reserved per CTA).  That is f32 L = 128 only: 3 instead of 4, which also lifts its register
   // cap from 64 to 80, at which it does not spill.
   static constexpr int MINB_WELCH = std::min<int>(MINB, (int)((228u << 10) / (smem_welch + 1024)));
+  // The csd and coherence kernels' the same way: csd's accumulators are Welch's size, the coherence's twice that
+  // (DESIGN.md §4.17 has the CTAs per SM this gives).
+  template <bool COH> using Csd = onchip::CsdBody<Cfg<true>, COH>;
+  static constexpr size_t smem_csd(bool coh) { return smem_fft + (coh ? Csd<true>::ACC_BYTES : Csd<false>::ACC_BYTES); }
+  static constexpr int minb_csd(bool coh) { return std::min<int>(MINB, (int)((228u << 10) / (smem_csd(coh) + 1024))); }
   static constexpr size_t smem_blue() {
     return BCfg::EX_BYTES + BCfg::TWA_BYTES +
            sizeof(cpx<T>) * (4 * (size_t)BCfg::L + (K::LOCAL_STASH ? 0 : (size_t)K::E * BCfg::THREADS));
@@ -100,8 +105,41 @@ struct OnChipImpl {
     if ((e = allow_smem(onchip::onchip_mel_kernel<Cfg<true>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_dct_kernel<Cfg<true>, MINB, 2>))) return e;
     if ((e = allow_smem(onchip::onchip_dct_kernel<Cfg<true>, MINB, 3>))) return e;
+    if ((e = cudaFuncSetAttribute(onchip::onchip_csd_kernel<Cfg<true>, minb_csd(false), false>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_csd(false)))) return e;
+    if ((e = cudaFuncSetAttribute(onchip::onchip_csd_kernel<Cfg<true>, minb_csd(true), true>,
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_csd(true)))) return e;
     return cudaFuncSetAttribute(onchip::onchip_welch_kernel<Cfg<true>, MINB_WELCH>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_welch);
+  }
+  // the csd (coh false) or coherence items of w over C/2 pair columns, as welch(); row b of m pairs with y row
+  // (y_off + b) mod y_rows
+  static cudaError_t csd(const T* x, const T* y, size_t y_rows, size_t y_off, const T* win, const T* base, int detrend,
+                         bool coh, T* part, void* out, const real::FrameMap& m, const real::WelchItems& w,
+                         const void* twa, const cpx<T>* tab, int sms, cudaStream_t s) {
+    onchip::CsdArgs<Cfg<true>> a;
+    static_cast<typename onchip::RealBody<Cfg<true>>::Args&>(a) = {
+        nullptr, nullptr, (const TwPair<T>*)twa, tab, 0, (T)0.5};
+    a.x = x;
+    a.win = win;
+    a.m = m;
+    a.part = part;
+    a.psd = (T*)out;
+    a.base = base;
+    a.w = w;
+    a.detrend = detrend;
+    a.y = y;
+    a.y_rows = (long)y_rows;
+    a.y_off = (long)y_off;
+    a.y_rcp = 1.0 / (double)y_rows;
+    if (coh) {
+      const unsigned grid = (unsigned)std::min<size_t>((size_t)w.groups, (size_t)sms * minb_csd(true) * 4);
+      onchip::onchip_csd_kernel<Cfg<true>, minb_csd(true), true><<<grid, Cfg<true>::THREADS, smem_csd(true), s>>>(a);
+    } else {
+      const unsigned grid = (unsigned)std::min<size_t>((size_t)w.groups, (size_t)sms * minb_csd(false) * 4);
+      onchip::onchip_csd_kernel<Cfg<true>, minb_csd(false), false><<<grid, Cfg<true>::THREADS, smem_csd(false), s>>>(a);
+    }
+    return cudaGetLastError();
   }
   // the items of w, groups grid-stride over at most sms * MINB_WELCH * 4 CTAs, as launch() does
   static cudaError_t welch(const T* in, const T* win, const T* base, int detrend, T* part, T* out,
@@ -187,7 +225,7 @@ struct OnChipImpl {
   }
   static const OnChipOps<T>* ops() {
     static const RealOnChipOps<T> r = {RA, RB, Cfg<true>::C, &real_prepare, &real, &conv, &lconv, &stft, &mel, &welch,
-                                      &dct};
+                                      &dct, &csd};
     static const OnChipOps<T> o = {RA, RB, &prepare, &fft, kHasBluestein ? &bluestein : nullptr, &r};
     return &o;
   }

@@ -14,6 +14,8 @@
 //     Dct2Body / Dct3Body through run_onchip_groups, tilefft.cuh)
 //   * onchip_welch_kernel:    detrended, windowed frames to Welch's averaged power spectrum, summed on chip
 //                             (WelchBody through run_welch_groups, below).
+//   * onchip_csd_kernel:      Welch's frames of two signals in pairs to their cross-spectral density or coherence
+//                             (CsdBody through run_welch_groups, below).
 //   * bluestein_fused_kernel: the whole chirp-z transform of the reference (bluesteins.rs:218-259) for
 //                             N <= L, M = 2L, in one kernel and without touching HBM in between.
 //
@@ -518,6 +520,11 @@ template <class Cfg> struct WelchBody {
     slot(a, g, r, t, i, b, f);
     const long fg = b * a.w.frames + f;
     const T* src = a.x + b * a.m.in_ld + f * a.m.hop;
+    load_frame(src, fg, u, t, smem, acc);
+  }
+  // the frame of N raw samples from src into the park of thread t (lane u), and its lane sum behind the C rows of
+  // accumulators; fg: the frame of the launch, for the access log
+  static FB_HD void load_frame(const T* src, long fg, int u, int t, V* smem, T* acc) {
     T* z = reinterpret_cast<T*>(smem + Real::park(t));
     opaque(z);
     T s = 0;
@@ -592,11 +599,141 @@ template <class Cfg> struct WelchBody {
     else if constexpr (P <= 5) Stft::template phase<P - 1>(f, a, 0, t, smem, twa);
     else accumulate(a, g, r, t, smem, acc);
   }
+  // the barrier after phase P: the threads of one FFT share a warp
+  static constexpr bool pair_barrier(int) { return false; }
 };
 
-// The device driver of WelchBody: run_onchip_groups' set-up, then per group its rounds, each phase followed by
-// __syncwarp, and the flush between two CTA barriers (the accumulators of every column are complete before it, and it
-// has read them before the next group's round 0 stores).  tools/emulate_common.h has the CPU driver.
+// ---- fused cross-spectral density and coherence of real rows, N = 2L (DESIGN.md §4.17) ----------------------------
+// WelchBody's rounds on frame pairs: pair column c of the tile holds the x frame in FFT column 2c and the y frame in
+// column 2c+1, so a round runs C/2 frame pairs and the items are real::WelchItems over C/2 pair columns.  Per frame pair:
+//   * load and detrend (phases 0-1): WelchBody's, each column from its own row (x row b, y row (y_off + b) mod y_rows);
+//   * phases 2-5: StftBody's stage A, scatter, gather + stage B and park, per column as in Welch;
+//   * cross (phase 6): the 2 TP lanes of a pair split its bin pairs (k = u + TP j, j even in the x column, odd in the
+//     y column; lane u = 0 of the x column also k = L/2), untangle X and Y of each from both parks (real::spec_pair)
+//     and add real::cross_terms to the pair column's PLANES planes of L+1 accumulators (stores them in round 0).
+// Phase 6 reads the partner column's park: with TP <= 16 both columns sit in one warp and __syncwarp orders it; at
+// TP = 32 (f32 L = 1024) they are two warps, and a barrier over the pair's 64 threads follows the park (phase 5) and
+// the cross phase (before the next round's load overwrites the parks).  The flush sums each plane of an item over its
+// pair columns in ascending order into the item's partial, or, when a row is one item, writes the row's output.
+// Shared memory behind the exchange and the stage twiddles: C/2 pair columns of PLANES (L+1) accumulators, then one lane
+// sum per thread (where WelchBody's load and detrend keep it).
+// WelchBody::Args (x, part, psd, base, w over C/2 pair columns, detrend) plus the y rows: row b of the launch pairs
+// with y row (y_off + b) mod y_rows, y_rcp = 1 / y_rows; psd: the csd's N/2+1 complex values per row (cpx<T>), or the
+// coherence's N/2+1 reals
+template <class Cfg> struct CsdArgs : WelchBody<Cfg>::Args {
+  const typename WelchBody<Cfg>::T* y;
+  long y_rows, y_off;
+  double y_rcp;
+};
+template <class Cfg, bool COH> struct CsdBody {
+  using Welch = WelchBody<Cfg>;
+  using Stft = StftBody<Cfg>;
+  using Real = RealBody<Cfg>;
+  using Tile = typename Cfg::Tile;   // FWD = true
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  static constexpr int L = Cfg::L, TP = Tile::TP, E = Tile::E, C = Cfg::C, THREADS = Cfg::THREADS, BINS = L + 1;
+  static constexpr int PLANES = COH ? real::kCoherencePlanes : real::kCsdPlanes, PAIRS = C / 2;
+  static constexpr size_t ACC_BYTES = sizeof(T) * ((size_t)PAIRS * PLANES * BINS + THREADS);
+  static_assert(C % 2 == 0 && E % 4 == 0 && (2 * TP <= 32 || TP == 32), "a frame pair is one warp or two");
+  using Args = CsdArgs<Cfg>;
+
+  template <typename U> static FB_HD void opaque(U& v) { Welch::opaque(v); }
+  // Welch's load and detrend find the lane sums behind C (L+1) reals
+  static FB_HD T* sums_base(T* acc) { return acc + ((size_t)PAIRS * PLANES * BINS - (size_t)C * BINS); }
+  static FB_HD bool slot(const Args& a, long g, long r, int t, long& i, long& b, long& f) {
+    Welch::opaque(g);
+    return a.w.slot(g, Tile::template col_of<true>(t) >> 1, r, i, b, f);
+  }
+  static FB_HD void load(const Args& a, long g, long r, int t, V* smem, T* acc) {
+    const int u = Tile::template u_of<true>(t);
+    long i, b, f;
+    slot(a, g, r, t, i, b, f);
+    const T* row = a.x + b * a.m.in_ld;
+    if (Tile::template col_of<true>(t) & 1) {
+      const long yb = a.y_off + b;
+      row = a.y + (yb - real::div_rcp(yb, a.y_rows, a.y_rcp) * a.y_rows) * a.m.in_ld;
+    }
+    Welch::load_frame(row + f * a.m.hop, b * a.w.frames + f, u, t, smem, sums_base(acc));
+  }
+  static FB_HD void cross(const Args& a, long g, long r, int t, const V* smem, T* acc) {
+    const int u = Tile::template u_of<true>(t), col = Tile::template col_of<true>(t), side = col & 1;
+    long i, b, f;
+    if (!slot(a, g, r, t, i, b, f)) return;
+    const V* zx = smem + (col - side) * Cfg::Lay::SC;
+    const V* zy = zx + Cfg::Lay::SC;
+    const V* tab = a.tab;
+    T* y = acc + (col >> 1) * PLANES * BINS;
+    Welch::opaque(zx);
+    Welch::opaque(zy);
+    Welch::opaque(tab);
+    Welch::opaque(y);
+    auto add = [&](int k, V xv, V yv) FB_LAMBDA {
+      T d[real::kCoherencePlanes];
+      real::cross_terms(xv, yv, d);
+#pragma unroll
+      for (int q = 0; q < PLANES; ++q) y[q * BINS + k] = r == 0 ? d[q] : y[q * BINS + k] + d[q];
+    };
+#pragma unroll 2
+    for (int jj = 0; jj < E / 4; ++jj) {
+      const int k = u + TP * (2 * jj + side);
+      V xk, xm, yk, ym;
+      real::spec_pair(zx, L, k, tab, a.h, xk, xm);
+      real::spec_pair(zy, L, k, tab, a.h, yk, ym);
+      add(k, xk, yk);
+      add(L - k, xm, ym);
+    }
+    if (u == 0 && side == 0) {
+      V xk, xm, yk, ym;
+      real::spec_pair(zx, L, L / 2, tab, a.h, xk, xm);
+      real::spec_pair(zy, L, L / 2, tab, a.h, yk, ym);
+      add(L / 2, xk, yk);
+    }
+  }
+  // the item sums of group g, after a CTA barrier; thread t takes outputs t, t + THREADS, ...
+  static FB_HD void flush(const Args& a, long g, int t, const T* acc) {
+    const int outs = (int)a.w.per_group * BINS;
+    for (int o = t; o < outs; o += THREADS) {
+      const int q = o / BINS, k = o - q * BINS;
+      const long i = g * a.w.per_group + q;
+      if (i >= a.w.total()) return;
+      const long cnt = a.w.count(i), used = cnt < PAIRS ? cnt : PAIRS;
+      const T* y = acc + q * a.w.block * PLANES * BINS + k;
+      T s[PLANES];
+#pragma unroll
+      for (int j = 0; j < PLANES; ++j) s[j] = 0;
+      for (long c = 0; c < used; ++c)
+#pragma unroll
+        for (int j = 0; j < PLANES; ++j) s[j] += y[(c * PLANES + j) * BINS];
+      if (a.w.items > 1) {
+#pragma unroll
+        for (int j = 0; j < PLANES; ++j) real::lin_st(a.part + (i * PLANES + j) * BINS + k, s[j], i);
+      } else if constexpr (COH) {
+        real::lin_st(a.psd + i * BINS + k, real::coherence_out(s[0], s[1], s[2], s[3]), i);
+      } else {
+        real::spec_st(reinterpret_cast<V*>(a.psd) + i * BINS + k, real::csd_out(s[0], s[1], *a.base, 2L * L, (long)k));
+      }
+    }
+  }
+
+  // phase protocol of run_welch_groups: WelchBody's load and detrend, StftBody's stage A, scatter, gather + stage B,
+  // park; cross
+  static constexpr int kPhases = 7;
+  template <int P>
+  static FB_HD void phase(Tile& f, const Args& a, long g, long r, int t, V* smem, T* acc, const TwPair<T>* twa) {
+    if constexpr (P == 0) load(a, g, r, t, smem, acc);
+    else if constexpr (P == 1) Welch::detrend(a, t, smem, sums_base(acc));
+    else if constexpr (P <= 5) Stft::template phase<P - 1>(f, a, 0, t, smem, twa);
+    else cross(a, g, r, t, smem, acc);
+  }
+  // the barrier after phase P over a frame pair in two warps (see above); __syncwarp otherwise
+  static constexpr bool pair_barrier(int p) { return TP == 32 && (p == 5 || p == 6); }
+};
+
+// The device driver of WelchBody and CsdBody: run_onchip_groups' set-up, then per group its rounds, each phase followed
+// by __syncwarp (or, where Body::pair_barrier asks, a barrier over the 64 threads of a frame pair), and the flush
+// between two CTA barriers (the accumulators of every column are complete before it, and it has read them before the
+// next group's round 0 stores).  tools/emulate_common.h has the CPU drivers.
 template <class Cfg, class Body> __device__ __forceinline__ void run_welch_groups(const typename Body::Args& a) {
   using Tile = typename Cfg::Tile;
   using T = typename Body::T;
@@ -615,7 +752,10 @@ template <class Cfg, class Body> __device__ __forceinline__ void run_welch_group
     Body::opaque(g);
     static_for<0, Body::kPhases>([&](auto P) FB_LAMBDA {
       Body::template phase<decltype(P)::value>(f, a, g, r, threadIdx.x, exch, acc, twa);
-      __syncwarp();
+      if constexpr (Body::pair_barrier(decltype(P)::value))
+        asm volatile("bar.sync %0, 64;" ::"r"(1 + (int)threadIdx.x / 64) : "memory");
+      else
+        __syncwarp();
     });
     if (++r == a.w.rounds(g)) {
       __syncthreads();
@@ -630,6 +770,10 @@ template <class Cfg, class Body> __device__ __forceinline__ void run_welch_group
 template <class Cfg, int MINB>
 __global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_welch_kernel(const typename WelchBody<Cfg>::Args a) {
   run_welch_groups<Cfg, WelchBody<Cfg>>(a);
+}
+template <class Cfg, int MINB, bool COH>
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_csd_kernel(const typename CsdBody<Cfg, COH>::Args a) {
+  run_welch_groups<Cfg, CsdBody<Cfg, COH>>(a);
 }
 
 // ---- fused discrete cosine transforms of real rows, N = 2L (real::dct2_pair / dct3_pair, DESIGN.md §4.16) --------

@@ -323,6 +323,11 @@ template <typename T> struct RealOnChipOps {
   // allowed; wq = W^k, k <= L; h, h0 from real::dct_scales
   cudaError_t (*dct)(const T* in, T* out, int type, const void* twa, const cpx<T>* tab, const cpx<T>* wq, size_t batch,
                      T h, T h0, int sms, cudaStream_t);
+  // csd(): welch() on frame pairs (DESIGN.md §4.17): the cross-spectral density (coh false) or coherence items w over
+  // cols / 2 pair columns of the rows of m from x on, row b with y row (y_off + b) mod y_rows; out: cpx<T> or T rows
+  cudaError_t (*csd)(const T* x, const T* y, size_t y_rows, size_t y_off, const T* win, const T* base, int detrend,
+                     bool coh, T* part, void* out, const real::FrameMap& m, const real::WelchItems& w, const void* twa,
+                     const cpx<T>* tab, int sms, cudaStream_t);
 };
 template <typename T> const RealOnChipOps<T>* real_onchip_lookup(size_t l);
 
@@ -405,6 +410,18 @@ class RealPlan {
   cudaError_t welch_host(const T* in, size_t in_len, const T* win, size_t hop, int detrend, int scaling, double fs,
                          T* out, size_t batch);
 
+  // Cross-spectral density and coherence (DESIGN.md §4.17): `batch` rows x of in_len >= N reals, row b paired with y row
+  // b mod y_rows (y_rows >= 1 rows of in_len reals), both framed, detrended and windowed as welch_device.  coh false:
+  // out[b][k] = c_k s / F sum_f conj(X_bf[k]) Y_bf[k], N/2+1 complex values per row; coh true: out[b][k] =
+  // |sum_f conj(X) Y|^2 / (sum_f |X|^2 sum_f |Y|^2), N/2+1 reals per row (scaling and fs unused).  Arguments checked by
+  // the caller.  Out of place only.  Device pointers, on `stream`, never synchronised.
+  cudaError_t cross_device(const T* x, const T* y, size_t y_rows, size_t in_len, const T* win, size_t hop, int detrend,
+                           bool coh, int scaling, double fs, void* out, size_t batch, cudaStream_t stream);
+  // Host pointers: the window is staged once, x rows through stage_rows and each chunk's y rows beside them; the same
+  // bits.
+  cudaError_t cross_host(const T* x, const T* y, size_t y_rows, size_t in_len, const T* win, size_t hop, int detrend,
+                         bool coh, int scaling, double fs, void* out, size_t batch);
+
   // Discrete cosine transform (DESIGN.md §4.16): `batch` rows of N reals -> rows of N reals, scipy.fft.dct(x, type,
   // norm), type 2 or 3, norm real::kDctNorm*; checked by the caller.  in == out allowed.  Device pointers, on `stream`.
   cudaError_t dct_device(const T* in, T* out, size_t batch, int type, int norm, cudaStream_t stream);
@@ -459,6 +476,11 @@ class RealPlan {
   // frames through seg_, then the finish; adds its kernels to launches_
   cudaError_t welch_rows(const T* in, size_t in_len, const T* win, size_t hop, int detrend, T* out, size_t batch,
                          cudaStream_t s);
+  // cross_device after welch_scale (csd only): row b of x with y row (y_off + b) mod y_rows; chunks of rows whose
+  // partials fit part_, each through the fused kernel or chunks of frame pairs through seg_, then the finish; adds its
+  // kernels to launches_
+  cudaError_t cross_rows(const T* x, const T* y, size_t y_rows, size_t y_off, size_t in_len, const T* win, size_t hop,
+                         int detrend, bool coh, void* out, size_t batch, cudaStream_t s);
   // The host-pointer loop (real.cu): chunks of rows of in_row / out_row bytes go H2D, through
   // step(dev_in, dev_out, first_row, rows) on host_stream_, and D2H; launches() then counts all chunks.
   template <class Step>
@@ -487,7 +509,9 @@ class RealPlan {
                                      // spectra behind them)
   DeviceBuffer bands_;               // the filter bands of the last mel call (real::Band per filter row)
   DeviceBuffer welch_base_;          // s / F of the last Welch call (one T)
-  DeviceBuffer part_;                // one chunk of rows of Welch partials (N/2+1 reals per item)
+  DeviceBuffer part_;                // one chunk of rows of Welch partials (N/2+1 reals per item; 2 or 4 planes of
+                                     // them for the csd and coherence)
+  DeviceBuffer stage_y_;             // the y rows of one host-pointer chunk of a csd or coherence call
   cudaStream_t host_stream_ = nullptr;
   std::string kernel_desc_;
 };

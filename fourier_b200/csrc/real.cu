@@ -19,6 +19,10 @@
 // Welch power spectral density (DESIGN.md §4.15): welch_scale_kernel, then per chunk of rows onchip_welch_kernel on the
 // fused path, or chunks of detrended windowed frames gathered into seg_, their spectra by the plan's own rfft behind
 // them and welch_accumulate_kernel into the partials; then welch_finish_kernel unless the fused kernel wrote the rows.
+// Cross-spectral density and coherence (DESIGN.md §4.17): Welch's steps on frame pairs: welch_scale_kernel (csd only),
+// then per chunk of rows onchip_csd_kernel, or chunks of x frames and their y frames gathered into seg_
+// (csd_gather_kernel), their spectra by the plan's own rfft behind them and cross_accumulate_kernel into the partials;
+// then cross_finish_kernel unless the fused kernel wrote the rows.
 // Discrete cosine transforms (DESIGN.md §4.16): onchip_dct_kernel on the fused path; otherwise per chunk of rows an O(N)
 // kernel into seg_, the inner plan in place there and an O(N) kernel into the output: dct_permute_kernel, Fft and
 // dct_untangle_kernel (type 2) or dct_tangle_kernel, UnscaledIfft and dct_unpermute_kernel (type 3) at half length;
@@ -201,6 +205,25 @@ welch_scale_kernel(const T* __restrict__ win, long n, int scaling, double fs, lo
   }
   if (threadIdx.x == 0) *base = (T)real::welch_base(s1[0], s2[0], scaling, fs, frames);
 }
+// one frame of a gather: its mean by a fixed tree in shared memory (detrend constant), then (x - mu) w into dst
+template <typename T>
+__device__ __forceinline__ void gather_detrended(const T* __restrict__ src, const T* __restrict__ win, T* __restrict__ dst,
+                                                 long n, int detrend, T* part) {
+  T mu = 0;
+  if (detrend == real::kDetrendConstant) {
+    T s = 0;
+    for (long p = threadIdx.x; p < n; p += kThreads) s += src[p];
+    part[threadIdx.x] = s;
+    __syncthreads();
+    for (int w = kThreads / 2; w > 0; w /= 2) {
+      if ((int)threadIdx.x < w) part[threadIdx.x] += part[threadIdx.x + w];
+      __syncthreads();
+    }
+    mu = part[0] / (T)n;
+    __syncthreads();
+  }
+  for (long p = threadIdx.x; p < n; p += kThreads) dst[p] = (src[p] - mu) * win[p];
+}
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
 welch_gather_kernel(const T* __restrict__ in, const T* __restrict__ win, T* __restrict__ seg, const real::FrameMap m,
@@ -208,21 +231,7 @@ welch_gather_kernel(const T* __restrict__ in, const T* __restrict__ win, T* __re
   __shared__ T part[kThreads];
   for (long q = blockIdx.x; q < nframes; q += gridDim.x) {
     const long g = m.g0 + q, b = m.row_of(g);
-    const T* src = in + (b - m.r0) * m.in_ld + m.start(g, b);
-    T mu = 0;
-    if (detrend == real::kDetrendConstant) {
-      T s = 0;
-      for (long p = threadIdx.x; p < m.n; p += kThreads) s += src[p];
-      part[threadIdx.x] = s;
-      __syncthreads();
-      for (int w = kThreads / 2; w > 0; w /= 2) {
-        if ((int)threadIdx.x < w) part[threadIdx.x] += part[threadIdx.x + w];
-        __syncthreads();
-      }
-      mu = part[0] / (T)m.n;
-      __syncthreads();
-    }
-    for (long p = threadIdx.x; p < m.n; p += kThreads) seg[q * m.n + p] = (src[p] - mu) * win[p];
+    gather_detrended(in + (b - m.r0) * m.in_ld + m.start(g, b), win, seg + q * m.n, m.n, detrend, part);
   }
 }
 template <typename T>
@@ -244,6 +253,43 @@ welch_finish_kernel(const T* __restrict__ part, long items, long n, const T* __r
   for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
     const long b = g / bins;
     real::welch_finish_one(part, items, n, s, out, b, g - b * bins);
+  }
+}
+// Cross-spectral density and coherence (DESIGN.md §4.17) on frame pairs.  gather: welch_gather_kernel's frames of x
+// into seg and those of their y rows (row b of the rows' FrameMap with y row (y_off + b) mod y_rows) nframes frames
+// behind.  accumulate: welch_accumulate_kernel's threads over the item's x and y spectra.  finish: one thread per
+// (row, bin).
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+csd_gather_kernel(const T* __restrict__ x, const T* __restrict__ y, long y_rows, long y_off,
+                  const T* __restrict__ win, T* __restrict__ seg, const real::FrameMap m, long nframes, int detrend) {
+  __shared__ T part[kThreads];
+  for (long q = blockIdx.x; q < nframes; q += gridDim.x) {
+    const long g = m.g0 + q, b = m.row_of(g), t0 = m.start(g, b);
+    gather_detrended(x + (b - m.r0) * m.in_ld + t0, win, seg + q * m.n, m.n, detrend, part);
+    gather_detrended(y + ((y_off + b) % y_rows) * m.in_ld + t0, win, seg + (nframes + q) * m.n, m.n, detrend, part);
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+cross_accumulate_kernel(const cpx<T>* __restrict__ specx, const cpx<T>* __restrict__ specy, const real::WelchItems w,
+                        long bins, long q0, long nq, long i0, long ni, int planes, T* __restrict__ part) {
+  const long total = ni * bins;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long i = i0 + g / bins, k = g - (g / bins) * bins, b = i / w.items;
+    real::cross_accumulate_one(specx, specy, bins, q0, nq, b * w.frames + (i - b * w.items) * w.block, w.count(i),
+                               planes, part, i, k);
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+cross_finish_kernel(const T* __restrict__ part, long items, long n, const T* __restrict__ base, bool coh,
+                    void* __restrict__ out, long rows) {
+  const long bins = n / 2 + 1, total = rows * bins;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / bins;
+    if (coh) real::coherence_finish_one(part, items, n, (T*)out, b, g - b * bins);
+    else real::csd_finish_one(part, items, n, *base, (cpx<T>*)out, b, g - b * bins);
   }
 }
 
@@ -1021,6 +1067,107 @@ cudaError_t RealPlan<T>::dct_host(const T* in, T* out, size_t batch, int type, i
   return stage_rows(in, out, batch, n_ * sizeof(T), n_ * sizeof(T), [&](const void* din, void* dout, size_t, size_t nb) {
     return dct_device((const T*)din, (T*)dout, nb, type, norm, host_stream_);
   });
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::cross_rows(const T* x, const T* y, size_t y_rows, size_t y_off, size_t in_len, const T* win,
+                                    size_t hop, int detrend, bool coh, void* out, size_t batch, cudaStream_t s) {
+  const real::FrameMap m = real::frame_map((long)n_, (long)in_len, (long)hop, real::kStftNone);
+  const size_t bins = n_ / 2 + 1, frames = (size_t)m.frames;
+  const size_t planes = coh ? real::kCoherencePlanes : real::kCsdPlanes, out_row = bins * (coh ? sizeof(T) : sizeof(C));
+  const bool fused = path_ == Path::kRealFused;
+  const long cols = fused ? fused_->cols / 2 : 1;
+  const size_t items = (size_t)real::welch_items(m.frames, cols, 1).items;
+  // the fused kernel writes a row of one item itself; every other row goes through partials and the finish
+  const bool direct = fused && items == 1;
+  const size_t rows = direct ? batch : scratch_chunk(batch, items * planes * bins * sizeof(T));
+  if (!direct) FB_CHECK(part_.reserve(rows * items * planes * bins * sizeof(T)));
+  T* part = (T*)part_.data();
+  const T* base = (const T*)welch_base_.data();
+  unsigned long long count = launches_;
+  for (size_t r0 = 0; r0 < batch; r0 += rows) {
+    const size_t nr = std::min(rows, batch - r0), yo = (y_off + r0) % y_rows;
+    const real::WelchItems w = real::welch_items(m.frames, cols, (long)nr);
+    const T* xr = x + r0 * in_len;
+    void* o = (char*)out + r0 * out_row;
+    if (fused) {
+      FB_CHECK(fused_->csd(xr, y, y_rows, yo, win, base, detrend, coh, part, o, m, w, twa_.data(),
+                           (const C*)tab_.data(), sm_count_, s));
+      count += 1;
+    } else {
+      // chunks of frame pairs through seg_: the x frames, then their y frames, their spectra from the plan's own rfft
+      // behind them, and the items with frames in the chunk accumulated from there
+      const size_t total = nr * frames;
+      const size_t chunk = scratch_chunk(total, 2 * (n_ * sizeof(T) + bins * sizeof(C)));
+      const size_t spec_off = (2 * chunk * n_ * sizeof(T) + 255) / 256 * 256;
+      FB_CHECK(seg_.reserve(spec_off + 2 * chunk * bins * sizeof(C)));
+      T* seg = (T*)seg_.data();
+      C* spec = (C*)((char*)seg_.data() + spec_off);
+      for (size_t q0 = 0; q0 < total; q0 += chunk) {
+        const size_t nq = std::min(chunk, total - q0);
+        real::FrameMap mc = m;
+        mc.g0 = (long)q0;
+        csd_gather_kernel<T><<<(unsigned)std::min<size_t>(nq, 132u * 32u), kThreads, 0, s>>>(
+            xr, y, (long)y_rows, (long)yo, win, seg, mc, (long)nq, detrend);
+        FB_CHECK(cudaGetLastError());
+        FB_CHECK(exec_device(true, seg, spec, 2 * nq, kFft, s));
+        count += 2 + launches_;
+        auto item_of = [&](size_t q) { return (q / frames) * items + (q % frames) / (size_t)w.block; };
+        const size_t i0 = item_of(q0), ni = item_of(q0 + nq - 1) + 1 - i0;
+        cross_accumulate_kernel<T><<<grid_for(ni * bins), kThreads, 0, s>>>(
+            spec, spec + nq * bins, w, (long)bins, (long)q0, (long)nq, (long)i0, (long)ni, (int)planes, part);
+        FB_CHECK(cudaGetLastError());
+      }
+    }
+    if (!direct) {
+      cross_finish_kernel<T><<<grid_for(nr * bins), kThreads, 0, s>>>(part, (long)items, (long)n_, base, coh, o,
+                                                                       (long)nr);
+      FB_CHECK(cudaGetLastError());
+      count += 1;
+    }
+  }
+  launches_ = count;
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::cross_device(const T* x, const T* y, size_t y_rows, size_t in_len, const T* win, size_t hop,
+                                      int detrend, bool coh, int scaling, double fs, void* out, size_t batch,
+                                      cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  if (!coh) FB_CHECK(welch_scale(win, scaling, fs, frame_count(in_len, hop, real::kStftNone), s));
+  return cross_rows(x, y, y_rows, 0, in_len, win, hop, detrend, coh, out, batch, s);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::cross_host(const T* x, const T* y, size_t y_rows, size_t in_len, const T* win, size_t hop,
+                                    int detrend, bool coh, int scaling, double fs, void* out, size_t batch) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  const T* dwin;
+  FB_CHECK(stage_consts(win, n_ * sizeof(T), &dwin));
+  if (!coh) FB_CHECK(welch_scale(dwin, scaling, fs, frame_count(in_len, hop, real::kStftNone), host_stream_));
+  const size_t row = in_len * sizeof(T), bins = n_ / 2 + 1;
+  FB_CHECK(stage_rows(x, out, batch, row, bins * (coh ? sizeof(T) : sizeof(C)),
+                      [&](const void* din, void* dout, size_t b0, size_t nb) {
+                        // y rows (b0 + j) mod y_rows, j < cnt, in one or two runs: row b of the chunk pairs with j =
+                        // b mod cnt
+                        const size_t cnt = std::min(nb, y_rows), first = b0 % y_rows;
+                        const size_t run = std::min(cnt, y_rows - first);
+                        FB_CHECK(stage_y_.reserve(cnt * row));
+                        FB_CHECK(cudaMemcpyAsync(stage_y_.data(), y + first * in_len, run * row,
+                                                 cudaMemcpyHostToDevice, host_stream_));
+                        if (run < cnt)
+                          FB_CHECK(cudaMemcpyAsync((char*)stage_y_.data() + run * row, y, (cnt - run) * row,
+                                                   cudaMemcpyHostToDevice, host_stream_));
+                        return cross_rows((const T*)din, (const T*)stage_y_.data(), cnt, 0, in_len, dwin, hop, detrend,
+                                          coh, dout, nb, host_stream_);
+                      }));
+  launches_ += coh ? 0 : 1;
+  return cudaSuccess;
 }
 
 template class RealPlan<float>;

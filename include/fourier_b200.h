@@ -411,6 +411,54 @@ int fourier_b200_dct_async_float(struct fourier_b200_rfft_float *plan, const flo
 int fourier_b200_dct_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev, double *out_dev,
                                   size_t batch, int type, int norm, void *cuda_stream);
 
+/* ---- cross-spectral density and coherence of real rows ----
+ * On a real plan of length N, for `batch` rows x_b of in_len >= N reals (row b at element b*in_len) and y_rows >= 1
+ * rows of in_len reals y: row b of x pairs with y row b mod y_rows (1: one y for every row; batch: one y per row).  Both
+ * are framed as by fourier_b200_welch_*: X_bf = rfft(w * (x_bf - mu_bf)), Y_bf = rfft(w * (y_bf - nu_bf)), the frame
+ * means taken off with FOURIER_B200_DETREND_CONSTANT, F = 1 + (in_len - N) / hop frames.  Then, for k <= N/2,
+ *   csd:        out[b][k] = c_k * s / F * sum_{f < F} conj(X_bf[k]) * Y_bf[k]             (complex),
+ *   coherence:  out[b][k] = |sum_f conj(X_bf[k]) Y_bf[k]|^2 / (sum_f |X_bf[k]|^2 * sum_f |Y_bf[k]|^2)   (real),
+ * with c_k and s as in fourier_b200_welch_*.  That is scipy.signal.csd(x, y, fs, window=w, nperseg=N,
+ * noverlap=N-hop, detrend=..., scaling=...)[1] and scipy.signal.coherence(x, y, fs, window=w, nperseg=N,
+ * noverlap=N-hop, detrend=...)[1].  The csd writes N/2+1 complex values per row in the rfft layout (row b from complex
+ * element b*(N/2+1) on), with Im exactly +0 at bins 0 and N/2; the coherence N/2+1 reals per row, NaN where the
+ * denominator is 0 (0/0, as scipy gives, e.g. for a row of zeros).
+ * A row's bits depend only on its x row, its y row, the window, hop, detrend, scaling, fs and the plan: not on the batch,
+ * the other rows, y_rows repetition, host or device memory or the stream.  Launches: the csd makes at most 3 on the
+ * real_fused path while the rows' partials fit one scratch chunk, the coherence at most 2 (no window sums).
+ * Refused with cudaErrorInvalidValue and a message: a NULL argument, y_rows == 0, hop == 0, in_len == 0, detrend other
+ * than 0 and 1, for the csd scaling other than 0 and 1 and fs not finite and > 0 (these also when batch == 0, which
+ * otherwise succeeds and launches nothing), in_len < N, the output overlapping the x rows, the y rows or the window
+ * (out of place only; x and y may overlap, y == x is allowed), and a mix of host and device buffers in the synchronous
+ * calls.  Device base pointers of x, y and the output must be 16-byte aligned (cudaErrorMisalignedAddress).  Host memory
+ * is staged through the plan's buffers (the window once, whole x rows in chunks with the y rows they pair with) and gives
+ * the same bits as device memory.  The _async calls take device memory, are enqueued on `cuda_stream` and never
+ * synchronise the host. */
+int fourier_b200_csd_float(struct fourier_b200_rfft_float *plan, const float *x, const float *y, size_t y_rows,
+                           size_t in_len, const float *window, size_t hop, int detrend, int scaling, double fs,
+                           void *out, size_t batch);
+int fourier_b200_csd_double(struct fourier_b200_rfft_double *plan, const double *x, const double *y, size_t y_rows,
+                            size_t in_len, const double *window, size_t hop, int detrend, int scaling, double fs,
+                            void *out, size_t batch);
+int fourier_b200_csd_async_float(struct fourier_b200_rfft_float *plan, const float *x_dev, const float *y_dev,
+                                 size_t y_rows, size_t in_len, const float *window_dev, size_t hop, int detrend,
+                                 int scaling, double fs, void *out_dev, size_t batch, void *cuda_stream);
+int fourier_b200_csd_async_double(struct fourier_b200_rfft_double *plan, const double *x_dev, const double *y_dev,
+                                  size_t y_rows, size_t in_len, const double *window_dev, size_t hop, int detrend,
+                                  int scaling, double fs, void *out_dev, size_t batch, void *cuda_stream);
+int fourier_b200_coherence_float(struct fourier_b200_rfft_float *plan, const float *x, const float *y, size_t y_rows,
+                                 size_t in_len, const float *window, size_t hop, int detrend, float *out,
+                                 size_t batch);
+int fourier_b200_coherence_double(struct fourier_b200_rfft_double *plan, const double *x, const double *y,
+                                  size_t y_rows, size_t in_len, const double *window, size_t hop, int detrend,
+                                  double *out, size_t batch);
+int fourier_b200_coherence_async_float(struct fourier_b200_rfft_float *plan, const float *x_dev, const float *y_dev,
+                                       size_t y_rows, size_t in_len, const float *window_dev, size_t hop, int detrend,
+                                       float *out_dev, size_t batch, void *cuda_stream);
+int fourier_b200_coherence_async_double(struct fourier_b200_rfft_double *plan, const double *x_dev,
+                                        const double *y_dev, size_t y_rows, size_t in_len, const double *window_dev,
+                                        size_t hop, int detrend, double *out_dev, size_t batch, void *cuda_stream);
+
 const char *fourier_b200_last_error(void);
 const char *fourier_b200_version(void);
 

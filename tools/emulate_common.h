@@ -61,6 +61,41 @@ static void run_welch_body(const typename Body::Args& a, const TwPair<typename B
   }
 }
 
+// The CPU driver of run_welch_groups that also mirrors its barriers between warps (CsdBody): per group, each warp in
+// ascending order runs its own (round, phase) steps, lane by lane per phase (the __syncwarp), until it has run a phase
+// that Body::pair_barrier marks (the barrier over a frame pair's two warps) or the group ends; the warps take turns
+// until all have finished the group, then the flush runs for every thread (the CTA barrier).  A warp that read another
+// warp's shared memory without a barrier ordering the two would see it stale here.
+template <class Body, class Tile, class LAY>
+static void run_warp_body(const typename Body::Args& a, const TwPair<typename Body::T>* twa) {
+  using T = typename Body::T;
+  std::vector<typename Tile::V> smem(Tile::template smem_elems<LAY>());
+  std::vector<T> acc(Body::ACC_BYTES / sizeof(T));
+  std::vector<Tile> thr(Tile::THREADS);
+  constexpr int warps = (Tile::THREADS + 31) / 32;
+  for (long g = 0; g < a.w.groups; ++g) {
+    const long steps = a.w.rounds(g) * Body::kPhases;
+    std::vector<long> pos(warps, 0);
+    for (bool left = true; left;) {
+      left = false;
+      for (int w = 0; w < warps; ++w) {
+        for (bool stop = false; !stop && pos[w] < steps; ++pos[w]) {
+          const long r = pos[w] / Body::kPhases;
+          const int p = (int)(pos[w] % Body::kPhases);
+          static_for<0, Body::kPhases>([&](auto P) {
+            if (decltype(P)::value != p) return;
+            for (int t = 32 * w; t < std::min(32 * (w + 1), Tile::THREADS); ++t)
+              Body::template phase<decltype(P)::value>(thr[t], a, g, r, t, smem.data(), acc.data(), twa);
+          });
+          stop = Body::pair_barrier(p);
+        }
+        left |= pos[w] < steps;
+      }
+    }
+    for (int t = 0; t < Tile::THREADS; ++t) Body::flush(a, g, t, acc.data());
+  }
+}
+
 // every on-chip size class of precision T (onchip_configs.cuh), smallest first: f(class)
 template <typename T, class F> static void for_each_onchip(F&& f) {
   for (size_t l = 1; l <= ((size_t)1 << 16); l *= 2) onchip::visit_onchip<T>(l, f);
