@@ -24,6 +24,9 @@ reference's operator interface name for name:
     (no counterpart)                                      RealFft.mel_spectrogram: |stft|^p through a caller's
                                                             mel filter bank (torchaudio's MelSpectrogram,
                                                             frames frame-major), the spectrum kept on chip
+    (no counterpart)                                      RealFft.mfcc: log mels, a top_db clamp and a DCT matrix
+                                                            (torchaudio's MFCC, librosa's mfcc, Whisper's
+                                                            log-mel), the mels kept on chip
     (no counterpart)                                      RealFft.welch: Welch's power spectral density of real
                                                             rows (scipy.signal.welch), frames summed on chip
     (no counterpart)                                      RealFft.csd / coherence: cross-spectral density and
@@ -39,6 +42,7 @@ allowed: shape (..., size) means prod(...) independent transforms.  There is no 
 """
 import ctypes
 import enum
+import math
 
 import numpy as np
 
@@ -464,6 +468,72 @@ class RealFft:
             return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
         self._call("mel_spectrogram", "mel spectrogram", di, si, pi, in_len, pw, hop, boundary, int(power), pf, n_mels,
                    po, batch)
+
+    def mfcc(self, input, window, hop, filters, dct, output, power=2, center=True, pad_mode="reflect",
+             log_scale=10.0 / math.log(10.0), log_floor=1e-10, log_offset=0.0, top_db=80.0, top_db_rows=1, bias=0.0):
+        """MFCC or log-mel spectrogram of every row of `input` (shape (..., L)), from mel_spectrogram's mels
+        mel[..., f, m] (same framing, window, power and filters), all in the plan's precision:
+        lm = log_scale * ln(max(mel + log_offset, log_floor)); with top_db not None, lc = max(lm, max_g(lm) - top_db)
+        where max_g is taken over clamp group g, top_db_rows consecutive rows of the flattened leading shape (their
+        count must be a multiple of it), all their frames and mels; else lc = lm.  Then output[..., f, j] = bias +
+        sum_m lc[..., f, m] * dct[m, j] (ascending m), or lc + bias with dct None (the log-mel spectrogram).  `dct` has
+        shape (n_mels, n_out): torchaudio's create_dct(n_mfcc, n_mels, "ortho"), or librosa's
+        scipy.fft.dct(np.eye(n_mels), norm="ortho")[:, :n_mfcc]; fold a lifter into its columns.  `output` has shape
+        (..., F, n_out), frame-major: the transpose of torchaudio's layout.
+        The defaults are torchaudio.transforms.MFCC(log_mels=False) for one-channel input; for input (..., C, L) pass
+        top_db_rows = C, as torchaudio takes the max over each item's channels.  MFCC(log_mels=True): log_scale=1,
+        log_floor = the smallest normal of the dtype, log_offset=1e-6, top_db=None.  librosa.feature.mfcc: top_db_rows
+        = all rows.  Whisper's log-mel: log_scale=1/(4 ln 10), log_floor=1e-10, top_db=2, dct=None, bias=1; Whisper
+        drops the last frame before its max and this takes the max over all F frames, so the two agree on frames
+        0 .. F-2 unless the last frame holds the row's maximum.  The mels stay on chip where the plan's path allows.
+        Out of place only."""
+        self._check_resolved(input, window, filters, dct, output)
+        if power not in (1, 2):
+            raise ValueError(f"power must be 1 or 2, got {power!r}")
+        log_scale, log_floor, log_offset, bias = float(log_scale), float(log_floor), float(log_offset), float(bias)
+        if not math.isfinite(log_offset):
+            raise ValueError(f"log_offset must be finite, got {log_offset!r}")
+        if not math.isfinite(bias):
+            raise ValueError(f"bias must be finite, got {bias!r}")
+        if not (math.isfinite(log_floor) and log_floor > 0):
+            raise ValueError(f"log_floor must be finite and positive, got {log_floor!r}")
+        if not (math.isfinite(log_scale) and log_scale > 0):
+            raise ValueError(f"log_scale must be finite and positive, got {log_scale!r}")
+        top_db = math.inf if top_db is None else float(top_db)
+        if not top_db >= 0:
+            raise ValueError(f"top_db must be None or >= 0, got {top_db!r}")
+        top_db_rows = int(top_db_rows)
+        if top_db_rows < 1:
+            raise ValueError(f"top_db_rows must be at least 1, got {top_db_rows}")
+        hop, boundary, in_len, frames, (pi, li, di, si), (pw, dw) = self._framing(input, window, hop, center, pad_mode)
+        n = self._size
+        if getattr(filters, "ndim", 0) != 2:
+            raise ValueError(f"filters must have shape (n_mels, {n // 2 + 1})")
+        pf, lf, df, _ = self._describe(filters, "real", last=n // 2 + 1)
+        n_mels = lf[0]
+        if n_mels < 1:
+            raise ValueError("filters must hold at least one mel row")
+        if dct is None:
+            n_out, pd, dd = n_mels, None, di
+        else:
+            if getattr(dct, "ndim", 0) != 2 or dct.shape[0] != n_mels or dct.shape[1] < 1:
+                raise ValueError(f"dct must have shape ({n_mels}, n_out) with n_out >= 1")
+            n_out = int(dct.shape[1])
+            pd, _, dd, _ = self._describe(dct, "real", last=n_out)
+        if getattr(output, "ndim", 0) < 2 or output.shape[-2] != frames:
+            raise ValueError(f"output must have shape (..., {frames}, {n_out}) (F = {frames} frames)")
+        po, lo, do_, _ = self._describe(output, "real", last=n_out)
+        if li != lo[:-1]:
+            raise ValueError(f"input and output leading shapes differ: {li} and {lo[:-1]}")
+        if not (di == dw == df == dd == do_):
+            raise ValueError("input, window, filters, dct and output must all be host or all be device buffers")
+        batch = int(np.prod(li, dtype=np.int64))
+        if math.isfinite(top_db) and batch % top_db_rows:
+            raise ValueError(f"{batch} rows do not form whole clamp groups of top_db_rows = {top_db_rows}")
+        if batch == 0:
+            return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
+        self._call("mfcc", "mfcc", di, si, pi, in_len, pw, hop, boundary, int(power), pf, n_mels, log_offset,
+                   log_floor, log_scale, top_db, top_db_rows, pd, n_out, bias, po, batch)
 
     DCT_NORMS = {"backward": 0, "ortho": 1, "forward": 2}
 

@@ -34,6 +34,7 @@ EXTENSION_SYMBOLS = (
     + [f"fourier_b200_linear_convolve_real_{op}{t}" for t in ("float", "double") for op in ("", "async_")]
     + [f"fourier_b200_{fn}_{op}{t}" for fn in ("stft", "istft") for t in ("float", "double") for op in ("", "async_")]
     + [f"fourier_b200_mel_spectrogram_{op}{t}" for t in ("float", "double") for op in ("", "async_")]
+    + [f"fourier_b200_mfcc_{op}{t}" for t in ("float", "double") for op in ("", "async_")]
     + [f"fourier_b200_welch_{op}{t}" for t in ("float", "double") for op in ("", "async_")]
     + [f"fourier_b200_{fn}_{op}{t}" for fn in ("csd", "coherence") for t in ("float", "double") for op in ("", "async_")]
     + [f"fourier_b200_dct_{op}{t}" for t in ("float", "double") for op in ("", "async_")])
@@ -48,7 +49,7 @@ def load():
             f"{LIB_PATH} is missing: build it with `python -m fourier_b200.build` "
             "(nvcc, sm_90a). fourier_b200 has no CPU or PyTorch fallback.")
     L = ctypes.CDLL(LIB_PATH)
-    vp, sz, ci = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int
+    vp, sz, ci, dbl = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_double
     for t in ("float", "double"):
         getattr(L, f"fourier_create_{t}").restype = vp
         getattr(L, f"fourier_create_{t}").argtypes = [sz]
@@ -95,6 +96,9 @@ def load():
         getattr(L, f"fourier_b200_istft_async_{t}").argtypes = [vp, vp, sz, vp, sz, ci, vp, sz, sz, vp]
         getattr(L, f"fourier_b200_mel_spectrogram_{t}").argtypes = [vp, vp, sz, vp, sz, ci, ci, vp, sz, vp, sz]
         getattr(L, f"fourier_b200_mel_spectrogram_async_{t}").argtypes = [vp, vp, sz, vp, sz, ci, ci, vp, sz, vp, sz, vp]
+        mfcc = [vp, vp, sz, vp, sz, ci, ci, vp, sz, dbl, dbl, dbl, dbl, sz, vp, sz, dbl, vp, sz]
+        getattr(L, f"fourier_b200_mfcc_{t}").argtypes = mfcc
+        getattr(L, f"fourier_b200_mfcc_async_{t}").argtypes = mfcc + [vp]
         getattr(L, f"fourier_b200_welch_{t}").argtypes = [vp, vp, sz, vp, sz, ci, ci, ctypes.c_double, vp, sz]
         getattr(L, f"fourier_b200_welch_async_{t}").argtypes = [vp, vp, sz, vp, sz, ci, ci, ctypes.c_double, vp, sz, vp]
         getattr(L, f"fourier_b200_csd_{t}").argtypes = [vp, vp, vp, sz, sz, vp, sz, ci, ci, ctypes.c_double, vp, sz]

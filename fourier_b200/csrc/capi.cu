@@ -336,6 +336,64 @@ int mel_exec(void* plan, const T* in, size_t in_len, const T* window, size_t hop
       });
 }
 
+// MFCC and log-mel spectrogram of real rows: mel_exec's rules, plus n_out, the matrix and the log, clamp and bias
+// scalars checked before the plan is touched; then, with the clamp, the batch against top_db_rows; the window, filters
+// and matrix kept apart from the output.
+template <typename T>
+int mfcc_exec(void* plan, const T* in, size_t in_len, const T* window, size_t hop, int boundary, int power,
+              const T* filters, size_t n_mels, double log_offset, double log_floor, double log_scale, double top_db,
+              size_t top_db_rows, const T* dct, size_t n_out, double bias, T* out, size_t batch, bool async,
+              void* stream) {
+  if (!plan || !in || !window || !filters || !out) {
+    fb200::set_last_error("null argument");
+    return (int)cudaErrorInvalidValue;
+  }
+  const bool clamp = std::isfinite(top_db);
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  if (!check_frames(p, in_len, hop, boundary,
+                    power != 1 && power != 2                          ? "power must be 1 or 2"
+                    : n_mels == 0                                     ? "n_mels must be at least 1"
+                    : n_out == 0                                      ? "n_out must be at least 1"
+                    : !dct && n_out != n_mels                         ? "dct NULL (the identity) needs n_out == n_mels"
+                    : !std::isfinite(log_offset)                      ? "log_offset must be finite"
+                    : !std::isfinite(bias)                            ? "bias must be finite"
+                    : !(std::isfinite(log_floor) && log_floor > 0)    ? "log_floor must be finite and positive"
+                    : !(std::isfinite(log_scale) && log_scale > 0)    ? "log_scale must be finite and positive"
+                    : !(top_db >= 0)                                  ? "top_db must be >= 0 (+inf: no clamp)"
+                    : top_db_rows == 0                                ? "top_db_rows must be at least 1"
+                    : clamp && batch % top_db_rows != 0               ? "batch must be a multiple of top_db_rows"
+                                                                      : nullptr))
+    return (int)cudaErrorInvalidValue;
+  const size_t n = p->size();
+  return run_call(
+      "mfcc", async, stream,
+      [&] {
+        if (batch == 0)
+          return (int)p->mfcc_device(in, in_len, window, hop, boundary, power, filters, n_mels, log_offset, log_floor,
+                                     log_scale, top_db, top_db_rows, dct, n_out, bias, out, 0, nullptr);
+        const size_t in_bytes = batch * in_len * sizeof(T);
+        const size_t out_bytes = batch * p->mel_row_bytes(in_len, hop, boundary, n_out);
+        if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, n * sizeof(T), out, out_bytes) ||
+            ranges_meet(filters, n_mels * (n / 2 + 1) * sizeof(T), out, out_bytes) ||
+            (dct && ranges_meet(dct, n_mels * n_out * sizeof(T), out, out_bytes))) {
+          fb200::set_last_error("input, window, filters or dct and output overlap (mfcc is out of place only)");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {in, window, filters, dct ? (const void*)dct : (const void*)out, out},
+      "input, window, filters, dct and output must all be host or all be device memory",
+      [&] {
+        return p->mfcc_host(in, in_len, window, hop, boundary, power, filters, n_mels, log_offset, log_floor, log_scale,
+                            top_db, top_db_rows, dct, n_out, bias, out, batch);
+      },
+      {in, out},
+      [&](cudaStream_t s) {
+        return p->mfcc_device(in, in_len, window, hop, boundary, power, filters, n_mels, log_offset, log_floor,
+                              log_scale, top_db, top_db_rows, dct, n_out, bias, out, batch, s);
+      });
+}
+
 // Welch power spectral density of real rows: stft_exec's rules with boundary none, plus detrend, scaling and fs checked
 // before the plan is touched.
 template <typename T>
@@ -781,6 +839,38 @@ int fourier_b200_mel_spectrogram_async_double(fourier_b200_rfft_double* plan, co
                                               void* stream) {
   return mel_exec<double>(plan, in_dev, in_len, window_dev, hop, boundary, power, filters_dev, n_mels, out_dev, batch,
                           true, stream);
+}
+
+int fourier_b200_mfcc_float(fourier_b200_rfft_float* plan, const float* in, size_t in_len, const float* window,
+                            size_t hop, int boundary, int power, const float* filters, size_t n_mels, double log_offset,
+                            double log_floor, double log_scale, double top_db, size_t top_db_rows, const float* dct,
+                            size_t n_out, double bias, float* out, size_t batch) {
+  return mfcc_exec<float>(plan, in, in_len, window, hop, boundary, power, filters, n_mels, log_offset, log_floor,
+                          log_scale, top_db, top_db_rows, dct, n_out, bias, out, batch, false, nullptr);
+}
+int fourier_b200_mfcc_double(fourier_b200_rfft_double* plan, const double* in, size_t in_len, const double* window,
+                             size_t hop, int boundary, int power, const double* filters, size_t n_mels,
+                             double log_offset, double log_floor, double log_scale, double top_db, size_t top_db_rows,
+                             const double* dct, size_t n_out, double bias, double* out, size_t batch) {
+  return mfcc_exec<double>(plan, in, in_len, window, hop, boundary, power, filters, n_mels, log_offset, log_floor,
+                           log_scale, top_db, top_db_rows, dct, n_out, bias, out, batch, false, nullptr);
+}
+int fourier_b200_mfcc_async_float(fourier_b200_rfft_float* plan, const float* in_dev, size_t in_len,
+                                  const float* window_dev, size_t hop, int boundary, int power,
+                                  const float* filters_dev, size_t n_mels, double log_offset, double log_floor,
+                                  double log_scale, double top_db, size_t top_db_rows, const float* dct_dev,
+                                  size_t n_out, double bias, float* out_dev, size_t batch, void* stream) {
+  return mfcc_exec<float>(plan, in_dev, in_len, window_dev, hop, boundary, power, filters_dev, n_mels, log_offset,
+                          log_floor, log_scale, top_db, top_db_rows, dct_dev, n_out, bias, out_dev, batch, true, stream);
+}
+int fourier_b200_mfcc_async_double(fourier_b200_rfft_double* plan, const double* in_dev, size_t in_len,
+                                   const double* window_dev, size_t hop, int boundary, int power,
+                                   const double* filters_dev, size_t n_mels, double log_offset, double log_floor,
+                                   double log_scale, double top_db, size_t top_db_rows, const double* dct_dev,
+                                   size_t n_out, double bias, double* out_dev, size_t batch, void* stream) {
+  return mfcc_exec<double>(plan, in_dev, in_len, window_dev, hop, boundary, power, filters_dev, n_mels, log_offset,
+                           log_floor, log_scale, top_db, top_db_rows, dct_dev, n_out, bias, out_dev, batch, true,
+                           stream);
 }
 
 int fourier_b200_welch_float(fourier_b200_rfft_float* plan, const float* in, size_t in_len, const float* window,

@@ -103,6 +103,8 @@ struct OnChipImpl {
     if ((e = allow_smem(onchip::onchip_lconv_kernel<Cfg<true>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_stft_kernel<Cfg<true>, MINB>))) return e;
     if ((e = allow_smem(onchip::onchip_mel_kernel<Cfg<true>, MINB>))) return e;
+    if ((e = allow_smem(onchip::onchip_mfcc_kernel<Cfg<true>, MINB, true>))) return e;
+    if ((e = allow_smem(onchip::onchip_mfcc_kernel<Cfg<true>, MINB, false>))) return e;
     if ((e = allow_smem(onchip::onchip_dct_kernel<Cfg<true>, MINB, 2>))) return e;
     if ((e = allow_smem(onchip::onchip_dct_kernel<Cfg<true>, MINB, 3>))) return e;
     if ((e = cudaFuncSetAttribute(onchip::onchip_csd_kernel<Cfg<true>, minb_csd(false), false>,
@@ -188,6 +190,24 @@ struct OnChipImpl {
     a.power = power;
     return launch(onchip::onchip_mel_kernel<Cfg<true>, MINB>, a, nframes, sms, s);
   }
+  static cudaError_t mfcc(const T* in, const T* win, const T* filters, const real::Band* bands, size_t n_mels,
+                          int power, const real::MfccArgs<T>& p, bool max_sweep, T* out, const real::FrameMap& m,
+                          size_t nframes, const void* twa, const cpx<T>* tab, int sms, cudaStream_t s) {
+    onchip::MfccArgs<Cfg<true>> a;
+    static_cast<typename onchip::RealBody<Cfg<true>>::Args&>(a) = {
+        nullptr, nullptr, (const TwPair<T>*)twa, tab, (long)nframes, (T)0.5};
+    a.x = in;
+    a.win = win;
+    a.m = m;
+    a.mel = out;
+    a.filters = filters;
+    a.bands = bands;
+    a.n_mels = (long)n_mels;
+    a.power = power;
+    a.p = p;
+    if (max_sweep) return launch(onchip::onchip_mfcc_kernel<Cfg<true>, MINB, true>, a, nframes, sms, s);
+    return launch(onchip::onchip_mfcc_kernel<Cfg<true>, MINB, false>, a, nframes, sms, s);
+  }
   static cudaError_t stft(const T* in, const T* win, void* out, const real::FrameMap& m, size_t nframes,
                           const void* twa, const cpx<T>* tab, int sms, cudaStream_t s) {
     typename onchip::StftBody<Cfg<true>>::Args a;
@@ -224,8 +244,8 @@ struct OnChipImpl {
                   {(const cpx<T>*)in, (cpx<T>*)out, (const TwPair<T>*)twa, tab, (long)batch, h}, batch, sms, s);
   }
   static const OnChipOps<T>* ops() {
-    static const RealOnChipOps<T> r = {RA, RB, Cfg<true>::C, &real_prepare, &real, &conv, &lconv, &stft, &mel, &welch,
-                                      &dct, &csd};
+    static const RealOnChipOps<T> r = {RA, RB, Cfg<true>::C, &real_prepare, &real, &conv, &lconv, &stft, &mel, &mfcc,
+                                      &welch, &dct, &csd};
     static const OnChipOps<T> o = {RA, RB, &prepare, &fft, kHasBluestein ? &bluestein : nullptr, &r};
     return &o;
   }

@@ -9,8 +9,9 @@
 //   * onchip_lconv_kernel:    linear convolution of real rows of any length by overlap-save on the same phases.
 //   * onchip_stft_kernel:     windowed frames of real rows of any length through the forward real-input phases.
 //   * onchip_mel_kernel:      the stft's frames to mel energies: power and filter bank on chip.
+//   * onchip_mfcc_kernel:     the mel energies on to their logs, a clamp and a projection (MFCC, log-mel) on chip.
 //   * onchip_dct_kernel:      discrete cosine transforms (types II and III) of real rows of length 2L.
-//     (these seven run the phases of FftBody / RealBody / ConvBody / LinConvBody / StftBody / MelBody /
+//     (these eight run the phases of FftBody / RealBody / ConvBody / LinConvBody / StftBody / MelBody / MfccBody /
 //     Dct2Body / Dct3Body through run_onchip_groups, tilefft.cuh)
 //   * onchip_welch_kernel:    detrended, windowed frames to Welch's averaged power spectrum, summed on chip
 //                             (WelchBody through run_welch_groups, below).
@@ -471,6 +472,95 @@ template <class Cfg> struct MelBody {
 template <class Cfg, int MINB>
 __global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_mel_kernel(const typename MelBody<Cfg>::Args a) {
   run_onchip_groups<Cfg, MelBody<Cfg>>(a);
+}
+
+// ---- fused MFCC and log-mel spectrogram of real rows, N = 2L (real::log_mel / mfcc_dot, DESIGN.md §4.18) -----------
+// MelBody's phases 0-6 as they are (the frame through the FFT, the untangle and the L+1 powers parked as reals), then:
+//   * log-mels (phase 7): lane u of the FFT forms mels m = u, u + TP, ... with real::mel_dot and their logs.  The output
+//     sweep parks them in the park's free L-1 reals behind the powers (n_mels <= L-1; no lane reads those in this phase).
+//     The max sweep (MAX) parks instead the key of each lane's largest log-mel, at real L+1+u;
+//   * project (phase 8): lane u computes outputs j = u, u + TP, ... < n_out from the parked log-mels, clamped to its
+//     row's group threshold, reading dct[m][j] (consecutive lanes on consecutive addresses) and storing out[q][j].
+//     The max sweep's phase 8 instead: lane 0 of the FFT folds the largest of the TP keys into the group slot, one fold
+//     per frame (a fold per lane made the max sweep four times slower than the output sweep at f32 N = 512).
+// MelBody::Args with mel = the output (n_out reals per frame, unused by the max sweep), for both sweeps
+template <class Cfg> struct MfccArgs : MelBody<Cfg>::Args { real::MfccArgs<typename MelBody<Cfg>::T> p; };
+template <class Cfg, bool MAX> struct MfccBody {
+  using Mel = MelBody<Cfg>;
+  using Real = RealBody<Cfg>;
+  using Tile = typename Cfg::Tile;   // FWD = true
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  static constexpr int L = Cfg::L, TP = Tile::TP;
+  using Args = MfccArgs<Cfg>;
+
+  static FB_HD void log_mels(const Args& a, long grp, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const long q = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (q >= a.batch) return;
+    T* pw = reinterpret_cast<T*>(smem + Real::park(t));
+    // opaque as in MelBody::mels: formed here, not hoisted through the FFT phases
+    const T* filters = a.filters;
+    const real::Band* bands = a.bands;
+#ifdef __CUDA_ARCH__
+    asm volatile("" : "+l"(filters), "+l"(bands), "+l"(pw));
+#endif
+    real::MaxKey<T> hi = 0;
+    for (long m = u; m < a.n_mels; m += TP) {
+      const T v = real::log_mel(real::mel_dot(filters, bands, (long)(L + 1), m, [&](long k) { return pw[k]; }), a.p);
+      if constexpr (MAX) {
+        const real::MaxKey<T> k = real::max_key(v);
+        hi = k > hi ? k : hi;
+      } else {
+        pw[L + 1 + m] = v;
+      }
+    }
+    if constexpr (MAX) memcpy(pw + L + 1 + u, &hi, sizeof hi);
+  }
+  static FB_HD void fold(const Args& a, long grp, int t, const V* smem) {
+    const long q = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (q >= a.batch || Tile::template u_of<true>(t) != 0) return;
+    const T* keys = reinterpret_cast<const T*>(smem + Real::park(t)) + (L + 1);
+#ifdef __CUDA_ARCH__
+    asm volatile("" : "+l"(keys));
+#endif
+    real::MaxKey<T> hi = 0;
+    for (int v = 0; v < TP; ++v) {
+      real::MaxKey<T> k;
+      memcpy(&k, keys + v, sizeof k);
+      hi = k > hi ? k : hi;
+    }
+    real::max_fold(a.p.slots + real::clamp_group(a.p, a.m.row_of(a.m.g0 + q)), hi);
+  }
+  static FB_HD void project(const Args& a, long grp, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const long q = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (q >= a.batch) return;
+    const long g = a.m.g0 + q;
+    const T* lm = reinterpret_cast<const T*>(smem + Real::park(t)) + (L + 1);
+#ifdef __CUDA_ARCH__
+    asm volatile("" : "+l"(lm));
+#endif
+    const T theta = real::clamp_threshold(a.p, a.m.row_of(g));
+    T* y = a.mel + q * a.p.n_out;
+    for (long j = u; j < a.p.n_out; j += TP)
+      real::lin_st(y + j, real::mfcc_dot(a.p, a.n_mels, j, [&](long m) { return real::clamp_db(lm[m], theta); }), g);
+  }
+
+  // phase protocol (tilefft.cuh): MelBody's load, stage A, scatter, gather + stage B, park, powers and park powers;
+  // log-mels; project (output sweep) or fold (max sweep)
+  static constexpr int kPhases = 9;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    if constexpr (P <= 6) Mel::template phase<P>(f, a, grp, t, smem, twa);
+    else if constexpr (P == 7) log_mels(a, grp, t, smem);
+    else if constexpr (MAX) fold(a, grp, t, smem);
+    else project(a, grp, t, smem);
+  }
+};
+
+template <class Cfg, int MINB, bool MAX>
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_mfcc_kernel(const typename MfccBody<Cfg, MAX>::Args a) {
+  run_onchip_groups<Cfg, MfccBody<Cfg, MAX>>(a);
 }
 
 // ---- fused Welch power spectral density of real rows, N = 2L (real::WelchItems, DESIGN.md §4.15) -----------------

@@ -315,6 +315,11 @@ template <typename T> struct RealOnChipOps {
   cudaError_t (*mel)(const T* in, const T* win, const T* filters, const real::Band* bands, size_t n_mels, int power,
                      T* out, const real::FrameMap& m, size_t nframes, const void* twa, const cpx<T>* tab, int sms,
                      cudaStream_t);
+  // mfcc(): the MFCC / log-mel outputs of the same frames (DESIGN.md §4.18), p.n_out reals per frame from `out` on, or
+  // with max_sweep only each frame's log-mel maximum folded into its group's slot (n_mels <= L - 1)
+  cudaError_t (*mfcc)(const T* in, const T* win, const T* filters, const real::Band* bands, size_t n_mels, int power,
+                      const real::MfccArgs<T>& p, bool max_sweep, T* out, const real::FrameMap& m, size_t nframes,
+                      const void* twa, const cpx<T>* tab, int sms, cudaStream_t);
   // welch(): the Welch items w (DESIGN.md §4.15) of the rows of m, from `in` on: each item's partial into part, or, when
   // a row is one item, the row's output into out; base = s / F in device memory, detrend real::kDetrend*
   cudaError_t (*welch)(const T* in, const T* win, const T* base, int detrend, T* part, T* out, const real::FrameMap& m,
@@ -400,6 +405,21 @@ class RealPlan {
   cudaError_t mel_host(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
                        size_t n_mels, int power, T* out, size_t batch);
 
+  // MFCC and log-mel spectrogram (DESIGN.md §4.18): the mels of mel_device -> n_out reals per frame, frame-major,
+  // out[b][f][j] = sum_m max(scale ln(max(mel + offset, floor)), theta_g) dct[m][j] + bias (real::MfccArgs; dct nullptr:
+  // the identity).  With top_db finite, theta_g = max over clamp group g (top_db_rows consecutive rows, batch a multiple
+  // of it) of the logs - top_db, found by a first sweep over the frames; else -inf.  Scalars finite, floor and scale > 0,
+  // checked by the caller with the mel spectrogram's arguments.  Out of place only.  Device pointers, on `stream`.
+  cudaError_t mfcc_device(const T* in, size_t in_len, const T* win, size_t hop, int boundary, int power,
+                          const T* filters, size_t n_mels, double log_offset, double log_floor, double log_scale,
+                          double top_db, size_t top_db_rows, const T* dct, size_t n_out, double bias, T* out,
+                          size_t batch, cudaStream_t stream);
+  // Host pointers: the window, filters and matrix are staged once, whole rows through stage_rows (twice with the clamp);
+  // the same bits.
+  cudaError_t mfcc_host(const T* in, size_t in_len, const T* win, size_t hop, int boundary, int power, const T* filters,
+                        size_t n_mels, double log_offset, double log_floor, double log_scale, double top_db,
+                        size_t top_db_rows, const T* dct, size_t n_out, double bias, T* out, size_t batch);
+
   // Welch power spectral density (DESIGN.md §4.15): `batch` rows of in_len >= N reals -> N/2+1 reals each, out[b][k] =
   // c_k s / F sum_f |rfft(win . (frame f - its mean))[k]|^2 over the F frames of hop `hop` (no padding), the mean only
   // with detrend real::kDetrendConstant, s from scaling real::kWelch* and fs.  Arguments checked by the caller.  Out of
@@ -448,6 +468,8 @@ class RealPlan {
   size_t mel_row_bytes(size_t in_len, size_t hop, int boundary, size_t n_mels) const {
     return frame_count(in_len, hop, boundary) * n_mels * sizeof(T);
   }
+  // an MFCC call runs the fused kernel: a fused plan, and n_mels <= L - 1 log-mels fit the park behind the L+1 powers
+  bool mfcc_fused(size_t n_mels) const { return path_ == Path::kRealFused && n_mels + 1 <= m_; }
 
  private:
   template <class P> friend P* create_plan(size_t, int, bool);
@@ -470,6 +492,15 @@ class RealPlan {
   // launches_
   cudaError_t mel_frames(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
                          size_t n_mels, int power, T* out, size_t batch, cudaStream_t s);
+  // one sweep of an MFCC call after mel_bands over `batch` rows (p.row0 the first one's row in the call): the max sweep
+  // (max_sweep) or the output sweep, by the fused kernel or chunks of frames through seg_; adds its kernels to launches_
+  cudaError_t mfcc_frames(const T* in, size_t in_len, const T* win, size_t hop, int boundary, int power,
+                          const T* filters, size_t n_mels, const real::MfccArgs<T>& p, bool max_sweep, T* out,
+                          size_t batch, cudaStream_t s);
+  // the MfccArgs of a call from its double scalars (each rounded to T once) and the slots of its groups in slots_, set
+  // to 0 on `s` when the clamp is on (a memset, not counted as a launch)
+  cudaError_t mfcc_args(double log_offset, double log_floor, double log_scale, double top_db, size_t top_db_rows,
+                        const T* dct, size_t n_out, double bias, size_t batch, cudaStream_t s, real::MfccArgs<T>* p);
   // s / F of a Welch call from the window into welch_base_ (one launch, added to launches_)
   cudaError_t welch_scale(const T* win, int scaling, double fs, size_t frames, cudaStream_t s);
   // welch_device after welch_scale: chunks of rows whose partials fit part_, each through the fused kernel or chunks of
@@ -482,7 +513,8 @@ class RealPlan {
   cudaError_t cross_rows(const T* x, const T* y, size_t y_rows, size_t y_off, size_t in_len, const T* win, size_t hop,
                          int detrend, bool coh, void* out, size_t batch, cudaStream_t s);
   // The host-pointer loop (real.cu): chunks of rows of in_row / out_row bytes go H2D, through
-  // step(dev_in, dev_out, first_row, rows) on host_stream_, and D2H; launches() then counts all chunks.
+  // step(dev_in, dev_out, first_row, rows) on host_stream_, and D2H (nothing with out_row 0); launches() then counts all
+  // chunks.
   template <class Step>
   cudaError_t stage_rows(const void* in, void* out, size_t batch, size_t in_row, size_t out_row, Step step);
   // A host-pointer call's constant operands, a and optionally b, go H2D into stage_spec_ on host_stream_, each at a
@@ -508,10 +540,12 @@ class RealPlan {
   DeviceBuffer seg_;                 // one chunk of N-real segments or frames (for the mel spectrogram, the frames'
                                      // spectra behind them)
   DeviceBuffer bands_;               // the filter bands of the last mel call (real::Band per filter row)
+  DeviceBuffer slots_;               // the clamp groups' maxima of the last MFCC call (real::MaxKey<T> per group)
   DeviceBuffer welch_base_;          // s / F of the last Welch call (one T)
   DeviceBuffer part_;                // one chunk of rows of Welch partials (N/2+1 reals per item; 2 or 4 planes of
                                      // them for the csd and coherence)
   DeviceBuffer stage_y_;             // the y rows of one host-pointer chunk of a csd or coherence call
+  DeviceBuffer stage_dct_;           // the projection matrix of a host-pointer MFCC call
   cudaStream_t host_stream_ = nullptr;
   std::string kernel_desc_;
 };

@@ -179,6 +179,48 @@ mel_spectra_kernel(const cpx<T>* __restrict__ spec, const T* __restrict__ filter
   }
 }
 
+// MFCC (real::log_mel / mfcc_dot) of a chunk's mels: the frame's n_mels mels at mel + q * n_mels, frame g0 + q of
+// rows of `frames` frames.  MAX: CTA c takes a contiguous run of frames, and each thread folds the key of its largest
+// log-mel (m = t, t + kThreads, ...) into a group's slot once per group the run meets.  Otherwise one CTA per frame: the
+// threads write the frame's clamped log-mels over its mels, and after a barrier thread t computes outputs j = t,
+// t + kThreads, ... into out (n_out reals per frame).
+template <typename T, bool MAX>
+__global__ void __launch_bounds__(kThreads)
+mfcc_frames_kernel(T* mel, long n_mels, const real::MfccArgs<T> p, T* __restrict__ out, long nframes, long g0,
+                   long frames) {
+  if constexpr (MAX) {
+    const long per = (nframes + gridDim.x - 1) / gridDim.x, q1 = std::min(nframes, (blockIdx.x + 1) * per);
+    real::MaxKey<T> hi = 0;
+    long grp = -1;
+    for (long q = blockIdx.x * per; q < q1; ++q) {
+      const long g = real::clamp_group(p, (g0 + q) / frames);
+      if (g != grp) {
+        if (grp >= 0) real::max_fold(p.slots + grp, hi);
+        grp = g;
+        hi = 0;
+      }
+      for (long m = threadIdx.x; m < n_mels; m += kThreads) {
+        const real::MaxKey<T> k = real::max_key(real::log_mel(mel[q * n_mels + m], p));
+        hi = k > hi ? k : hi;
+      }
+    }
+    if (grp >= 0) real::max_fold(p.slots + grp, hi);
+    return;
+  }
+  for (long q = blockIdx.x; q < nframes; q += gridDim.x) {
+    T* x = mel + q * n_mels;
+    const long b = (g0 + q) / frames;
+    {
+      const T theta = real::clamp_threshold(p, b);
+      for (long m = threadIdx.x; m < n_mels; m += kThreads) x[m] = real::clamp_db(real::log_mel(x[m], p), theta);
+      __syncthreads();
+      for (long j = threadIdx.x; j < p.n_out; j += kThreads)
+        real::lin_st(out + q * p.n_out + j, real::mfcc_dot(p, n_mels, j, [&](long m) { return x[m]; }), g0 + q);
+      __syncthreads();
+    }
+  }
+}
+
 // Welch (real::WelchItems).  scale: one CTA, the window sums in double, each thread over every kThreads-th sample in
 // ascending order, then a tree in shared memory.  gather: one CTA per frame q of the chunk (frame g0 + q of the rows'
 // FrameMap), the frame mean by the same two steps in T, then (x - mu) w into seg.  accumulate: one thread per (item, bin)
@@ -542,8 +584,9 @@ cudaError_t RealPlan<T>::stage_rows(const void* in, void* out, size_t batch, siz
     launches_ = 0;
     FB_CHECK(step(stage_in_.data(), stage_out_.data(), b0, nb));
     total += launches_;
-    FB_CHECK(cudaMemcpyAsync((char*)out + b0 * out_row, stage_out_.data(), nb * out_row, cudaMemcpyDeviceToHost,
-                             host_stream_));
+    if (out_row)
+      FB_CHECK(cudaMemcpyAsync((char*)out + b0 * out_row, stage_out_.data(), nb * out_row, cudaMemcpyDeviceToHost,
+                               host_stream_));
     FB_CHECK(cudaStreamSynchronize(host_stream_));
   }
   launches_ = total;
@@ -901,6 +944,132 @@ cudaError_t RealPlan<T>::mel_host(const T* in, size_t in_len, const T* win, size
                                           nb, host_stream_);
                       }));
   launches_ += 1;
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::mfcc_args(double log_offset, double log_floor, double log_scale, double top_db,
+                                   size_t top_db_rows, const T* dct, size_t n_out, double bias, size_t batch,
+                                   cudaStream_t s, real::MfccArgs<T>* p) {
+  const bool clamp = std::isfinite(top_db);
+  p->offset = (T)log_offset;
+  p->floor = (T)log_floor;
+  p->scale = (T)log_scale;
+  p->top_db = clamp ? (T)top_db : (T)0;
+  p->bias = (T)bias;
+  p->dct = dct;
+  p->n_out = (long)n_out;
+  p->rows = clamp ? (long)top_db_rows : 0;
+  p->row0 = 0;
+  p->rows_rcp = clamp ? 1.0 / (double)top_db_rows : 0.0;
+  p->slots = nullptr;
+  if (clamp) {
+    const size_t bytes = batch / top_db_rows * sizeof(real::MaxKey<T>);
+    FB_CHECK(slots_.reserve(bytes));
+    FB_CHECK(cudaMemsetAsync(slots_.data(), 0, bytes, s));
+    p->slots = (real::MaxKey<T>*)slots_.data();
+  }
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::mfcc_frames(const T* in, size_t in_len, const T* win, size_t hop, int boundary, int power,
+                                     const T* filters, size_t n_mels, const real::MfccArgs<T>& p, bool max_sweep,
+                                     T* out, size_t batch, cudaStream_t s) {
+  const real::FrameMap m = real::frame_map((long)n_, (long)in_len, (long)hop, boundary);
+  const size_t total = batch * (size_t)m.frames, bins = n_ / 2 + 1;
+  const real::Band* bands = (const real::Band*)bands_.data();
+  if (mfcc_fused(n_mels)) {
+    FB_CHECK(fused_->mfcc(in, win, filters, bands, n_mels, power, p, max_sweep, out, m, total, twa_.data(),
+                          (const C*)tab_.data(), sm_count_, s));
+    launches_ += 1;
+    return cudaSuccess;
+  }
+  // chunks of frames through seg_ as in mel_frames, the mels into a third region behind the spectra, then
+  // mfcc_frames_kernel from there
+  const size_t chunk = scratch_chunk(total, n_ * sizeof(T) + bins * sizeof(C) + n_mels * sizeof(T));
+  const size_t spec_off = (chunk * n_ * sizeof(T) + 255) / 256 * 256;
+  const size_t mel_off = spec_off + (chunk * bins * sizeof(C) + 255) / 256 * 256;
+  FB_CHECK(seg_.reserve(mel_off + chunk * n_mels * sizeof(T)));
+  T* seg = (T*)seg_.data();
+  C* spec = (C*)((char*)seg_.data() + spec_off);
+  T* mel = (T*)((char*)seg_.data() + mel_off);
+  const unsigned long long before = launches_;
+  unsigned long long count = 0;
+  for (size_t q0 = 0; q0 < total; q0 += chunk) {
+    const size_t nq = std::min(chunk, total - q0);
+    real::FrameMap mc = m;
+    mc.g0 = (long)q0;
+    gather_frames_kernel<T><<<grid_for(nq * n_), kThreads, 0, s>>>(in, win, seg, mc, (long)nq);
+    FB_CHECK(cudaGetLastError());
+    FB_CHECK(exec_device(true, seg, spec, nq, kFft, s));
+    count += 3 + launches_;
+    mel_spectra_kernel<T><<<grid_for(nq * n_mels), kThreads, 0, s>>>(spec, filters, bands, (long)bins, (long)n_mels,
+                                                                      power, mel, (long)nq, (long)q0);
+    FB_CHECK(cudaGetLastError());
+    const unsigned grid = (unsigned)std::min<size_t>(nq, (size_t)sm_count_ * 16);
+    if (max_sweep)
+      mfcc_frames_kernel<T, true><<<grid, kThreads, 0, s>>>(mel, (long)n_mels, p, nullptr, (long)nq, (long)q0,
+                                                            m.frames);
+    else
+      mfcc_frames_kernel<T, false><<<grid, kThreads, 0, s>>>(mel, (long)n_mels, p, out + q0 * p.n_out, (long)nq,
+                                                             (long)q0, m.frames);
+    FB_CHECK(cudaGetLastError());
+  }
+  launches_ = before + count;
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::mfcc_device(const T* in, size_t in_len, const T* win, size_t hop, int boundary, int power,
+                                     const T* filters, size_t n_mels, double log_offset, double log_floor,
+                                     double log_scale, double top_db, size_t top_db_rows, const T* dct, size_t n_out,
+                                     double bias, T* out, size_t batch, cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  real::MfccArgs<T> p;
+  FB_CHECK(mfcc_args(log_offset, log_floor, log_scale, top_db, top_db_rows, dct, n_out, bias, batch, s, &p));
+  FB_CHECK(mel_bands(filters, n_mels, s));
+  if (p.rows) FB_CHECK(mfcc_frames(in, in_len, win, hop, boundary, power, filters, n_mels, p, true, out, batch, s));
+  return mfcc_frames(in, in_len, win, hop, boundary, power, filters, n_mels, p, false, out, batch, s);
+}
+
+// The max sweep stages every row once more (through stage_rows with no output), in chunks of its own size: the group
+// slots are indexed by the call's rows, so where the chunks cut a group does not matter.
+template <typename T>
+cudaError_t RealPlan<T>::mfcc_host(const T* in, size_t in_len, const T* win, size_t hop, int boundary, int power,
+                                   const T* filters, size_t n_mels, double log_offset, double log_floor,
+                                   double log_scale, double top_db, size_t top_db_rows, const T* dct, size_t n_out,
+                                   double bias, T* out, size_t batch) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  const T *dwin, *dfilt, *ddct = nullptr;
+  FB_CHECK(stage_consts(win, n_ * sizeof(T), &dwin, filters, n_mels * (n_ / 2 + 1) * sizeof(T), &dfilt));
+  if (dct) {
+    FB_CHECK(stage_dct_.reserve(n_mels * n_out * sizeof(T)));
+    FB_CHECK(cudaMemcpyAsync(stage_dct_.data(), dct, n_mels * n_out * sizeof(T), cudaMemcpyHostToDevice, host_stream_));
+    ddct = (const T*)stage_dct_.data();
+  }
+  real::MfccArgs<T> p;
+  FB_CHECK(mfcc_args(log_offset, log_floor, log_scale, top_db, top_db_rows, ddct, n_out, bias, batch, host_stream_, &p));
+  FB_CHECK(mel_bands(dfilt, n_mels, host_stream_));
+  const unsigned long long setup = launches_;
+  unsigned long long sweeps = 0;
+  auto sweep = [&](bool max_sweep, void* dst, size_t out_row) -> cudaError_t {
+    FB_CHECK(stage_rows(in, dst, batch, in_len * sizeof(T), out_row, [&](const void* din, void* dout, size_t b0, size_t nb) {
+      real::MfccArgs<T> pc = p;
+      pc.row0 = (long)b0;
+      return mfcc_frames((const T*)din, in_len, dwin, hop, boundary, power, dfilt, n_mels, pc, max_sweep, (T*)dout, nb,
+                         host_stream_);
+    }));
+    sweeps += launches_;
+    return cudaSuccess;
+  };
+  if (p.rows) FB_CHECK(sweep(true, out, 0));
+  FB_CHECK(sweep(false, out, mel_row_bytes(in_len, hop, boundary, n_out)));
+  launches_ = setup + sweeps;
   return cudaSuccess;
 }
 

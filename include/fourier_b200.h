@@ -339,6 +339,54 @@ int fourier_b200_mel_spectrogram_async_double(struct fourier_b200_rfft_double *p
                                               int power, const double *filters_dev, size_t n_mels, double *out_dev,
                                               size_t batch, void *cuda_stream);
 
+/* ---- MFCC and log-mel spectrogram of real rows ----
+ * On a real plan of length N, with the mel spectrogram's framing, window, power and filters above (mel[b][f][m], F
+ * frames per row), in the plan's precision T (each double scalar rounded to T once):
+ *   lm[b][f][m]  = log_scale * ln(max(mel[b][f][m] + log_offset, log_floor)),
+ *   lc           = max(lm, theta_g) with theta_g = (max of lm over the rows, frames and mels of clamp group g) - top_db,
+ *                  the rows [g*top_db_rows, (g+1)*top_db_rows) forming group g; lc = lm when top_db is +inf,
+ *   out[b][f][j] = bias + sum_{m = 0 .. n_mels-1, ascending} lc[b][f][m] * dct[m*n_out + j],   j < n_out,
+ * where dct is a dense row-major (n_mels, n_out) matrix of any real values (torchaudio's create_dct layout; fold a
+ * lifter into its columns), or NULL for the identity with n_out == n_mels, which gives the log-mel spectrogram lc + bias.
+ * The output is frame-major, row b from element b*F*n_out on.  Recipes: torchaudio's MFCC(log_mels=False) with
+ * log_scale 10/ln 10, log_floor 1e-10, log_offset 0, top_db 80, top_db_rows = the channel count (1 for 1-D input);
+ * MFCC(log_mels=True) with log_scale 1, log_floor the smallest normal of T, log_offset 1e-6, top_db +inf; librosa's
+ * mfcc with top_db_rows = batch; Whisper's log-mel with log_scale 1/(4 ln 10), log_floor 1e-10, top_db 2, dct NULL,
+ * bias 1 (Whisper drops the last frame before its max; this takes the max over all F frames).
+ * The group maximum is exact and order-independent, and each output a fixed ascending sum, so a row's bits depend only on
+ * its clamp group's rows, the arguments and the plan: not on the rest of the batch, host or device memory or the stream.
+ * With the clamp (top_db finite) the frames are swept twice: once for the group maxima (kept in a plan-owned buffer),
+ * once for the outputs.  Launches: on the real_fused path with n_mels <= N/2 - 1, 2 (3 with the clamp); otherwise 1,
+ * plus per sweep and scratch chunk of frames 3 + those of the plan's rfft of that many rows.
+ * Refused with cudaErrorInvalidValue and a message (these also when batch == 0, which otherwise succeeds and launches
+ * nothing): a NULL in, window, filters or out, hop == 0, an unknown boundary, in_len == 0, power other than 1 and 2,
+ * n_mels == 0, n_out == 0, dct NULL with n_out != n_mels, log_offset or bias not finite, log_floor or log_scale not
+ * finite and > 0, top_db NaN or < 0, top_db_rows == 0, and with top_db finite a batch that is not a multiple of
+ * top_db_rows.  Also refused: in_len < N with _NONE, in_len <= N/2 with _REFLECT, the output overlapping the input,
+ * window, filters or dct (out of place only), and a mix of host and device buffers in the synchronous calls.  Device base
+ * pointers of input and output must be 16-byte aligned (cudaErrorMisalignedAddress).  Host memory is staged through the
+ * plan's buffers (the window, filters and dct once, whole rows in chunks) and gives the same bits as device memory.
+ * The _async calls take device memory, are enqueued on `cuda_stream` and never synchronise the host. */
+int fourier_b200_mfcc_float(struct fourier_b200_rfft_float *plan, const float *in, size_t in_len, const float *window,
+                            size_t hop, int boundary, int power, const float *filters, size_t n_mels, double log_offset,
+                            double log_floor, double log_scale, double top_db, size_t top_db_rows, const float *dct,
+                            size_t n_out, double bias, float *out, size_t batch);
+int fourier_b200_mfcc_double(struct fourier_b200_rfft_double *plan, const double *in, size_t in_len,
+                             const double *window, size_t hop, int boundary, int power, const double *filters,
+                             size_t n_mels, double log_offset, double log_floor, double log_scale, double top_db,
+                             size_t top_db_rows, const double *dct, size_t n_out, double bias, double *out,
+                             size_t batch);
+int fourier_b200_mfcc_async_float(struct fourier_b200_rfft_float *plan, const float *in_dev, size_t in_len,
+                                  const float *window_dev, size_t hop, int boundary, int power,
+                                  const float *filters_dev, size_t n_mels, double log_offset, double log_floor,
+                                  double log_scale, double top_db, size_t top_db_rows, const float *dct_dev,
+                                  size_t n_out, double bias, float *out_dev, size_t batch, void *cuda_stream);
+int fourier_b200_mfcc_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev, size_t in_len,
+                                   const double *window_dev, size_t hop, int boundary, int power,
+                                   const double *filters_dev, size_t n_mels, double log_offset, double log_floor,
+                                   double log_scale, double top_db, size_t top_db_rows, const double *dct_dev,
+                                   size_t n_out, double bias, double *out_dev, size_t batch, void *cuda_stream);
+
 /* ---- Welch power spectral density of real rows ----
  * On a real plan of length N, for `batch` rows of in_len >= N reals (row b at element b*in_len), a window of N reals
  * and hop >= 1: the F = 1 + (in_len - N) / hop frames x_bf[p] = in[b*in_len + f*hop + p], p < N (no padding, F =
