@@ -433,8 +433,9 @@ class RealPlan {
   // Cross-spectral density and coherence (DESIGN.md §4.17): `batch` rows x of in_len >= N reals, row b paired with y row
   // b mod y_rows (y_rows >= 1 rows of in_len reals), both framed, detrended and windowed as welch_device.  coh false:
   // out[b][k] = c_k s / F sum_f conj(X_bf[k]) Y_bf[k], N/2+1 complex values per row; coh true: out[b][k] =
-  // |sum_f conj(X) Y|^2 / (sum_f |X|^2 sum_f |Y|^2), N/2+1 reals per row (scaling and fs unused).  Arguments checked by
-  // the caller.  Out of place only.  Device pointers, on `stream`, never synchronised.
+  // |sum_f conj(X) Y|^2 / (sum_f |X|^2 sum_f |Y|^2), N/2+1 reals per row (scaling and fs unused).  y nullptr with coh
+  // false and y_rows 1: welch_device.  Arguments checked by the caller.  Out of place only.  Device pointers, on
+  // `stream`, never synchronised.
   cudaError_t cross_device(const T* x, const T* y, size_t y_rows, size_t in_len, const T* win, size_t hop, int detrend,
                            bool coh, int scaling, double fs, void* out, size_t batch, cudaStream_t stream);
   // Host pointers: the window is staged once, x rows through stage_rows and each chunk's y rows beside them; the same
@@ -479,42 +480,50 @@ class RealPlan {
   size_t frame_count(size_t in_len, size_t hop, int boundary) const {
     return (size_t)real::frame_map((long)n_, (long)in_len, (long)hop, boundary).frames;
   }
-  // convolve_device with row b using spectrum row ((row0 + b) / per) mod rows; adds its kernels to launches_
+  // exec_device after its checks
+  cudaError_t rfft_rows(bool forward, const void* in, void* out, size_t batch, int code, cudaStream_t s);
+  // convolve_device with row b using spectrum row ((row0 + b) / per) mod rows
   cudaError_t convolve_rows(const T* in, const C* spec, size_t rows, size_t row0, size_t per, T* out, size_t batch,
                             cudaStream_t s);
   // segments m.g0 .. m.g0 + nseg - 1 of a linear convolution: the fused kernel, or chunks of gather, convolve_rows and
-  // scatter through seg_; adds its kernels to launches_
+  // scatter through seg_
   cudaError_t linear_segments(const T* in, T* out, const real::SegMap& m, size_t nseg, const C* spec, size_t rows,
                               cudaStream_t s);
-  // the band of every filter row into bands_ (one launch, added to launches_)
+  // stft_device, istft_device and dct_device after their checks: the fused kernel, or chunks through seg_
+  cudaError_t stft_rows(const T* in, size_t in_len, const T* win, size_t hop, int boundary, C* out, size_t batch,
+                        cudaStream_t s);
+  cudaError_t istft_rows(const C* in, size_t frames, const T* win, size_t hop, bool center, T* out, size_t out_len,
+                         size_t batch, cudaStream_t s);
+  cudaError_t dct_rows(const T* in, T* out, size_t batch, int type, int norm, cudaStream_t s);
+  // the band of every filter row into bands_ (one launch)
   cudaError_t mel_bands(const T* filters, size_t n_mels, cudaStream_t s);
-  // mel_device after mel_bands: the fused kernel, or chunks of gathered frames and their spectra through seg_; sets
-  // launches_
-  cudaError_t mel_frames(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
-                         size_t n_mels, int power, T* out, size_t batch, cudaStream_t s);
+  // mel_device after mel_bands: the fused kernel, or chunks of frames through seg_
+  cudaError_t mel_rows(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
+                       size_t n_mels, int power, T* out, size_t batch, cudaStream_t s);
   // one sweep of an MFCC call after mel_bands over `batch` rows (p.row0 the first one's row in the call): the max sweep
-  // (max_sweep) or the output sweep, by the fused kernel or chunks of frames through seg_; adds its kernels to launches_
-  cudaError_t mfcc_frames(const T* in, size_t in_len, const T* win, size_t hop, int boundary, int power,
-                          const T* filters, size_t n_mels, const real::MfccArgs<T>& p, bool max_sweep, T* out,
-                          size_t batch, cudaStream_t s);
+  // (max_sweep) or the output sweep, by the fused kernel or chunks of frames through seg_
+  cudaError_t mfcc_rows(const T* in, size_t in_len, const T* win, size_t hop, int boundary, int power,
+                        const T* filters, size_t n_mels, const real::MfccArgs<T>& p, bool max_sweep, T* out,
+                        size_t batch, cudaStream_t s);
   // the MfccArgs of a call from its double scalars (each rounded to T once) and the slots of its groups in slots_, set
   // to 0 on `s` when the clamp is on (a memset, not counted as a launch)
   cudaError_t mfcc_args(double log_offset, double log_floor, double log_scale, double top_db, size_t top_db_rows,
                         const T* dct, size_t n_out, double bias, size_t batch, cudaStream_t s, real::MfccArgs<T>* p);
-  // s / F of a Welch call from the window into welch_base_ (one launch, added to launches_)
+  // s / F of a Welch call from the window into welch_base_ (one launch)
   cudaError_t welch_scale(const T* win, int scaling, double fs, size_t frames, cudaStream_t s);
-  // welch_device after welch_scale: chunks of rows whose partials fit part_, each through the fused kernel or chunks of
-  // frames through seg_, then the finish; adds its kernels to launches_
-  cudaError_t welch_rows(const T* in, size_t in_len, const T* win, size_t hop, int detrend, T* out, size_t batch,
-                         cudaStream_t s);
-  // cross_device after welch_scale (csd only): row b of x with y row (y_off + b) mod y_rows; chunks of rows whose
-  // partials fit part_, each through the fused kernel or chunks of frame pairs through seg_, then the finish; adds its
-  // kernels to launches_
-  cudaError_t cross_rows(const T* x, const T* y, size_t y_rows, size_t y_off, size_t in_len, const T* win, size_t hop,
-                         int detrend, bool coh, void* out, size_t batch, cudaStream_t s);
+  // cross_device after welch_scale (Welch and csd): row b of x with y row (y_off + b) mod y_rows, or alone (y nullptr:
+  // Welch); chunks of rows whose partials fit part_, each through the fused kernel or chunks of frames (x and y frame
+  // pairs) through seg_, then the finish
+  cudaError_t welch_cross_rows(const T* x, const T* y, size_t y_rows, size_t y_off, size_t in_len, const T* win,
+                               size_t hop, int detrend, bool coh, void* out, size_t batch, cudaStream_t s);
+  // Frames 0 .. total-1 of m, k per index, in chunks through seg_: per chunk gather(seg, mc, nq) (one launch), the
+  // plan's rfft of the chunk's k * nq frames into spec_out + k * q0 spectra or into seg_ behind the frames, then
+  // use(spec, q0, nq, extra_region) with `extra` bytes per index behind the spectra (real.cu).
+  template <class Gather, class Use>
+  cudaError_t frame_chunks(const real::FrameMap& m, size_t total, size_t k, C* spec_out, size_t extra, cudaStream_t s,
+                           Gather gather, Use use);
   // The host-pointer loop (real.cu): chunks of rows of in_row / out_row bytes go H2D, through
-  // step(dev_in, dev_out, first_row, rows) on host_stream_, and D2H (nothing with out_row 0); launches() then counts all
-  // chunks.
+  // step(dev_in, dev_out, first_row, rows) on host_stream_, and D2H (nothing with out_row 0).
   template <class Step>
   cudaError_t stage_rows(const void* in, void* out, size_t batch, size_t in_row, size_t out_row, Step step);
   // A host-pointer call's constant operands, a and optionally b, go H2D into stage_spec_ on host_stream_, each at a
@@ -528,6 +537,8 @@ class RealPlan {
   size_t n_ = 0, m_ = 0;        // m_ = N/2 (even N)
   int device_ = 0;
   Path path_ = Path::kRealFull;
+  // launches() of the last call: each public method sets it to 0 at its start, and every private step adds the launches
+  // it makes, 1 per kernel and inner_->launches() after each call of the inner plan
   unsigned long long launches_ = 0;
   int sm_count_ = 132;
   const RealOnChipOps<T>* fused_ = nullptr;
@@ -537,8 +548,8 @@ class RealPlan {
   DeviceBuffer work_;                // one chunk of inner-plan rows
   DeviceBuffer stage_in_, stage_out_;
   DeviceBuffer stage_spec_;          // the constant operands of a host-pointer call: spectra, window, filters
-  DeviceBuffer seg_;                 // one chunk of N-real segments or frames (for the mel spectrogram, the frames'
-                                     // spectra behind them)
+  DeviceBuffer seg_;                 // one chunk of N-real segments or frames (real::FrameMap: the frames' spectra
+                                     // and per-frame values behind them)
   DeviceBuffer bands_;               // the filter bands of the last mel call (real::Band per filter row)
   DeviceBuffer slots_;               // the clamp groups' maxima of the last MFCC call (real::MaxKey<T> per group)
   DeviceBuffer welch_base_;          // s / F of the last Welch call (one T)

@@ -19,10 +19,12 @@
 // Welch power spectral density (DESIGN.md §4.15): welch_scale_kernel, then per chunk of rows onchip_welch_kernel on the
 // fused path, or chunks of detrended windowed frames gathered into seg_, their spectra by the plan's own rfft behind
 // them and welch_accumulate_kernel into the partials; then welch_finish_kernel unless the fused kernel wrote the rows.
-// Cross-spectral density and coherence (DESIGN.md §4.17): Welch's steps on frame pairs: welch_scale_kernel (csd only),
-// then per chunk of rows onchip_csd_kernel, or chunks of x frames and their y frames gathered into seg_
-// (csd_gather_kernel), their spectra by the plan's own rfft behind them and cross_accumulate_kernel into the partials;
-// then cross_finish_kernel unless the fused kernel wrote the rows.
+// Cross-spectral density and coherence (DESIGN.md §4.17): Welch's steps on frame pairs, in the same row driver
+// (welch_cross_rows): welch_scale_kernel (csd only), then per chunk of rows onchip_csd_kernel, or chunks of x frames and
+// their y frames gathered into seg_ (csd_gather_kernel), their spectra by the plan's own rfft behind them and
+// cross_accumulate_kernel into the partials; then cross_finish_kernel unless the fused kernel wrote the rows.
+// Off the fused path, every chunk of frames above goes through one loop, frame_chunks: the gather, the plan's own rfft
+// (rfft_rows) and the transform's consumer kernels.
 // Discrete cosine transforms (DESIGN.md §4.16): onchip_dct_kernel on the fused path; otherwise per chunk of rows an O(N)
 // kernel into seg_, the inner plan in place there and an O(N) kernel into the output: dct_permute_kernel, Fft and
 // dct_untangle_kernel (type 2) or dct_tangle_kernel, UnscaledIfft and dct_unpermute_kernel (type 3) at half length;
@@ -509,11 +511,16 @@ cudaError_t RealPlan<T>::exec_device(bool forward, const void* in, void* out, si
   if (cudaError_t e = check_code(forward, code)) return e;
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
+  return rfft_rows(forward, in, out, batch, code, s);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::rfft_rows(bool forward, const void* in, void* out, size_t batch, int code, cudaStream_t s) {
   const T scale = scale_for<T>(code, n_);
   if (path_ == Path::kRealFused) {
     FB_CHECK(fused_->run(in, out, twa_.data(), (const C*)tab_.data(), batch, forward, forward ? scale / 2 : scale,
                          sm_count_, s));
-    launches_ = 1;
+    launches_ += 1;
     return cudaSuccess;
   }
   const size_t len = inner_->size(), bins = n_ / 2 + 1;
@@ -576,20 +583,16 @@ cudaError_t RealPlan<T>::stage_rows(const void* in, void* out, size_t batch, siz
   const size_t rows = std::min(batch, std::max<size_t>(1, kHostChunkBytes / std::max(in_row, out_row)));
   FB_CHECK(stage_in_.reserve(rows * in_row));
   FB_CHECK(stage_out_.reserve(rows * out_row));
-  unsigned long long total = 0;
   for (size_t b0 = 0; b0 < batch; b0 += rows) {
     const size_t nb = std::min(rows, batch - b0);
     FB_CHECK(cudaMemcpyAsync(stage_in_.data(), (const char*)in + b0 * in_row, nb * in_row, cudaMemcpyHostToDevice,
                              host_stream_));
-    launches_ = 0;
     FB_CHECK(step(stage_in_.data(), stage_out_.data(), b0, nb));
-    total += launches_;
     if (out_row)
       FB_CHECK(cudaMemcpyAsync((char*)out + b0 * out_row, stage_out_.data(), nb * out_row, cudaMemcpyDeviceToHost,
                                host_stream_));
     FB_CHECK(cudaStreamSynchronize(host_stream_));
   }
-  launches_ = total;
   return cudaSuccess;
 }
 
@@ -618,7 +621,7 @@ cudaError_t RealPlan<T>::exec_host(bool forward, const void* in, void* out, size
   DeviceGuard g(device_);
   return stage_rows(in, out, batch, row_bytes(forward, true), row_bytes(forward, false),
                     [&](const void* din, void* dout, size_t, size_t nb) {
-                      return exec_device(forward, din, dout, nb, code, host_stream_);
+                      return rfft_rows(forward, din, dout, nb, code, host_stream_);
                     });
 }
 
@@ -750,7 +753,6 @@ cudaError_t RealPlan<T>::linear_convolve_host(const T* in, size_t in_len, const 
   const size_t run = cap > n_ ? std::max<size_t>(1, (cap - n_) / (size_t)m.s) : 1;
   FB_CHECK(stage_in_.reserve((run * (size_t)m.s + n_) * sizeof(T)));
   FB_CHECK(stage_out_.reserve(run * (size_t)m.s * sizeof(T)));
-  unsigned long long total = 0;
   for (size_t b = 0; b < batch; ++b)
     for (long j0 = 0; j0 < m.per; j0 += (long)run) {
       const long j1 = std::min(m.per, j0 + (long)run);
@@ -764,15 +766,44 @@ cudaError_t RealPlan<T>::linear_convolve_host(const T* in, size_t in_len, const 
       if (mp.hi > mp.lo)
         FB_CHECK(cudaMemcpyAsync(stage_in_.data(), in + b * in_len + mp.lo, (mp.hi - mp.lo) * sizeof(T),
                                  cudaMemcpyHostToDevice, host_stream_));
-      launches_ = 0;
       FB_CHECK(linear_segments((const T*)stage_in_.data(), (T*)stage_out_.data(), mp, (size_t)(j1 - j0), dspec, rows,
                                host_stream_));
-      total += launches_;
       FB_CHECK(cudaMemcpyAsync(out + b * out_len + mp.out_lo, stage_out_.data(), (out_hi - mp.out_lo) * sizeof(T),
                                cudaMemcpyDeviceToHost, host_stream_));
       FB_CHECK(cudaStreamSynchronize(host_stream_));
     }
-  launches_ = total;
+  return cudaSuccess;
+}
+
+// Chunks of frames 0 .. total-1 of m through seg_, k frames per index (a frame, or an x frame and its y frame): per
+// chunk, gather(seg, mc, nq) launches one kernel that writes the chunk's k * nq frames into seg (mc is m with g0 at the
+// chunk's first index), the plan's own rfft turns them into spectra (at spec_out + k * q0 spectra, or in seg_ behind
+// the frames without spec_out), and use(spec, q0, nq, extra) runs the chunk's consumers, `extra` pointing at `extra`
+// bytes per index in seg_ behind the spectra, and adds their launches.
+template <typename T>
+template <class Gather, class Use>
+cudaError_t RealPlan<T>::frame_chunks(const real::FrameMap& m, size_t total, size_t k, C* spec_out, size_t extra,
+                                      cudaStream_t s, Gather gather, Use use) {
+  const size_t bins = n_ / 2 + 1, frame = n_ * sizeof(T), spectrum = bins * sizeof(C);
+  const size_t chunk = scratch_chunk(total, k * (frame + (spec_out ? 0 : spectrum)) + extra);
+  auto align = [](size_t bytes) { return (bytes + 255) / 256 * 256; };
+  const size_t spec_off = align(k * chunk * frame);
+  size_t end = spec_out ? k * chunk * frame : spec_off + k * chunk * spectrum;
+  const size_t extra_off = align(end);
+  if (extra) end = extra_off + chunk * extra;
+  FB_CHECK(seg_.reserve(end));
+  char* seg = (char*)seg_.data();
+  for (size_t q0 = 0; q0 < total; q0 += chunk) {
+    const size_t nq = std::min(chunk, total - q0);
+    real::FrameMap mc = m;
+    mc.g0 = (long)q0;
+    gather((T*)seg, mc, nq);
+    FB_CHECK(cudaGetLastError());
+    launches_ += 1;
+    C* spec = spec_out ? spec_out + k * q0 * bins : (C*)(seg + spec_off);
+    FB_CHECK(rfft_rows(true, seg, spec, k * nq, kFft, s));
+    FB_CHECK(use(spec, q0, nq, (T*)(seg + extra_off)));
+  }
   return cudaSuccess;
 }
 
@@ -782,29 +813,26 @@ cudaError_t RealPlan<T>::stft_device(const T* in, size_t in_len, const T* win, s
   launches_ = 0;
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
+  return stft_rows(in, in_len, win, hop, boundary, out, batch, s);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::stft_rows(const T* in, size_t in_len, const T* win, size_t hop, int boundary, C* out,
+                                   size_t batch, cudaStream_t s) {
   const real::FrameMap m = real::frame_map((long)n_, (long)in_len, (long)hop, boundary);
-  const size_t total = batch * (size_t)m.frames, bins = n_ / 2 + 1;
+  const size_t total = batch * (size_t)m.frames;
   if (path_ == Path::kRealFused) {
     FB_CHECK(fused_->stft(in, win, out, m, total, twa_.data(), (const C*)tab_.data(), sm_count_, s));
-    launches_ = 1;
+    launches_ += 1;
     return cudaSuccess;
   }
-  // chunks of frames through seg_: gather the windowed frames, then the plan's own rfft straight into the output rows
-  const size_t chunk = scratch_chunk(total, n_ * sizeof(T));
-  FB_CHECK(seg_.reserve(chunk * n_ * sizeof(T)));
-  T* seg = (T*)seg_.data();
-  unsigned long long count = 0;
-  for (size_t q0 = 0; q0 < total; q0 += chunk) {
-    const size_t nq = std::min(chunk, total - q0);
-    real::FrameMap mc = m;
-    mc.g0 = (long)q0;
-    gather_frames_kernel<T><<<grid_for(nq * n_), kThreads, 0, s>>>(in, win, seg, mc, (long)nq);
-    FB_CHECK(cudaGetLastError());
-    FB_CHECK(exec_device(true, seg, out + q0 * bins, nq, kFft, s));
-    count += 1 + launches_;
-  }
-  launches_ = count;
-  return cudaSuccess;
+  // the windowed frames, then the plan's own rfft straight into the output rows
+  return frame_chunks(
+      m, total, 1, out, 0, s,
+      [&](T* seg, const real::FrameMap& mc, size_t nq) {
+        gather_frames_kernel<T><<<grid_for(nq * n_), kThreads, 0, s>>>(in, win, seg, mc, (long)nq);
+      },
+      [](C*, size_t, size_t, T*) { return cudaSuccess; });
 }
 
 // Runs of frames through seg_ (real::istft_runs): each run's spectra are inverted there by the plan's own irfft, then
@@ -816,6 +844,12 @@ cudaError_t RealPlan<T>::istft_device(const C* in, size_t frames, const T* win, 
   launches_ = 0;
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
+  return istft_rows(in, frames, win, hop, center, out, out_len, batch, s);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::istft_rows(const C* in, size_t frames, const T* win, size_t hop, bool center, T* out,
+                                    size_t out_len, size_t batch, cudaStream_t s) {
   real::FrameMap m = real::frame_map((long)n_, (long)n_, (long)hop, real::kStftNone);
   m.pad = center ? (long)n_ / 2 : 0;
   m.frames = (long)frames;
@@ -825,20 +859,15 @@ cudaError_t RealPlan<T>::istft_device(const C* in, size_t frames, const T* win, 
   const size_t cap = real::istft_scratch_frames(scratch_chunk(batch * frames, n_ * sizeof(T)), n_, hop, frames);
   FB_CHECK(seg_.reserve(cap * n_ * sizeof(T)));
   T* seg = (T*)seg_.data();
-  unsigned long long count = 0;
-  const int e = real::istft_runs(n_, hop, (size_t)m.pad, frames, out_len, batch, cap,
-                                 [&](size_t gs, size_t ge, size_t b0, size_t nb, size_t i0, size_t i1) -> int {
-    FB_CHECK(exec_device(false, in + gs * bins, seg, ge - gs, kIfft, s));
-    count += launches_;
+  return (cudaError_t)real::istft_runs(n_, hop, (size_t)m.pad, frames, out_len, batch, cap,
+                                       [&](size_t gs, size_t ge, size_t b0, size_t nb, size_t i0, size_t i1) -> int {
+    FB_CHECK(rfft_rows(false, in + gs * bins, seg, ge - gs, kIfft, s));
     overlap_add_kernel<T><<<grid_for(nb * (i1 - i0)), kThreads, 0, s>>>(
         seg, win, out + b0 * out_len, m, (long)gs, (long)b0, (long)nb, (long)i0, (long)i1, (long)out_len);
     FB_CHECK(cudaGetLastError());
-    count += 1;
+    launches_ += 1;
     return 0;
   });
-  if (e) return (cudaError_t)e;
-  launches_ = count;
-  return cudaSuccess;
 }
 
 template <typename T>
@@ -851,7 +880,7 @@ cudaError_t RealPlan<T>::stft_host(const T* in, size_t in_len, const T* win, siz
   FB_CHECK(stage_consts(win, n_ * sizeof(T), &dwin));
   return stage_rows(in, out, batch, in_len * sizeof(T), stft_row_bytes(in_len, hop, boundary),
                     [&](const void* din, void* dout, size_t, size_t nb) {
-                      return stft_device((const T*)din, in_len, dwin, hop, boundary, (C*)dout, nb, host_stream_);
+                      return stft_rows((const T*)din, in_len, dwin, hop, boundary, (C*)dout, nb, host_stream_);
                     });
 }
 
@@ -865,8 +894,7 @@ cudaError_t RealPlan<T>::istft_host(const C* in, size_t frames, const T* win, si
   FB_CHECK(stage_consts(win, n_ * sizeof(T), &dwin));
   return stage_rows(in, out, batch, spec_bytes(frames), out_len * sizeof(T),
                     [&](const void* din, void* dout, size_t, size_t nb) {
-                      return istft_device((const C*)din, frames, dwin, hop, center, (T*)dout, out_len, nb,
-                                          host_stream_);
+                      return istft_rows((const C*)din, frames, dwin, hop, center, (T*)dout, out_len, nb, host_stream_);
                     });
 }
 
@@ -882,39 +910,30 @@ cudaError_t RealPlan<T>::mel_bands(const T* filters, size_t n_mels, cudaStream_t
 }
 
 template <typename T>
-cudaError_t RealPlan<T>::mel_frames(const T* in, size_t in_len, const T* win, size_t hop, int boundary,
-                                    const T* filters, size_t n_mels, int power, T* out, size_t batch, cudaStream_t s) {
+cudaError_t RealPlan<T>::mel_rows(const T* in, size_t in_len, const T* win, size_t hop, int boundary, const T* filters,
+                                  size_t n_mels, int power, T* out, size_t batch, cudaStream_t s) {
   const real::FrameMap m = real::frame_map((long)n_, (long)in_len, (long)hop, boundary);
   const size_t total = batch * (size_t)m.frames, bins = n_ / 2 + 1;
   const real::Band* bands = (const real::Band*)bands_.data();
   if (path_ == Path::kRealFused) {
     FB_CHECK(fused_->mel(in, win, filters, bands, n_mels, power, out, m, total, twa_.data(), (const C*)tab_.data(),
                          sm_count_, s));
-    launches_ = 1;
+    launches_ += 1;
     return cudaSuccess;
   }
-  // chunks of frames through seg_: the windowed frames, then their spectra from the plan's own rfft behind them, then
-  // the mels of those spectra straight into the output rows
-  const size_t chunk = scratch_chunk(total, n_ * sizeof(T) + bins * sizeof(C));
-  const size_t spec_off = (chunk * n_ * sizeof(T) + 255) / 256 * 256;
-  FB_CHECK(seg_.reserve(spec_off + chunk * bins * sizeof(C)));
-  T* seg = (T*)seg_.data();
-  C* spec = (C*)((char*)seg_.data() + spec_off);
-  unsigned long long count = 0;
-  for (size_t q0 = 0; q0 < total; q0 += chunk) {
-    const size_t nq = std::min(chunk, total - q0);
-    real::FrameMap mc = m;
-    mc.g0 = (long)q0;
-    gather_frames_kernel<T><<<grid_for(nq * n_), kThreads, 0, s>>>(in, win, seg, mc, (long)nq);
-    FB_CHECK(cudaGetLastError());
-    FB_CHECK(exec_device(true, seg, spec, nq, kFft, s));
-    count += 2 + launches_;
-    mel_spectra_kernel<T><<<grid_for(nq * n_mels), kThreads, 0, s>>>(spec, filters, bands, (long)bins, (long)n_mels,
-                                                                      power, out + q0 * n_mels, (long)nq, (long)q0);
-    FB_CHECK(cudaGetLastError());
-  }
-  launches_ = count;
-  return cudaSuccess;
+  // the windowed frames, their spectra behind them, then the mels of those spectra straight into the output rows
+  return frame_chunks(
+      m, total, 1, nullptr, 0, s,
+      [&](T* seg, const real::FrameMap& mc, size_t nq) {
+        gather_frames_kernel<T><<<grid_for(nq * n_), kThreads, 0, s>>>(in, win, seg, mc, (long)nq);
+      },
+      [&](C* spec, size_t q0, size_t nq, T*) {
+        mel_spectra_kernel<T><<<grid_for(nq * n_mels), kThreads, 0, s>>>(
+            spec, filters, bands, (long)bins, (long)n_mels, power, out + q0 * n_mels, (long)nq, (long)q0);
+        FB_CHECK(cudaGetLastError());
+        launches_ += 1;
+        return cudaSuccess;
+      });
 }
 
 template <typename T>
@@ -924,9 +943,7 @@ cudaError_t RealPlan<T>::mel_device(const T* in, size_t in_len, const T* win, si
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
   FB_CHECK(mel_bands(filters, n_mels, s));
-  FB_CHECK(mel_frames(in, in_len, win, hop, boundary, filters, n_mels, power, out, batch, s));
-  launches_ += 1;
-  return cudaSuccess;
+  return mel_rows(in, in_len, win, hop, boundary, filters, n_mels, power, out, batch, s);
 }
 
 template <typename T>
@@ -938,13 +955,11 @@ cudaError_t RealPlan<T>::mel_host(const T* in, size_t in_len, const T* win, size
   const T *dwin, *dfilt;
   FB_CHECK(stage_consts(win, n_ * sizeof(T), &dwin, filters, n_mels * (n_ / 2 + 1) * sizeof(T), &dfilt));
   FB_CHECK(mel_bands(dfilt, n_mels, host_stream_));
-  FB_CHECK(stage_rows(in, out, batch, in_len * sizeof(T), mel_row_bytes(in_len, hop, boundary, n_mels),
-                      [&](const void* din, void* dout, size_t, size_t nb) {
-                        return mel_frames((const T*)din, in_len, dwin, hop, boundary, dfilt, n_mels, power, (T*)dout,
-                                          nb, host_stream_);
-                      }));
-  launches_ += 1;
-  return cudaSuccess;
+  return stage_rows(in, out, batch, in_len * sizeof(T), mel_row_bytes(in_len, hop, boundary, n_mels),
+                    [&](const void* din, void* dout, size_t, size_t nb) {
+                      return mel_rows((const T*)din, in_len, dwin, hop, boundary, dfilt, n_mels, power, (T*)dout, nb,
+                                      host_stream_);
+                    });
 }
 
 template <typename T>
@@ -973,9 +988,9 @@ cudaError_t RealPlan<T>::mfcc_args(double log_offset, double log_floor, double l
 }
 
 template <typename T>
-cudaError_t RealPlan<T>::mfcc_frames(const T* in, size_t in_len, const T* win, size_t hop, int boundary, int power,
-                                     const T* filters, size_t n_mels, const real::MfccArgs<T>& p, bool max_sweep,
-                                     T* out, size_t batch, cudaStream_t s) {
+cudaError_t RealPlan<T>::mfcc_rows(const T* in, size_t in_len, const T* win, size_t hop, int boundary, int power,
+                                   const T* filters, size_t n_mels, const real::MfccArgs<T>& p, bool max_sweep, T* out,
+                                   size_t batch, cudaStream_t s) {
   const real::FrameMap m = real::frame_map((long)n_, (long)in_len, (long)hop, boundary);
   const size_t total = batch * (size_t)m.frames, bins = n_ / 2 + 1;
   const real::Band* bands = (const real::Band*)bands_.data();
@@ -985,39 +1000,27 @@ cudaError_t RealPlan<T>::mfcc_frames(const T* in, size_t in_len, const T* win, s
     launches_ += 1;
     return cudaSuccess;
   }
-  // chunks of frames through seg_ as in mel_frames, the mels into a third region behind the spectra, then
-  // mfcc_frames_kernel from there
-  const size_t chunk = scratch_chunk(total, n_ * sizeof(T) + bins * sizeof(C) + n_mels * sizeof(T));
-  const size_t spec_off = (chunk * n_ * sizeof(T) + 255) / 256 * 256;
-  const size_t mel_off = spec_off + (chunk * bins * sizeof(C) + 255) / 256 * 256;
-  FB_CHECK(seg_.reserve(mel_off + chunk * n_mels * sizeof(T)));
-  T* seg = (T*)seg_.data();
-  C* spec = (C*)((char*)seg_.data() + spec_off);
-  T* mel = (T*)((char*)seg_.data() + mel_off);
-  const unsigned long long before = launches_;
-  unsigned long long count = 0;
-  for (size_t q0 = 0; q0 < total; q0 += chunk) {
-    const size_t nq = std::min(chunk, total - q0);
-    real::FrameMap mc = m;
-    mc.g0 = (long)q0;
-    gather_frames_kernel<T><<<grid_for(nq * n_), kThreads, 0, s>>>(in, win, seg, mc, (long)nq);
-    FB_CHECK(cudaGetLastError());
-    FB_CHECK(exec_device(true, seg, spec, nq, kFft, s));
-    count += 3 + launches_;
-    mel_spectra_kernel<T><<<grid_for(nq * n_mels), kThreads, 0, s>>>(spec, filters, bands, (long)bins, (long)n_mels,
-                                                                      power, mel, (long)nq, (long)q0);
-    FB_CHECK(cudaGetLastError());
-    const unsigned grid = (unsigned)std::min<size_t>(nq, (size_t)sm_count_ * 16);
-    if (max_sweep)
-      mfcc_frames_kernel<T, true><<<grid, kThreads, 0, s>>>(mel, (long)n_mels, p, nullptr, (long)nq, (long)q0,
-                                                            m.frames);
-    else
-      mfcc_frames_kernel<T, false><<<grid, kThreads, 0, s>>>(mel, (long)n_mels, p, out + q0 * p.n_out, (long)nq,
-                                                             (long)q0, m.frames);
-    FB_CHECK(cudaGetLastError());
-  }
-  launches_ = before + count;
-  return cudaSuccess;
+  // as in mel_rows, the mels into a third region behind the spectra, then mfcc_frames_kernel from there
+  return frame_chunks(
+      m, total, 1, nullptr, n_mels * sizeof(T), s,
+      [&](T* seg, const real::FrameMap& mc, size_t nq) {
+        gather_frames_kernel<T><<<grid_for(nq * n_), kThreads, 0, s>>>(in, win, seg, mc, (long)nq);
+      },
+      [&](C* spec, size_t q0, size_t nq, T* mel) {
+        mel_spectra_kernel<T><<<grid_for(nq * n_mels), kThreads, 0, s>>>(spec, filters, bands, (long)bins,
+                                                                          (long)n_mels, power, mel, (long)nq, (long)q0);
+        FB_CHECK(cudaGetLastError());
+        const unsigned grid = (unsigned)std::min<size_t>(nq, (size_t)sm_count_ * 16);
+        if (max_sweep)
+          mfcc_frames_kernel<T, true><<<grid, kThreads, 0, s>>>(mel, (long)n_mels, p, nullptr, (long)nq, (long)q0,
+                                                                m.frames);
+        else
+          mfcc_frames_kernel<T, false><<<grid, kThreads, 0, s>>>(mel, (long)n_mels, p, out + q0 * p.n_out, (long)nq,
+                                                                 (long)q0, m.frames);
+        FB_CHECK(cudaGetLastError());
+        launches_ += 2;
+        return cudaSuccess;
+      });
 }
 
 template <typename T>
@@ -1031,8 +1034,8 @@ cudaError_t RealPlan<T>::mfcc_device(const T* in, size_t in_len, const T* win, s
   real::MfccArgs<T> p;
   FB_CHECK(mfcc_args(log_offset, log_floor, log_scale, top_db, top_db_rows, dct, n_out, bias, batch, s, &p));
   FB_CHECK(mel_bands(filters, n_mels, s));
-  if (p.rows) FB_CHECK(mfcc_frames(in, in_len, win, hop, boundary, power, filters, n_mels, p, true, out, batch, s));
-  return mfcc_frames(in, in_len, win, hop, boundary, power, filters, n_mels, p, false, out, batch, s);
+  if (p.rows) FB_CHECK(mfcc_rows(in, in_len, win, hop, boundary, power, filters, n_mels, p, true, out, batch, s));
+  return mfcc_rows(in, in_len, win, hop, boundary, power, filters, n_mels, p, false, out, batch, s);
 }
 
 // The max sweep stages every row once more (through stage_rows with no output), in chunks of its own size: the group
@@ -1055,22 +1058,16 @@ cudaError_t RealPlan<T>::mfcc_host(const T* in, size_t in_len, const T* win, siz
   real::MfccArgs<T> p;
   FB_CHECK(mfcc_args(log_offset, log_floor, log_scale, top_db, top_db_rows, ddct, n_out, bias, batch, host_stream_, &p));
   FB_CHECK(mel_bands(dfilt, n_mels, host_stream_));
-  const unsigned long long setup = launches_;
-  unsigned long long sweeps = 0;
-  auto sweep = [&](bool max_sweep, void* dst, size_t out_row) -> cudaError_t {
-    FB_CHECK(stage_rows(in, dst, batch, in_len * sizeof(T), out_row, [&](const void* din, void* dout, size_t b0, size_t nb) {
+  auto sweep = [&](bool max_sweep, void* dst, size_t out_row) {
+    return stage_rows(in, dst, batch, in_len * sizeof(T), out_row, [&](const void* din, void* dout, size_t b0, size_t nb) {
       real::MfccArgs<T> pc = p;
       pc.row0 = (long)b0;
-      return mfcc_frames((const T*)din, in_len, dwin, hop, boundary, power, dfilt, n_mels, pc, max_sweep, (T*)dout, nb,
-                         host_stream_);
-    }));
-    sweeps += launches_;
-    return cudaSuccess;
+      return mfcc_rows((const T*)din, in_len, dwin, hop, boundary, power, dfilt, n_mels, pc, max_sweep, (T*)dout, nb,
+                       host_stream_);
+    });
   };
   if (p.rows) FB_CHECK(sweep(true, out, 0));
-  FB_CHECK(sweep(false, out, mel_row_bytes(in_len, hop, boundary, n_out)));
-  launches_ = setup + sweeps;
-  return cudaSuccess;
+  return sweep(false, out, mel_row_bytes(in_len, hop, boundary, n_out));
 }
 
 template <typename T>
@@ -1083,88 +1080,128 @@ cudaError_t RealPlan<T>::welch_scale(const T* win, int scaling, double fs, size_
 }
 
 template <typename T>
-cudaError_t RealPlan<T>::welch_rows(const T* in, size_t in_len, const T* win, size_t hop, int detrend, T* out,
-                                    size_t batch, cudaStream_t s) {
+cudaError_t RealPlan<T>::welch_cross_rows(const T* x, const T* y, size_t y_rows, size_t y_off, size_t in_len,
+                                          const T* win, size_t hop, int detrend, bool coh, void* out, size_t batch,
+                                          cudaStream_t s) {
   const real::FrameMap m = real::frame_map((long)n_, (long)in_len, (long)hop, real::kStftNone);
-  const size_t bins = n_ / 2 + 1, frames = (size_t)m.frames;
+  const size_t bins = n_ / 2 + 1, frames = (size_t)m.frames, k = y ? 2 : 1;
+  const size_t planes = !y ? 1 : coh ? real::kCoherencePlanes : real::kCsdPlanes;
+  const size_t out_row = bins * (y && !coh ? sizeof(C) : sizeof(T));
   const bool fused = path_ == Path::kRealFused;
-  const long cols = fused ? fused_->cols : 1;
+  const long cols = fused ? fused_->cols / (long)k : 1;
   const size_t items = (size_t)real::welch_items(m.frames, cols, 1).items;
   // the fused kernel writes a row of one item itself; every other row goes through partials and the finish
   const bool direct = fused && items == 1;
-  const size_t rows = direct ? batch : scratch_chunk(batch, items * bins * sizeof(T));
-  if (!direct) FB_CHECK(part_.reserve(rows * items * bins * sizeof(T)));
+  const size_t rows = direct ? batch : scratch_chunk(batch, items * planes * bins * sizeof(T));
+  if (!direct) FB_CHECK(part_.reserve(rows * items * planes * bins * sizeof(T)));
   T* part = (T*)part_.data();
   const T* base = (const T*)welch_base_.data();
-  unsigned long long count = launches_;
   for (size_t r0 = 0; r0 < batch; r0 += rows) {
-    const size_t nr = std::min(rows, batch - r0);
+    const size_t nr = std::min(rows, batch - r0), yo = (y_off + r0) % y_rows;
     const real::WelchItems w = real::welch_items(m.frames, cols, (long)nr);
-    const T* x = in + r0 * in_len;
-    T* y = out + r0 * bins;
+    const T* xr = x + r0 * in_len;
+    void* o = (char*)out + r0 * out_row;
     if (fused) {
-      FB_CHECK(fused_->welch(x, win, base, detrend, part, y, m, w, twa_.data(), (const C*)tab_.data(), sm_count_, s));
-      count += 1;
+      if (y)
+        FB_CHECK(fused_->csd(xr, y, y_rows, yo, win, base, detrend, coh, part, o, m, w, twa_.data(),
+                             (const C*)tab_.data(), sm_count_, s));
+      else
+        FB_CHECK(fused_->welch(xr, win, base, detrend, part, (T*)o, m, w, twa_.data(), (const C*)tab_.data(),
+                               sm_count_, s));
+      launches_ += 1;
     } else {
-      // chunks of frames through seg_: the detrended windowed frames, their spectra from the plan's own rfft behind
-      // them, and the items with frames in the chunk accumulated from there
-      const size_t total = nr * frames;
-      const size_t chunk = scratch_chunk(total, n_ * sizeof(T) + bins * sizeof(C));
-      const size_t spec_off = (chunk * n_ * sizeof(T) + 255) / 256 * 256;
-      FB_CHECK(seg_.reserve(spec_off + chunk * bins * sizeof(C)));
-      T* seg = (T*)seg_.data();
-      C* spec = (C*)((char*)seg_.data() + spec_off);
-      for (size_t q0 = 0; q0 < total; q0 += chunk) {
-        const size_t nq = std::min(chunk, total - q0);
-        real::FrameMap mc = m;
-        mc.g0 = (long)q0;
-        welch_gather_kernel<T><<<(unsigned)std::min<size_t>(nq, 132u * 32u), kThreads, 0, s>>>(x, win, seg, mc, (long)nq,
-                                                                                             detrend);
-        FB_CHECK(cudaGetLastError());
-        FB_CHECK(exec_device(true, seg, spec, nq, kFft, s));
-        count += 2 + launches_;
-        auto item_of = [&](size_t q) { return (q / frames) * items + (q % frames) / (size_t)w.block; };
-        const size_t i0 = item_of(q0), ni = item_of(q0 + nq - 1) + 1 - i0;
-        welch_accumulate_kernel<T><<<grid_for(ni * bins), kThreads, 0, s>>>(spec, w, (long)bins, (long)q0, (long)nq,
-                                                                            (long)i0, (long)ni, part);
-        FB_CHECK(cudaGetLastError());
-      }
+      // the detrended windowed frames (x frames, then their y frames), their spectra behind them, and the items with
+      // frames in the chunk accumulated from there
+      auto item_of = [&](size_t q) { return (q / frames) * items + (q % frames) / (size_t)w.block; };
+      FB_CHECK(frame_chunks(
+          m, nr * frames, k, nullptr, 0, s,
+          [&](T* seg, const real::FrameMap& mc, size_t nq) {
+            const unsigned grid = (unsigned)std::min<size_t>(nq, 132u * 32u);
+            if (y)
+              csd_gather_kernel<T><<<grid, kThreads, 0, s>>>(xr, y, (long)y_rows, (long)yo, win, seg, mc, (long)nq,
+                                                             detrend);
+            else
+              welch_gather_kernel<T><<<grid, kThreads, 0, s>>>(xr, win, seg, mc, (long)nq, detrend);
+          },
+          [&](C* spec, size_t q0, size_t nq, T*) {
+            const size_t i0 = item_of(q0), ni = item_of(q0 + nq - 1) + 1 - i0;
+            if (y)
+              cross_accumulate_kernel<T><<<grid_for(ni * bins), kThreads, 0, s>>>(
+                  spec, spec + nq * bins, w, (long)bins, (long)q0, (long)nq, (long)i0, (long)ni, (int)planes, part);
+            else
+              welch_accumulate_kernel<T><<<grid_for(ni * bins), kThreads, 0, s>>>(spec, w, (long)bins, (long)q0,
+                                                                                  (long)nq, (long)i0, (long)ni, part);
+            FB_CHECK(cudaGetLastError());
+            launches_ += 1;
+            return cudaSuccess;
+          }));
     }
     if (!direct) {
-      welch_finish_kernel<T><<<grid_for(nr * bins), kThreads, 0, s>>>(part, (long)items, (long)n_, base, y, (long)nr);
+      if (y)
+        cross_finish_kernel<T><<<grid_for(nr * bins), kThreads, 0, s>>>(part, (long)items, (long)n_, base, coh, o,
+                                                                         (long)nr);
+      else
+        welch_finish_kernel<T><<<grid_for(nr * bins), kThreads, 0, s>>>(part, (long)items, (long)n_, base, (T*)o,
+                                                                         (long)nr);
       FB_CHECK(cudaGetLastError());
-      count += 1;
+      launches_ += 1;
     }
   }
-  launches_ = count;
   return cudaSuccess;
 }
 
 template <typename T>
 cudaError_t RealPlan<T>::welch_device(const T* in, size_t in_len, const T* win, size_t hop, int detrend, int scaling,
                                       double fs, T* out, size_t batch, cudaStream_t s) {
-  launches_ = 0;
-  if (batch == 0) return cudaSuccess;
-  DeviceGuard g(device_);
-  FB_CHECK(welch_scale(win, scaling, fs, frame_count(in_len, hop, real::kStftNone), s));
-  return welch_rows(in, in_len, win, hop, detrend, out, batch, s);
+  return cross_device(in, nullptr, 1, in_len, win, hop, detrend, false, scaling, fs, out, batch, s);
 }
 
 template <typename T>
 cudaError_t RealPlan<T>::welch_host(const T* in, size_t in_len, const T* win, size_t hop, int detrend, int scaling,
                                     double fs, T* out, size_t batch) {
+  return cross_host(in, nullptr, 1, in_len, win, hop, detrend, false, scaling, fs, out, batch);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::cross_device(const T* x, const T* y, size_t y_rows, size_t in_len, const T* win, size_t hop,
+                                      int detrend, bool coh, int scaling, double fs, void* out, size_t batch,
+                                      cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  if (!coh) FB_CHECK(welch_scale(win, scaling, fs, frame_count(in_len, hop, real::kStftNone), s));
+  return welch_cross_rows(x, y, y_rows, 0, in_len, win, hop, detrend, coh, out, batch, s);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::cross_host(const T* x, const T* y, size_t y_rows, size_t in_len, const T* win, size_t hop,
+                                    int detrend, bool coh, int scaling, double fs, void* out, size_t batch) {
   launches_ = 0;
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
   const T* dwin;
   FB_CHECK(stage_consts(win, n_ * sizeof(T), &dwin));
-  FB_CHECK(welch_scale(dwin, scaling, fs, frame_count(in_len, hop, real::kStftNone), host_stream_));
-  FB_CHECK(stage_rows(in, out, batch, in_len * sizeof(T), (n_ / 2 + 1) * sizeof(T),
-                      [&](const void* din, void* dout, size_t, size_t nb) {
-                        return welch_rows((const T*)din, in_len, dwin, hop, detrend, (T*)dout, nb, host_stream_);
-                      }));
-  launches_ += 1;
-  return cudaSuccess;
+  if (!coh) FB_CHECK(welch_scale(dwin, scaling, fs, frame_count(in_len, hop, real::kStftNone), host_stream_));
+  const size_t row = in_len * sizeof(T), bins = n_ / 2 + 1;
+  return stage_rows(x, out, batch, row, bins * (y && !coh ? sizeof(C) : sizeof(T)),
+                    [&](const void* din, void* dout, size_t b0, size_t nb) {
+                      // y rows (b0 + j) mod y_rows, j < cnt, in one or two runs: row b of the chunk pairs with j =
+                      // b mod cnt
+                      const T* dy = nullptr;
+                      const size_t cnt = std::min(nb, y_rows), first = b0 % y_rows;
+                      if (y) {
+                        const size_t run = std::min(cnt, y_rows - first);
+                        FB_CHECK(stage_y_.reserve(cnt * row));
+                        FB_CHECK(cudaMemcpyAsync(stage_y_.data(), y + first * in_len, run * row,
+                                                 cudaMemcpyHostToDevice, host_stream_));
+                        if (run < cnt)
+                          FB_CHECK(cudaMemcpyAsync((char*)stage_y_.data() + run * row, y, (cnt - run) * row,
+                                                   cudaMemcpyHostToDevice, host_stream_));
+                        dy = (const T*)stage_y_.data();
+                      }
+                      return welch_cross_rows((const T*)din, dy, cnt, 0, in_len, dwin, hop, detrend, coh, dout, nb,
+                                              host_stream_);
+                    });
 }
 
 template <typename T>
@@ -1172,6 +1209,11 @@ cudaError_t RealPlan<T>::dct_device(const T* in, T* out, size_t batch, int type,
   launches_ = 0;
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
+  return dct_rows(in, out, batch, type, norm, s);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::dct_rows(const T* in, T* out, size_t batch, int type, int norm, cudaStream_t s) {
   double hd, h0d;
   real::dct_scales(type, norm, (long)n_, hd, h0d);
   const T h = (T)hd, h0 = (T)h0d;
@@ -1179,7 +1221,7 @@ cudaError_t RealPlan<T>::dct_device(const T* in, T* out, size_t batch, int type,
   const C* tab = (const C*)tab_.data();
   if (path_ == Path::kRealFused) {
     FB_CHECK(fused_->dct(in, out, type, twa_.data(), tab, wq, batch, h, h0, sm_count_, s));
-    launches_ = 1;
+    launches_ += 1;
     return cudaSuccess;
   }
   // chunks of rows through seg_: N reals per row (half length) or N complex values (full length); the first kernel reads
@@ -1189,7 +1231,6 @@ cudaError_t RealPlan<T>::dct_device(const T* in, T* out, size_t batch, int type,
   const size_t chunk = scratch_chunk(batch, row);
   FB_CHECK(seg_.reserve(chunk * row));
   void* seg = seg_.data();
-  unsigned long long count = 0;
   for (size_t b0 = 0; b0 < batch; b0 += chunk) {
     const size_t nb = std::min(chunk, batch - b0);
     const T* x = in + b0 * n_;
@@ -1222,9 +1263,8 @@ cudaError_t RealPlan<T>::dct_device(const T* in, T* out, size_t batch, int type,
       }
     }
     FB_CHECK(cudaGetLastError());
-    count += 2 + inner_->launches();
+    launches_ += 2 + inner_->launches();
   }
-  launches_ = count;
   return cudaSuccess;
 }
 
@@ -1234,109 +1274,8 @@ cudaError_t RealPlan<T>::dct_host(const T* in, T* out, size_t batch, int type, i
   if (batch == 0) return cudaSuccess;
   DeviceGuard g(device_);
   return stage_rows(in, out, batch, n_ * sizeof(T), n_ * sizeof(T), [&](const void* din, void* dout, size_t, size_t nb) {
-    return dct_device((const T*)din, (T*)dout, nb, type, norm, host_stream_);
+    return dct_rows((const T*)din, (T*)dout, nb, type, norm, host_stream_);
   });
-}
-
-template <typename T>
-cudaError_t RealPlan<T>::cross_rows(const T* x, const T* y, size_t y_rows, size_t y_off, size_t in_len, const T* win,
-                                    size_t hop, int detrend, bool coh, void* out, size_t batch, cudaStream_t s) {
-  const real::FrameMap m = real::frame_map((long)n_, (long)in_len, (long)hop, real::kStftNone);
-  const size_t bins = n_ / 2 + 1, frames = (size_t)m.frames;
-  const size_t planes = coh ? real::kCoherencePlanes : real::kCsdPlanes, out_row = bins * (coh ? sizeof(T) : sizeof(C));
-  const bool fused = path_ == Path::kRealFused;
-  const long cols = fused ? fused_->cols / 2 : 1;
-  const size_t items = (size_t)real::welch_items(m.frames, cols, 1).items;
-  // the fused kernel writes a row of one item itself; every other row goes through partials and the finish
-  const bool direct = fused && items == 1;
-  const size_t rows = direct ? batch : scratch_chunk(batch, items * planes * bins * sizeof(T));
-  if (!direct) FB_CHECK(part_.reserve(rows * items * planes * bins * sizeof(T)));
-  T* part = (T*)part_.data();
-  const T* base = (const T*)welch_base_.data();
-  unsigned long long count = launches_;
-  for (size_t r0 = 0; r0 < batch; r0 += rows) {
-    const size_t nr = std::min(rows, batch - r0), yo = (y_off + r0) % y_rows;
-    const real::WelchItems w = real::welch_items(m.frames, cols, (long)nr);
-    const T* xr = x + r0 * in_len;
-    void* o = (char*)out + r0 * out_row;
-    if (fused) {
-      FB_CHECK(fused_->csd(xr, y, y_rows, yo, win, base, detrend, coh, part, o, m, w, twa_.data(),
-                           (const C*)tab_.data(), sm_count_, s));
-      count += 1;
-    } else {
-      // chunks of frame pairs through seg_: the x frames, then their y frames, their spectra from the plan's own rfft
-      // behind them, and the items with frames in the chunk accumulated from there
-      const size_t total = nr * frames;
-      const size_t chunk = scratch_chunk(total, 2 * (n_ * sizeof(T) + bins * sizeof(C)));
-      const size_t spec_off = (2 * chunk * n_ * sizeof(T) + 255) / 256 * 256;
-      FB_CHECK(seg_.reserve(spec_off + 2 * chunk * bins * sizeof(C)));
-      T* seg = (T*)seg_.data();
-      C* spec = (C*)((char*)seg_.data() + spec_off);
-      for (size_t q0 = 0; q0 < total; q0 += chunk) {
-        const size_t nq = std::min(chunk, total - q0);
-        real::FrameMap mc = m;
-        mc.g0 = (long)q0;
-        csd_gather_kernel<T><<<(unsigned)std::min<size_t>(nq, 132u * 32u), kThreads, 0, s>>>(
-            xr, y, (long)y_rows, (long)yo, win, seg, mc, (long)nq, detrend);
-        FB_CHECK(cudaGetLastError());
-        FB_CHECK(exec_device(true, seg, spec, 2 * nq, kFft, s));
-        count += 2 + launches_;
-        auto item_of = [&](size_t q) { return (q / frames) * items + (q % frames) / (size_t)w.block; };
-        const size_t i0 = item_of(q0), ni = item_of(q0 + nq - 1) + 1 - i0;
-        cross_accumulate_kernel<T><<<grid_for(ni * bins), kThreads, 0, s>>>(
-            spec, spec + nq * bins, w, (long)bins, (long)q0, (long)nq, (long)i0, (long)ni, (int)planes, part);
-        FB_CHECK(cudaGetLastError());
-      }
-    }
-    if (!direct) {
-      cross_finish_kernel<T><<<grid_for(nr * bins), kThreads, 0, s>>>(part, (long)items, (long)n_, base, coh, o,
-                                                                       (long)nr);
-      FB_CHECK(cudaGetLastError());
-      count += 1;
-    }
-  }
-  launches_ = count;
-  return cudaSuccess;
-}
-
-template <typename T>
-cudaError_t RealPlan<T>::cross_device(const T* x, const T* y, size_t y_rows, size_t in_len, const T* win, size_t hop,
-                                      int detrend, bool coh, int scaling, double fs, void* out, size_t batch,
-                                      cudaStream_t s) {
-  launches_ = 0;
-  if (batch == 0) return cudaSuccess;
-  DeviceGuard g(device_);
-  if (!coh) FB_CHECK(welch_scale(win, scaling, fs, frame_count(in_len, hop, real::kStftNone), s));
-  return cross_rows(x, y, y_rows, 0, in_len, win, hop, detrend, coh, out, batch, s);
-}
-
-template <typename T>
-cudaError_t RealPlan<T>::cross_host(const T* x, const T* y, size_t y_rows, size_t in_len, const T* win, size_t hop,
-                                    int detrend, bool coh, int scaling, double fs, void* out, size_t batch) {
-  launches_ = 0;
-  if (batch == 0) return cudaSuccess;
-  DeviceGuard g(device_);
-  const T* dwin;
-  FB_CHECK(stage_consts(win, n_ * sizeof(T), &dwin));
-  if (!coh) FB_CHECK(welch_scale(dwin, scaling, fs, frame_count(in_len, hop, real::kStftNone), host_stream_));
-  const size_t row = in_len * sizeof(T), bins = n_ / 2 + 1;
-  FB_CHECK(stage_rows(x, out, batch, row, bins * (coh ? sizeof(T) : sizeof(C)),
-                      [&](const void* din, void* dout, size_t b0, size_t nb) {
-                        // y rows (b0 + j) mod y_rows, j < cnt, in one or two runs: row b of the chunk pairs with j =
-                        // b mod cnt
-                        const size_t cnt = std::min(nb, y_rows), first = b0 % y_rows;
-                        const size_t run = std::min(cnt, y_rows - first);
-                        FB_CHECK(stage_y_.reserve(cnt * row));
-                        FB_CHECK(cudaMemcpyAsync(stage_y_.data(), y + first * in_len, run * row,
-                                                 cudaMemcpyHostToDevice, host_stream_));
-                        if (run < cnt)
-                          FB_CHECK(cudaMemcpyAsync((char*)stage_y_.data() + run * row, y, (cnt - run) * row,
-                                                   cudaMemcpyHostToDevice, host_stream_));
-                        return cross_rows((const T*)din, (const T*)stage_y_.data(), cnt, 0, in_len, dwin, hop, detrend,
-                                          coh, dout, nb, host_stream_);
-                      }));
-  launches_ += coh ? 0 : 1;
-  return cudaSuccess;
 }
 
 template class RealPlan<float>;

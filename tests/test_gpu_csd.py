@@ -117,6 +117,13 @@ def launches(p):
     return p.info()["last_launches"]
 
 
+def rfft_launches(p, rows):
+    torch = torch_mod()
+    p.rfft(torch.zeros(rows, p.size(), dtype=tdt(p.real), device="cuda"),
+           torch.empty(rows, p.size() // 2 + 1, dtype=tdt(p.real, True), device="cuda"))
+    return launches(p)
+
+
 def row_len(n, hop, frames):
     return n + (frames - 1) * hop + hop // 2
 
@@ -282,7 +289,7 @@ def test_async_on_a_side_stream():
 
 def test_real_half_two_scratch_chunks():
     """60 rows of 2998 frame pairs at N = 400: two frames and two spectra of 3208 bytes each per pair fill the 512 MB
-    scratch after 83677 pairs, and the item of 12 frames that straddles the cut is continued in the second chunk"""
+    scratch after 83676 pairs, and the item of 12 frames that straddles the cut is continued in the second chunk"""
     p = plan("f32", 400)
     rows = 60
     x = reals("f32", (rows, 480000), 33, dc=0.5)
@@ -292,7 +299,11 @@ def test_real_half_two_scratch_chunks():
     frames = 1 + (480000 - 400) // 160
     chunk = (512 << 20) // (2 * (400 * 4 + 201 * 8))
     assert chunk < rows * frames and (chunk % frames) % 12 != 0
-    assert launches(p) > 2 + 2 * 3
+    n = launches(p)
+    total = rows * frames
+    # the scale; per scratch chunk the gather, the plan's rfft of its frames of x and y, and the accumulate; the finish
+    nqs = [min(chunk, total - q0) for q0 in range(0, total, chunk)]
+    assert n == 1 + sum(2 + rfft_launches(p, 2 * nq) for nq in nqs) + 1
     for r in (0, chunk // frames, chunk // frames + 1, rows - 1):
         assert row_err(got[r:r + 1], ref_csd(x[r:r + 1], y, w, 160)) < TOL["f32"], r
 
