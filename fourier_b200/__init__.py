@@ -35,6 +35,10 @@ reference's operator interface name for name:
     (no counterpart)                                      RealFft.dct / idct: discrete cosine transforms of real
                                                             rows, types 2 and 3 (scipy.fft.dct / idct; torch has
                                                             none)
+    (no counterpart)                                      RealFft.hilbert: analytic signal of real rows
+                                                            (scipy.signal.hilbert; torch has none)
+    (no counterpart)                                      RealFft.envelope: its modulus, the amplitude envelope
+                                                            (numpy.abs(scipy.signal.hilbert))
 
 Buffers are numpy arrays (host memory: staged over PCIe by the library) or torch CUDA tensors
 (device memory: transformed in HBM on torch's current stream).  A leading batch dimension is
@@ -566,6 +570,31 @@ class RealFft:
             raise ValueError(f"type must be 2 or 3, got {type!r}")
         swapped = {"backward": "forward", "forward": "backward", "ortho": "ortho"}[norm]
         self.dct(input, output, type=5 - type, norm=swapped)
+
+    def hilbert(self, input, output):
+        """output = scipy.signal.hilbert(input, axis=-1): the analytic signal x + i y of every row of `input` (shape
+        (..., N), real dtype), y = irfft(G * rfft(x), n=N) with G = -i on the bins 0 < k < N/2 and 0 at k = 0 and
+        (N even) N/2.  `output` is complex with the input's shape and must not overlap it.  Its real part is a copy of
+        the input, bit for bit."""
+        self._hilbert(input, output, "spec", 0)
+
+    def envelope(self, input, output):
+        """output = numpy.abs(scipy.signal.hilbert(input, axis=-1)): the amplitude envelope sqrt(x^2 + y^2) of every
+        row of `input` (shape (..., N), real dtype).  `output` is real with the input's shape and may be `input`."""
+        self._hilbert(input, output, "real", 1)
+
+    def _hilbert(self, input, output, out_kind, code):
+        self._check_resolved(input, output)
+        pi, li, di, si = self._describe(input, "real")
+        po, lo, do_, _ = self._describe(output, out_kind, last=self._size)
+        if li != lo:
+            raise ValueError(f"input and output shapes differ: {li} and {lo}")
+        if di != do_:
+            raise ValueError("input and output must both be host or both be device buffers")
+        batch = int(np.prod(li, dtype=np.int64))
+        if batch == 0:
+            return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
+        self._call("hilbert", "hilbert" if code == 0 else "envelope", di, si, pi, po, batch, code)
 
     WELCH_SCALINGS = {"density": 0, "spectrum": 1}
     WELCH_DETRENDS = {False: 0, "constant": 1}

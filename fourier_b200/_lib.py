@@ -37,7 +37,8 @@ EXTENSION_SYMBOLS = (
     + [f"fourier_b200_mfcc_{op}{t}" for t in ("float", "double") for op in ("", "async_")]
     + [f"fourier_b200_welch_{op}{t}" for t in ("float", "double") for op in ("", "async_")]
     + [f"fourier_b200_{fn}_{op}{t}" for fn in ("csd", "coherence") for t in ("float", "double") for op in ("", "async_")]
-    + [f"fourier_b200_dct_{op}{t}" for t in ("float", "double") for op in ("", "async_")])
+    + [f"fourier_b200_dct_{op}{t}" for t in ("float", "double") for op in ("", "async_")]
+    + [f"fourier_b200_hilbert_{op}{t}" for t in ("float", "double") for op in ("", "async_")])
 
 
 def load():
@@ -108,6 +109,8 @@ def load():
         getattr(L, f"fourier_b200_coherence_async_{t}").argtypes = [vp, vp, vp, sz, sz, vp, sz, ci, vp, sz, vp]
         getattr(L, f"fourier_b200_dct_{t}").argtypes = [vp, vp, vp, sz, ci, ci]
         getattr(L, f"fourier_b200_dct_async_{t}").argtypes = [vp, vp, vp, sz, ci, ci, vp]
+        getattr(L, f"fourier_b200_hilbert_{t}").argtypes = [vp, vp, vp, sz, ci]
+        getattr(L, f"fourier_b200_hilbert_async_{t}").argtypes = [vp, vp, vp, sz, ci, vp]
     L.fourier_b200_peer_alloc.argtypes = [sz, ctypes.POINTER(vp), ctypes.c_char_p]
     L.fourier_b200_peer_open.argtypes = [ctypes.c_char_p, ctypes.POINTER(vp)]
     L.fourier_b200_peer_close.argtypes = [vp]

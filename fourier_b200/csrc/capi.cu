@@ -451,6 +451,37 @@ int dct_exec(void* plan, const T* in, T* out, size_t batch, int type, int norm, 
       {in, out}, [&](cudaStream_t s) { return p->dct_device(in, out, batch, type, norm, s); });
 }
 
+// Analytic signal and envelope of real rows: the arguments and the output kind checked before the plan is touched, even
+// for batch == 0; the envelope may run in place (in == out), the analytic signal is out of place, and any other overlap
+// is refused.
+template <typename T>
+int hilbert_exec(void* plan, const T* in, void* out, size_t batch, int output, bool async, void* stream) {
+  const char* bad = !plan ? "null argument: plan"
+                    : !in ? "null argument: in"
+                    : !out ? "null argument: out"
+                    : output != fb200::real::kHilbertAnalytic && output != fb200::real::kHilbertEnvelope
+                        ? "unknown output (FOURIER_B200_HILBERT_ANALYTIC or _ENVELOPE)"
+                        : nullptr;
+  if (bad) { fb200::set_last_error(bad); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  const bool env = output == fb200::real::kHilbertEnvelope;
+  return run_call(
+      "hilbert", async, stream,
+      [&] {
+        if (batch == 0) return (int)p->hilbert_device(in, out, 0, output, nullptr);
+        const size_t in_bytes = batch * p->size() * sizeof(T), out_bytes = env ? in_bytes : 2 * in_bytes;
+        if (!(env && (const void*)in == out) && ranges_meet(in, in_bytes, out, out_bytes)) {
+          fb200::set_last_error(env ? "input and output overlap (the envelope runs in place or on disjoint buffers)"
+                                    : "input and output overlap (the analytic signal is out of place only)");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {in, out}, "input and output must both be host or both be device memory",
+      [&] { return p->hilbert_host(in, out, batch, output); },
+      {in, out}, [&](cudaStream_t s) { return p->hilbert_device(in, out, batch, output, s); });
+}
+
 // Cross-spectral density (coh false) and coherence of real rows: welch_exec's rules for x, the window, hop, detrend
 // (and for the csd scaling and fs), plus y and y_rows, checked before the plan is touched; y may overlap x.
 template <typename T>
@@ -949,6 +980,21 @@ int fourier_b200_coherence_async_double(fourier_b200_rfft_double* plan, const do
                                    double* out_dev, size_t batch, void* stream) {
   return cross_exec<double>(plan, x_dev, y_dev, y_rows, in_len, window_dev, hop, detrend, true, 0, 1.0, out_dev, batch,
                            true, stream);
+}
+
+int fourier_b200_hilbert_float(fourier_b200_rfft_float* plan, const float* in, void* out, size_t batch, int output) {
+  return hilbert_exec<float>(plan, in, out, batch, output, false, nullptr);
+}
+int fourier_b200_hilbert_double(fourier_b200_rfft_double* plan, const double* in, void* out, size_t batch, int output) {
+  return hilbert_exec<double>(plan, in, out, batch, output, false, nullptr);
+}
+int fourier_b200_hilbert_async_float(fourier_b200_rfft_float* plan, const float* in_dev, void* out_dev, size_t batch,
+                                     int output, void* stream) {
+  return hilbert_exec<float>(plan, in_dev, out_dev, batch, output, true, stream);
+}
+int fourier_b200_hilbert_async_double(fourier_b200_rfft_double* plan, const double* in_dev, void* out_dev, size_t batch,
+                                      int output, void* stream) {
+  return hilbert_exec<double>(plan, in_dev, out_dev, batch, output, true, stream);
 }
 
 const char* fourier_b200_last_error(void) { return fb200::last_error(); }

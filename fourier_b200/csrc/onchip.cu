@@ -107,6 +107,8 @@ struct OnChipImpl {
     if ((e = allow_smem(onchip::onchip_mfcc_kernel<Cfg<true>, MINB, false>))) return e;
     if ((e = allow_smem(onchip::onchip_dct_kernel<Cfg<true>, MINB, 2>))) return e;
     if ((e = allow_smem(onchip::onchip_dct_kernel<Cfg<true>, MINB, 3>))) return e;
+    if ((e = allow_smem(onchip::onchip_hilbert_kernel<Cfg<true>, MINB, false>))) return e;
+    if ((e = allow_smem(onchip::onchip_hilbert_kernel<Cfg<true>, MINB, true>))) return e;
     if ((e = cudaFuncSetAttribute(onchip::onchip_csd_kernel<Cfg<true>, minb_csd(false), false>,
                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_csd(false)))) return e;
     if ((e = cudaFuncSetAttribute(onchip::onchip_csd_kernel<Cfg<true>, minb_csd(true), true>,
@@ -173,6 +175,16 @@ struct OnChipImpl {
     a.h0 = h0;
     if (type == 2) return launch(onchip::onchip_dct_kernel<Cfg<true>, MINB, 2>, a, batch, sms, s);
     return launch(onchip::onchip_dct_kernel<Cfg<true>, MINB, 3>, a, batch, sms, s);
+  }
+  static cudaError_t hilbert(const T* in, void* out, int output, const void* twa, const cpx<T>* tab, size_t batch, T h,
+                             int sms, cudaStream_t s) {
+    onchip::HilbertArgs<Cfg<true>> a;
+    static_cast<typename onchip::ConvBody<Cfg<true>>::Args&>(a) = {
+        (const cpx<T>*)in, nullptr, (const TwPair<T>*)twa, tab, nullptr, 1, 0, (long)batch, h, 1};
+    a.y = out;
+    if (output == real::kHilbertEnvelope)
+      return launch(onchip::onchip_hilbert_kernel<Cfg<true>, MINB, true>, a, batch, sms, s);
+    return launch(onchip::onchip_hilbert_kernel<Cfg<true>, MINB, false>, a, batch, sms, s);
   }
   static cudaError_t mel(const T* in, const T* win, const T* filters, const real::Band* bands, size_t n_mels, int power,
                          T* out, const real::FrameMap& m, size_t nframes, const void* twa, const cpx<T>* tab, int sms,
@@ -245,7 +257,7 @@ struct OnChipImpl {
   }
   static const OnChipOps<T>* ops() {
     static const RealOnChipOps<T> r = {RA, RB, Cfg<true>::C, &real_prepare, &real, &conv, &lconv, &stft, &mel, &mfcc,
-                                      &welch, &dct, &csd};
+                                      &welch, &dct, &csd, &hilbert};
     static const OnChipOps<T> o = {RA, RB, &prepare, &fft, kHasBluestein ? &bluestein : nullptr, &r};
     return &o;
   }

@@ -11,8 +11,9 @@
 //   * onchip_mel_kernel:      the stft's frames to mel energies: power and filter bank on chip.
 //   * onchip_mfcc_kernel:     the mel energies on to their logs, a clamp and a projection (MFCC, log-mel) on chip.
 //   * onchip_dct_kernel:      discrete cosine transforms (types II and III) of real rows of length 2L.
-//     (these eight run the phases of FftBody / RealBody / ConvBody / LinConvBody / StftBody / MelBody / MfccBody /
-//     Dct2Body / Dct3Body through run_onchip_groups, tilefft.cuh)
+//   * onchip_hilbert_kernel:  the analytic signal (Hilbert transform) or its envelope of real rows of length 2L.
+//     (these nine run the phases of FftBody / RealBody / ConvBody / LinConvBody / StftBody / MelBody / MfccBody /
+//     Dct2Body / Dct3Body / HilbertBody through run_onchip_groups, tilefft.cuh)
 //   * onchip_welch_kernel:    detrended, windowed frames to Welch's averaged power spectrum, summed on chip
 //                             (WelchBody through run_welch_groups, below).
 //   * onchip_csd_kernel:      Welch's frames of two signals in pairs to their cross-spectral density or coherence
@@ -1057,6 +1058,82 @@ template <class Cfg, int TYPE> using DctBody = typename DctBodyOf<Cfg, TYPE>::ty
 template <class Cfg, int MINB, int TYPE>
 __global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_dct_kernel(const typename Dct2Body<Cfg>::Args a) {
   run_onchip_groups<Cfg, DctBody<Cfg, TYPE>>(a);
+}
+
+// ---- fused analytic signal and envelope of real rows, N = 2L (real::hilbert_pair, DESIGN.md §4.19) -----------------
+// ConvBody's phases 0-5 as they are, with the pair step real::hilbert_pair (a fixed multiplier, no spectrum read) in
+// phase 3.  Then:
+//   * store (phase 6): ConvBody's gather + stage B leave y at the lane's stage-B positions p as conj(y[2p], y[2p+1]);
+//     the lane re-reads x[2p], x[2p+1] from the row (which the load just brought into L2) and writes, per position,
+//     (x[2p], y[2p]), (x[2p+1], y[2p+1]) as one 16-byte store in f32 (ANALYTIC), or the two moduli (ENV).
+// The re-reads go G positions at a time ahead of their stores, so a lane has G loads in flight rather than one.  Every
+// lane reads x only at the positions it stores, each before its store, and in and y are not __restrict__, so the
+// envelope may run in place (y == in).
+template <class Cfg> struct HilbertArgs : ConvBody<Cfg>::Args { void* y; };
+template <class Cfg, bool ENV> struct HilbertBody {
+  using Conv = ConvBody<Cfg>;
+  using Real = RealBody<Cfg>;
+  using Tile = typename Cfg::Tile;   // FWD = true
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  static constexpr int L = Cfg::L, TP = Tile::TP, RA = Tile::RA, RB = Tile::RB, E = Tile::E;
+  static constexpr int G = sizeof(T) == 4 && !ENV ? 8 : 4;
+  static_assert(RB % G == 0, "the re-reads go G stage-B registers at a time");
+  // Conv::Args with in = the rows (L complex values each), out = spec = nullptr, rows = per = 1 and h = 1 / (2N); y: the
+  // output rows, N complex values (analytic) or N reals (ENV) each
+  using Args = HilbertArgs<Cfg>;
+
+  static FB_HD void pairs(const Args& a, long grp, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const long b = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (b >= a.batch) return;
+    V* z = smem + Real::park(t);
+#pragma unroll 4
+    for (int j = 0; j < E / 2; ++j) real::hilbert_pair(z, (long)L, (long)(u + TP * j), a.tab, a.h);
+    if (u == 0) real::hilbert_pair(z, (long)L, (long)(L / 2), a.tab, a.h);
+  }
+  static FB_HD void store(Tile& f, const Args& a, long grp, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    f.template gather<true, typename Cfg::Lay>(t, smem);
+    f.stage_b();
+    const long b = grp * Cfg::C + Tile::template col_of<true>(t);
+    if (b >= a.batch) return;
+    const V* x = a.in + b * L;
+    V* y = reinterpret_cast<V*>(a.y) + (ENV ? b * L : b * 2 * L);
+    static_for<0, Tile::NB>([&](auto Cc) FB_LAMBDA {
+      constexpr int c = decltype(Cc)::value;
+      static_for<0, RB / G>([&](auto Gg) FB_LAMBDA {
+        constexpr int r0 = decltype(Gg)::value * G;
+        V xs[G];
+        static_for<0, G>([&](auto Rr) FB_LAMBDA {
+          constexpr int i = decltype(Rr)::value;
+          xs[i] = real::lin_ld(x + (u + TP * c) + RA * (r0 + i), b);
+        });
+        static_for<0, G>([&](auto Rr) FB_LAMBDA {
+          constexpr int i = decltype(Rr)::value;
+          const int p = (u + TP * c) + RA * (r0 + i);
+          const V v = cconj(f.v[c * RB + bitrev(r0 + i, ilog2(RB))]);
+          if constexpr (ENV)
+            real::lin_st(y + p, mk<T>(real::hilbert_mod(xs[i].x, v.x), real::hilbert_mod(xs[i].y, v.y)), b);
+          else
+            real::analytic_st2(y + 2 * p, xs[i], v, b);
+        });
+      });
+    });
+  }
+
+  // phase protocol (tilefft.cuh): ConvBody's phases 0-5 with the pair step of phase 3 replaced; store
+  static constexpr int kPhases = 7;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    if constexpr (P == 3) pairs(a, grp, t, smem);
+    else if constexpr (P < 6) Conv::template phase<P>(f, a, grp, t, smem, twa);
+    else store(f, a, grp, t, smem);
+  }
+};
+
+template <class Cfg, int MINB, bool ENV>
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_hilbert_kernel(const HilbertArgs<Cfg> a) {
+  run_onchip_groups<Cfg, HilbertBody<Cfg, ENV>>(a);
 }
 
 // ---- fused Bluestein -------------------------------------------------------------------------------------------

@@ -333,6 +333,10 @@ template <typename T> struct RealOnChipOps {
   cudaError_t (*csd)(const T* x, const T* y, size_t y_rows, size_t y_off, const T* win, const T* base, int detrend,
                      bool coh, T* part, void* out, const real::FrameMap& m, const real::WelchItems& w, const void* twa,
                      const cpx<T>* tab, int sms, cudaStream_t);
+  // hilbert(): the analytic signal or its envelope (output real::kHilbert*, DESIGN.md §4.19) of `batch` rows of N reals
+  // into N complex values or N reals per row, out == in allowed for the envelope; h = 1 / (2N)
+  cudaError_t (*hilbert)(const T* in, void* out, int output, const void* twa, const cpx<T>* tab, size_t batch, T h,
+                         int sms, cudaStream_t);
 };
 template <typename T> const RealOnChipOps<T>* real_onchip_lookup(size_t l);
 
@@ -449,6 +453,14 @@ class RealPlan {
   // Host pointers: whole rows through stage_rows; the same bits.
   cudaError_t dct_host(const T* in, T* out, size_t batch, int type, int norm);
 
+  // Analytic signal (DESIGN.md §4.19): `batch` rows of N reals -> scipy.signal.hilbert of each row, N complex values
+  // (x[n], y[n]) per row with the real part a copy of x (output real::kHilbertAnalytic), or its modulus, N reals per row
+  // (real::kHilbertEnvelope); checked by the caller.  in == out allowed for the envelope, else out of place.  Device
+  // pointers, on `stream`.
+  cudaError_t hilbert_device(const T* in, void* out, size_t batch, int output, cudaStream_t stream);
+  // Host pointers: whole rows through stage_rows; the same bits.
+  cudaError_t hilbert_host(const T* in, void* out, size_t batch, int output);
+
   unsigned long long launches() const { return launches_; }
   const char* kernel_name() const { return kernel_desc_.c_str(); }
 
@@ -495,6 +507,8 @@ class RealPlan {
   cudaError_t istft_rows(const C* in, size_t frames, const T* win, size_t hop, bool center, T* out, size_t out_len,
                          size_t batch, cudaStream_t s);
   cudaError_t dct_rows(const T* in, T* out, size_t batch, int type, int norm, cudaStream_t s);
+  // hilbert_device after its checks: the fused kernel, or chunks of rows through seg_ (half length) or work_ (full)
+  cudaError_t hilbert_rows(const T* in, void* out, size_t batch, int output, cudaStream_t s);
   // the band of every filter row into bands_ (one launch)
   cudaError_t mel_bands(const T* filters, size_t n_mels, cudaStream_t s);
   // mel_device after mel_bands: the fused kernel, or chunks of frames through seg_

@@ -29,6 +29,9 @@
 // kernel into seg_, the inner plan in place there and an O(N) kernel into the output: dct_permute_kernel, Fft and
 // dct_untangle_kernel (type 2) or dct_tangle_kernel, UnscaledIfft and dct_unpermute_kernel (type 3) at half length;
 // dct_widen_kernel, Fft and dct_post_kernel or dct_pre_kernel, UnscaledIfft and dct_unpermute_kernel at full length.
+// Analytic signal and envelope (DESIGN.md §4.19): onchip_hilbert_kernel on the fused path; otherwise per chunk of rows
+// through seg_: Fft of the rows read as M complex values, hilbert_pair_kernel, UnscaledIfft and hilbert_out_kernel at
+// half length; widen_kernel, Fft, hilbert_mul_kernel, UnscaledIfft and hilbert_out_kernel at full length.
 #include <algorithm>
 #include <string>
 #include <vector>
@@ -413,6 +416,37 @@ dct_unpermute_kernel(const void* __restrict__ seg, T* __restrict__ out, long n, 
   for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
     const long b = g / n, s = b * n + real::dct_pos(n, g - b * n);
     real::lin_st(out + g, WIDE ? ((const cpx<T>*)seg)[s].x : ((const T*)seg)[s], b);
+  }
+}
+
+// Analytic signal (real::hilbert_pair, hilbert_bin, hilbert_out_one).  pair: one thread per pair k <= M/2 of a row, in
+// place on z (M complex values per row).  mul: one thread per bin k < N of a row of length-N spectra, in place.  out: one
+// thread per output n of a row, from x[n] and y[n] (seg holds N reals per row at half length, N complex values whose
+// real parts are y at full length); it is the only kernel that writes `out`, so in == out is safe.
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+hilbert_pair_kernel(cpx<T>* __restrict__ z, const cpx<T>* __restrict__ tab, long m, long batch, T h) {
+  const long pairs = m / 2 + 1, total = pairs * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / pairs;
+    real::hilbert_pair(z + b * m, m, g - b * pairs, tab, h);
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+hilbert_mul_kernel(cpx<T>* __restrict__ y, long n, long batch, T s) {
+  const long total = n * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x)
+    y[g] = real::hilbert_bin(y[g], n, g - (g / n) * n, s);
+}
+template <typename T, bool WIDE>
+__global__ void __launch_bounds__(kThreads)
+hilbert_out_kernel(const T* in, const void* __restrict__ seg, void* out, long n, long batch, int output) {
+  const long total = n * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / n;
+    const T y = WIDE ? ((const cpx<T>*)seg)[g].x : ((const T*)seg)[g];
+    real::hilbert_out_one(real::lin_ld(in + g, b), y, out, g, output, b);
   }
 }
 
@@ -1275,6 +1309,72 @@ cudaError_t RealPlan<T>::dct_host(const T* in, T* out, size_t batch, int type, i
   DeviceGuard g(device_);
   return stage_rows(in, out, batch, n_ * sizeof(T), n_ * sizeof(T), [&](const void* din, void* dout, size_t, size_t nb) {
     return dct_rows((const T*)din, (T*)dout, nb, type, norm, host_stream_);
+  });
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::hilbert_device(const T* in, void* out, size_t batch, int output, cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  return hilbert_rows(in, out, batch, output, s);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::hilbert_rows(const T* in, void* out, size_t batch, int output, cudaStream_t s) {
+  const C* tab = (const C*)tab_.data();
+  if (path_ == Path::kRealFused) {
+    FB_CHECK(fused_->hilbert(in, out, output, twa_.data(), tab, batch, (T)1 / (T)(2 * n_), sm_count_, s));
+    launches_ += 1;
+    return cudaSuccess;
+  }
+  // chunks of rows through seg_: y of N reals per row (half length) or N complex values (full length); only the last
+  // kernel of a chunk writes its output rows, after reading their input, so in == out is safe
+  const bool half = path_ == Path::kRealHalf;
+  const size_t row = half ? n_ * sizeof(T) : n_ * sizeof(C);
+  const size_t out_row = output == real::kHilbertAnalytic ? n_ * sizeof(C) : n_ * sizeof(T);
+  const size_t chunk = scratch_chunk(batch, row);
+  FB_CHECK(seg_.reserve(chunk * row));
+  C* w = (C*)seg_.data();
+  for (size_t b0 = 0; b0 < batch; b0 += chunk) {
+    const size_t nb = std::min(chunk, batch - b0);
+    const T* x = in + b0 * n_;
+    void* y = (char*)out + b0 * out_row;
+    if (half) {
+      FB_CHECK(inner_->exec_device((const C*)x, w, nb, kFft, s));
+      launches_ += inner_->launches();
+      hilbert_pair_kernel<T><<<grid_for((m_ / 2 + 1) * nb), kThreads, 0, s>>>(w, tab, (long)m_, (long)nb,
+                                                                              (T)1 / (T)(2 * n_));
+      FB_CHECK(cudaGetLastError());
+      FB_CHECK(inner_->exec_device(w, w, nb, kUnscaledIfft, s));
+      launches_ += inner_->launches();
+      hilbert_out_kernel<T, false><<<grid_for(nb * n_), kThreads, 0, s>>>(x, w, y, (long)n_, (long)nb, output);
+    } else {
+      widen_kernel<T><<<grid_for(nb * n_), kThreads, 0, s>>>(x, w, nb * n_);
+      FB_CHECK(cudaGetLastError());
+      FB_CHECK(inner_->exec_device(w, w, nb, kFft, s));
+      launches_ += inner_->launches();
+      hilbert_mul_kernel<T><<<grid_for(nb * n_), kThreads, 0, s>>>(w, (long)n_, (long)nb, (T)1 / (T)n_);
+      FB_CHECK(cudaGetLastError());
+      FB_CHECK(inner_->exec_device(w, w, nb, kUnscaledIfft, s));
+      launches_ += inner_->launches();
+      hilbert_out_kernel<T, true><<<grid_for(nb * n_), kThreads, 0, s>>>(x, w, y, (long)n_, (long)nb, output);
+      launches_ += 1;
+    }
+    FB_CHECK(cudaGetLastError());
+    launches_ += 2;
+  }
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::hilbert_host(const T* in, void* out, size_t batch, int output) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  const size_t out_row = output == real::kHilbertAnalytic ? n_ * sizeof(C) : n_ * sizeof(T);
+  return stage_rows(in, out, batch, n_ * sizeof(T), out_row, [&](const void* din, void* dout, size_t, size_t nb) {
+    return hilbert_rows((const T*)din, dout, nb, output, host_stream_);
   });
 }
 

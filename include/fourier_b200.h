@@ -507,6 +507,36 @@ int fourier_b200_coherence_async_double(struct fourier_b200_rfft_double *plan, c
                                         const double *y_dev, size_t y_rows, size_t in_len, const double *window_dev,
                                         size_t hop, int detrend, double *out_dev, size_t batch, void *cuda_stream);
 
+/* ---- analytic signal and envelope of real rows (Hilbert transform) ----
+ * On a real plan of length N >= 1, for `batch` rows of N reals x (row b at element b*N):
+ *   y = irfft(G * rfft(x), n = N),  G[k] = -i (0 < k < N/2),  G[0] = 0,  G[N/2] = 0 (N even),
+ *   z = x + i y,
+ * which is scipy.signal.hilbert(x, axis=-1).  FOURIER_B200_HILBERT_ANALYTIC writes z, N complex values (x[n], y[n])
+ * interleaved per row (row b from complex element b*N on); FOURIER_B200_HILBERT_ENVELOPE writes |z[n]| =
+ * sqrt(x[n]^2 + y[n]^2), N reals per row (row b from real element b*N on).  The real part of the analytic output is a
+ * copy of x, bit for bit, on every path; scipy's equals x only up to rounding (it inverts the whole spectrum).  torch
+ * has no Hilbert transform.
+ * Launches: 1 on the real_fused path (N = 128 .. 2048 in f32, 128 .. 512 in f64); on real_half (other even N), per
+ * scratch chunk of rows (512 MB), 2 plus twice those of the inner complex plan of length N/2 (its forward and its
+ * unscaled inverse); on real_full (odd N), per scratch chunk, 3 plus twice those of the inner plan of length N.
+ * Refused with cudaErrorInvalidValue and a message naming the argument: a NULL argument and an output other than the
+ * two macros (these also when batch == 0, which otherwise succeeds and launches nothing); input and output overlapping,
+ * except in == out for the envelope, which runs in place (the analytic signal is out of place only); and a mix of host
+ * and device buffers in the synchronous calls.  Device base pointers must be 16-byte aligned
+ * (cudaErrorMisalignedAddress).  Host memory is staged through the plan's buffers in whole rows and gives the same bits
+ * as device memory.  The _async calls take device memory, are enqueued on `cuda_stream` and never synchronise the
+ * host. */
+#define FOURIER_B200_HILBERT_ANALYTIC 0
+#define FOURIER_B200_HILBERT_ENVELOPE 1
+int fourier_b200_hilbert_float(struct fourier_b200_rfft_float *plan, const float *in, void *out, size_t batch,
+                               int output);
+int fourier_b200_hilbert_double(struct fourier_b200_rfft_double *plan, const double *in, void *out, size_t batch,
+                                int output);
+int fourier_b200_hilbert_async_float(struct fourier_b200_rfft_float *plan, const float *in_dev, void *out_dev,
+                                     size_t batch, int output, void *cuda_stream);
+int fourier_b200_hilbert_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev, void *out_dev,
+                                      size_t batch, int output, void *cuda_stream);
+
 const char *fourier_b200_last_error(void);
 const char *fourier_b200_version(void);
 
