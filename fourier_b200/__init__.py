@@ -39,6 +39,11 @@ reference's operator interface name for name:
                                                             (scipy.signal.hilbert; torch has none)
     (no counterpart)                                      RealFft.envelope: its modulus, the amplitude envelope
                                                             (numpy.abs(scipy.signal.hilbert))
+    (no counterpart)                                      RealFft.dct4: the type-IV DCT of real rows
+                                                            (scipy.fft.dct(type=4))
+    (no counterpart)                                      RealFft.mdct / imdct / mdct_frames: the modified discrete
+                                                            cosine transform of real rows and its overlap-add inverse
+                                                            (tf.signal.mdct / inverse_mdct; torch has none)
 
 Buffers are numpy arrays (host memory: staged over PCIe by the library) or torch CUDA tensors
 (device memory: transformed in HBM on torch's current stream).  A leading batch dimension is
@@ -595,6 +600,101 @@ class RealFft:
         if batch == 0:
             return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
         self._call("hilbert", "hilbert" if code == 0 else "envelope", di, si, pi, po, batch, code)
+
+    def _check_norm(self, norm):
+        if not isinstance(norm, str) or norm not in self.DCT_NORMS:
+            raise ValueError(f"norm must be one of {sorted(self.DCT_NORMS)}, got {norm!r}")
+        if self._size % 2:
+            raise ValueError(f"the type-IV DCT and the MDCT need an even plan length, got N = {self._size}")
+        return self.DCT_NORMS[norm]
+
+    def dct4(self, input, output, norm="backward"):
+        """output = scipy.fft.dct(input, type=4, norm=norm) along the last axis: the type-IV DCT y[k] = 2 h sum_n x[n]
+        cos(pi (2n+1)(2k+1) / (4N)) of every row of `input` (shape (..., N), real dtype, N even), h = 1, 1/sqrt(2N) or
+        1/(2N) for the norms "backward", "ortho" and "forward".  `output` has the input's shape and may be `input`
+        itself.  The inverse is dct4 with "backward" and "forward" swapped (scipy.fft.idct(type=4)); "ortho" is its own
+        inverse."""
+        self._check_resolved(input, output)
+        code = self._check_norm(norm)
+        pi, li, di, si = self._describe(input, "real")
+        po, lo, do_, _ = self._describe(output, "real")
+        if li != lo:
+            raise ValueError(f"input and output shapes differ: {li} and {lo}")
+        if di != do_:
+            raise ValueError("input and output must both be host or both be device buffers")
+        batch = int(np.prod(li, dtype=np.int64))
+        if batch == 0:
+            return   # nothing to do; an empty torch tensor has no data pointer for the C entry point
+        self._call("dct4", "dct4", di, si, pi, po, batch, code)
+
+    def mdct_frames(self, in_len, center=True):
+        """F, the number of frames `mdct` makes of rows of in_len samples: ceil(in_len / N) + 1 with center, else
+        1 + (in_len - 2N) // N (in_len >= 2N)."""
+        n, in_len = self._size, int(in_len)
+        return -(-in_len // n) + 1 if center else 1 + (in_len - 2 * n) // n
+
+    def _mdct_window(self, window):
+        pw, lw, dw, _ = self._describe(window, "real", last=2 * self._size)
+        if lw != ():
+            raise ValueError(f"window must hold exactly 2N = {2 * self._size} reals, got shape {tuple(window.shape)}")
+        return pw, dw
+
+    def mdct(self, input, window, output, center=True, norm="backward"):
+        """The modified discrete cosine transform of every row of `input` (shape (..., L)): N = size() coefficients per
+        frame of 2N samples every N, X_f[k] = 2 h sum_s w[s] x[fN - pad + s] cos(pi/N (s + 1/2 + N/2)(k + 1/2)), h as
+        for dct4, `window` 2N reals.  center=True pads N zeros at both ends, so every sample lies in two frames
+        (F = ceil(L/N) + 1); center=False needs L >= 2N (F = 1 + (L - 2N) // N) and is tf.signal.mdct(x, 2N,
+        window_fn, pad_end=False).  `output` has shape (..., F, N), F = mdct_frames(L, center).  Out of place only."""
+        self._check_resolved(input, window, output)
+        code = self._check_norm(norm)
+        n = self._size
+        in_len = input.shape[-1] if getattr(input, "ndim", 0) > 0 else 0
+        if in_len < 1:
+            raise ValueError("input rows must hold at least one sample")
+        if not center and in_len < 2 * n:
+            raise ValueError(f"center=False needs rows of at least 2N = {2 * n} samples, got {in_len}")
+        frames = self.mdct_frames(in_len, center)
+        pi, li, di, si = self._describe(input, "real", last=in_len)
+        pw, dw = self._mdct_window(window)
+        if getattr(output, "ndim", 0) < 2 or output.shape[-2] != frames:
+            raise ValueError(f"output must have shape (..., {frames}, {n}) for rows of {in_len} samples")
+        po, lo, do_, _ = self._describe(output, "real")
+        if lo[:-1] != li:
+            raise ValueError(f"input and output leading shapes differ: {li} and {lo[:-1]}")
+        if not (di == dw == do_):
+            raise ValueError("input, window and output must all be host or all be device buffers")
+        batch = int(np.prod(li, dtype=np.int64))
+        if batch == 0:
+            return
+        self._call("mdct", "mdct", di, si, pi, in_len, pw, int(bool(center)), code, po, batch)
+
+    def imdct(self, input, window, output, center=True, norm="backward"):
+        """Inverse of mdct: `input` (shape (..., F, N)) -> `output` (shape (..., out_len), any out_len >= 1).  Output i
+        is the overlap-add of window * v_f over the frames covering padded position t = i + pad (pad = N if center),
+        v_f the unfolded dct4 of frame f with the norm's backward and forward swapped, with no division: the aliasing
+        cancels between frames.  With center, out_len = L and a Princen-Bradley window (w[s]^2 + w[s+N]^2 = 1, w
+        symmetric), imdct(mdct(x)) = x in every norm.  Without center and out_len = (F + 1) N this is
+        tf.signal.inverse_mdct.  Out of place only."""
+        self._check_resolved(input, window, output)
+        code = self._check_norm(norm)
+        n = self._size
+        if getattr(input, "ndim", 0) < 2 or input.shape[-2] < 1:
+            raise ValueError(f"input must have shape (..., F, {n}) with F >= 1")
+        frames = int(input.shape[-2])
+        out_len = output.shape[-1] if getattr(output, "ndim", 0) > 0 else 0
+        if out_len < 1:
+            raise ValueError("output rows must hold at least one sample")
+        pi, li, di, si = self._describe(input, "real")
+        pw, dw = self._mdct_window(window)
+        po, lo, do_, _ = self._describe(output, "real", last=out_len)
+        if li[:-1] != lo:
+            raise ValueError(f"input and output leading shapes differ: {li[:-1]} and {lo}")
+        if not (di == dw == do_):
+            raise ValueError("input, window and output must all be host or all be device buffers")
+        batch = int(np.prod(lo, dtype=np.int64))
+        if batch == 0:
+            return
+        self._call("imdct", "imdct", di, si, pi, frames, pw, int(bool(center)), code, po, out_len, batch)
 
     WELCH_SCALINGS = {"density": 0, "spectrum": 1}
     WELCH_DETRENDS = {False: 0, "constant": 1}

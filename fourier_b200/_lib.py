@@ -38,7 +38,9 @@ EXTENSION_SYMBOLS = (
     + [f"fourier_b200_welch_{op}{t}" for t in ("float", "double") for op in ("", "async_")]
     + [f"fourier_b200_{fn}_{op}{t}" for fn in ("csd", "coherence") for t in ("float", "double") for op in ("", "async_")]
     + [f"fourier_b200_dct_{op}{t}" for t in ("float", "double") for op in ("", "async_")]
-    + [f"fourier_b200_hilbert_{op}{t}" for t in ("float", "double") for op in ("", "async_")])
+    + [f"fourier_b200_hilbert_{op}{t}" for t in ("float", "double") for op in ("", "async_")]
+    + [f"fourier_b200_{fn}_{op}{t}" for fn in ("dct4", "mdct", "imdct") for t in ("float", "double")
+       for op in ("", "async_")])
 
 
 def load():
@@ -111,6 +113,12 @@ def load():
         getattr(L, f"fourier_b200_dct_async_{t}").argtypes = [vp, vp, vp, sz, ci, ci, vp]
         getattr(L, f"fourier_b200_hilbert_{t}").argtypes = [vp, vp, vp, sz, ci]
         getattr(L, f"fourier_b200_hilbert_async_{t}").argtypes = [vp, vp, vp, sz, ci, vp]
+        getattr(L, f"fourier_b200_dct4_{t}").argtypes = [vp, vp, vp, sz, ci]
+        getattr(L, f"fourier_b200_dct4_async_{t}").argtypes = [vp, vp, vp, sz, ci, vp]
+        getattr(L, f"fourier_b200_mdct_{t}").argtypes = [vp, vp, sz, vp, ci, ci, vp, sz]
+        getattr(L, f"fourier_b200_mdct_async_{t}").argtypes = [vp, vp, sz, vp, ci, ci, vp, sz, vp]
+        getattr(L, f"fourier_b200_imdct_{t}").argtypes = [vp, vp, sz, vp, ci, ci, vp, sz, sz]
+        getattr(L, f"fourier_b200_imdct_async_{t}").argtypes = [vp, vp, sz, vp, ci, ci, vp, sz, sz, vp]
     L.fourier_b200_peer_alloc.argtypes = [sz, ctypes.POINTER(vp), ctypes.c_char_p]
     L.fourier_b200_peer_open.argtypes = [ctypes.c_char_p, ctypes.POINTER(vp)]
     L.fourier_b200_peer_close.argtypes = [vp]

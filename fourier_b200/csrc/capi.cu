@@ -482,6 +482,99 @@ int hilbert_exec(void* plan, const T* in, void* out, size_t batch, int output, b
       {in, out}, [&](cudaStream_t s) { return p->hilbert_device(in, out, batch, output, s); });
 }
 
+// Type-IV DCT, MDCT and IMDCT of real rows (DESIGN.md §4.20): the arguments that need no plan checked first, even for
+// batch == 0, each refusal naming its argument; then an odd plan length.
+const char* bad_norm(int norm) {
+  return norm < 0 || norm > 2 ? "unknown norm (FOURIER_B200_DCT_NORM_BACKWARD, _ORTHO or _FORWARD)" : nullptr;
+}
+template <typename T> bool even_plan(const RealPlan<T>* p, const char* what) {
+  if (p->size() % 2 == 0) return true;
+  fb200::set_last_error(std::string(what) + " needs an even plan length N");
+  return false;
+}
+
+// dct4: in == out allowed, otherwise disjoint
+template <typename T>
+int dct4_exec(void* plan, const T* in, T* out, size_t batch, int norm, bool async, void* stream) {
+  const char* bad = !plan ? "null argument: plan" : !in ? "null argument: in" : !out ? "null argument: out" : bad_norm(norm);
+  if (bad) { fb200::set_last_error(bad); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  if (!even_plan(p, "the type-IV DCT")) return (int)cudaErrorInvalidValue;
+  return run_call(
+      "dct4", async, stream,
+      [&] {
+        if (batch == 0) return (int)p->dct4_device(in, out, 0, norm, nullptr);
+        const size_t bytes = batch * p->size() * sizeof(T);
+        if (in != out && ranges_meet(in, bytes, out, bytes)) {
+          fb200::set_last_error("input and output overlap (they must be the same buffer or disjoint)");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {in, out}, "input and output must both be host or both be device memory",
+      [&] { return p->dct4_host(in, out, batch, norm); },
+      {in, out}, [&](cudaStream_t s) { return p->dct4_device(in, out, batch, norm, s); });
+}
+
+// mdct: out of place only; the window (2N reals) must not overlap the output either
+template <typename T>
+int mdct_exec(void* plan, const T* in, size_t in_len, const T* window, int center, int norm, T* out, size_t batch,
+              bool async, void* stream) {
+  const char* bad = !plan ? "null argument: plan" : !in ? "null argument: in" : !window ? "null argument: window"
+                    : !out ? "null argument: out" : in_len == 0 ? "in_len must be at least 1" : bad_norm(norm);
+  if (bad) { fb200::set_last_error(bad); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  if (!even_plan(p, "the MDCT")) return (int)cudaErrorInvalidValue;
+  const size_t n = p->size();
+  if (!center && in_len < 2 * n) {
+    fb200::set_last_error("in_len must be at least 2N without center");
+    return (int)cudaErrorInvalidValue;
+  }
+  return run_call(
+      "mdct", async, stream,
+      [&] {
+        if (batch == 0) return (int)p->mdct_device(in, in_len, window, center != 0, norm, out, 0, nullptr);
+        const size_t in_bytes = batch * in_len * sizeof(T);
+        const size_t out_bytes = batch * p->mdct_frames(in_len, center != 0) * n * sizeof(T);
+        if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, 2 * n * sizeof(T), out, out_bytes)) {
+          fb200::set_last_error("input or window and output overlap (the mdct is out of place only)");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {in, window, out}, "input, window and output must all be host or all be device memory",
+      [&] { return p->mdct_host(in, in_len, window, center != 0, norm, out, batch); },
+      {in, out}, [&](cudaStream_t s) { return p->mdct_device(in, in_len, window, center != 0, norm, out, batch, s); });
+}
+
+// imdct: out of place only; the window (2N reals) must not overlap the output either
+template <typename T>
+int imdct_exec(void* plan, const T* in, size_t frames, const T* window, int center, int norm, T* out, size_t out_len,
+               size_t batch, bool async, void* stream) {
+  const char* bad = !plan ? "null argument: plan" : !in ? "null argument: in" : !window ? "null argument: window"
+                    : !out ? "null argument: out" : frames == 0 ? "frames must be at least 1"
+                    : out_len == 0 ? "out_len must be at least 1" : bad_norm(norm);
+  if (bad) { fb200::set_last_error(bad); return (int)cudaErrorInvalidValue; }
+  auto* p = static_cast<RealPlan<T>*>(plan);
+  if (!even_plan(p, "the IMDCT")) return (int)cudaErrorInvalidValue;
+  const size_t n = p->size();
+  return run_call(
+      "imdct", async, stream,
+      [&] {
+        if (batch == 0) return (int)p->imdct_device(in, frames, window, center != 0, norm, out, out_len, 0, nullptr);
+        const size_t in_bytes = batch * frames * n * sizeof(T), out_bytes = batch * out_len * sizeof(T);
+        if (ranges_meet(in, in_bytes, out, out_bytes) || ranges_meet(window, 2 * n * sizeof(T), out, out_bytes)) {
+          fb200::set_last_error("input or window and output overlap (the imdct is out of place only)");
+          return (int)cudaErrorInvalidValue;
+        }
+        return kRun;
+      },
+      {in, window, out}, "input, window and output must all be host or all be device memory",
+      [&] { return p->imdct_host(in, frames, window, center != 0, norm, out, out_len, batch); },
+      {in, out},
+      [&](cudaStream_t s) { return p->imdct_device(in, frames, window, center != 0, norm, out, out_len, batch, s); });
+}
+
 // Cross-spectral density (coh false) and coherence of real rows: welch_exec's rules for x, the window, hop, detrend
 // (and for the csd scaling and fs), plus y and y_rows, checked before the plan is touched; y may overlap x.
 template <typename T>
@@ -995,6 +1088,59 @@ int fourier_b200_hilbert_async_float(fourier_b200_rfft_float* plan, const float*
 int fourier_b200_hilbert_async_double(fourier_b200_rfft_double* plan, const double* in_dev, void* out_dev, size_t batch,
                                       int output, void* stream) {
   return hilbert_exec<double>(plan, in_dev, out_dev, batch, output, true, stream);
+}
+
+int fourier_b200_dct4_float(fourier_b200_rfft_float* plan, const float* in, float* out, size_t batch, int norm) {
+  return dct4_exec<float>(plan, in, out, batch, norm, false, nullptr);
+}
+int fourier_b200_dct4_double(fourier_b200_rfft_double* plan, const double* in, double* out, size_t batch, int norm) {
+  return dct4_exec<double>(plan, in, out, batch, norm, false, nullptr);
+}
+int fourier_b200_dct4_async_float(fourier_b200_rfft_float* plan, const float* in_dev, float* out_dev, size_t batch,
+                                  int norm, void* stream) {
+  return dct4_exec<float>(plan, in_dev, out_dev, batch, norm, true, stream);
+}
+int fourier_b200_dct4_async_double(fourier_b200_rfft_double* plan, const double* in_dev, double* out_dev, size_t batch,
+                                   int norm, void* stream) {
+  return dct4_exec<double>(plan, in_dev, out_dev, batch, norm, true, stream);
+}
+
+int fourier_b200_mdct_float(fourier_b200_rfft_float* plan, const float* in, size_t in_len, const float* window,
+                            int center, int norm, float* out, size_t batch) {
+  return mdct_exec<float>(plan, in, in_len, window, center, norm, out, batch, false, nullptr);
+}
+int fourier_b200_mdct_double(fourier_b200_rfft_double* plan, const double* in, size_t in_len, const double* window,
+                             int center, int norm, double* out, size_t batch) {
+  return mdct_exec<double>(plan, in, in_len, window, center, norm, out, batch, false, nullptr);
+}
+int fourier_b200_mdct_async_float(fourier_b200_rfft_float* plan, const float* in_dev, size_t in_len,
+                                  const float* window_dev, int center, int norm, float* out_dev, size_t batch,
+                                  void* stream) {
+  return mdct_exec<float>(plan, in_dev, in_len, window_dev, center, norm, out_dev, batch, true, stream);
+}
+int fourier_b200_mdct_async_double(fourier_b200_rfft_double* plan, const double* in_dev, size_t in_len,
+                                   const double* window_dev, int center, int norm, double* out_dev, size_t batch,
+                                   void* stream) {
+  return mdct_exec<double>(plan, in_dev, in_len, window_dev, center, norm, out_dev, batch, true, stream);
+}
+
+int fourier_b200_imdct_float(fourier_b200_rfft_float* plan, const float* in, size_t frames, const float* window,
+                             int center, int norm, float* out, size_t out_len, size_t batch) {
+  return imdct_exec<float>(plan, in, frames, window, center, norm, out, out_len, batch, false, nullptr);
+}
+int fourier_b200_imdct_double(fourier_b200_rfft_double* plan, const double* in, size_t frames, const double* window,
+                              int center, int norm, double* out, size_t out_len, size_t batch) {
+  return imdct_exec<double>(plan, in, frames, window, center, norm, out, out_len, batch, false, nullptr);
+}
+int fourier_b200_imdct_async_float(fourier_b200_rfft_float* plan, const float* in_dev, size_t frames,
+                                   const float* window_dev, int center, int norm, float* out_dev, size_t out_len,
+                                   size_t batch, void* stream) {
+  return imdct_exec<float>(plan, in_dev, frames, window_dev, center, norm, out_dev, out_len, batch, true, stream);
+}
+int fourier_b200_imdct_async_double(fourier_b200_rfft_double* plan, const double* in_dev, size_t frames,
+                                    const double* window_dev, int center, int norm, double* out_dev, size_t out_len,
+                                    size_t batch, void* stream) {
+  return imdct_exec<double>(plan, in_dev, frames, window_dev, center, norm, out_dev, out_len, batch, true, stream);
 }
 
 const char* fourier_b200_last_error(void) { return fb200::last_error(); }

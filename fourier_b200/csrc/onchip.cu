@@ -109,6 +109,8 @@ struct OnChipImpl {
     if ((e = allow_smem(onchip::onchip_dct_kernel<Cfg<true>, MINB, 3>))) return e;
     if ((e = allow_smem(onchip::onchip_hilbert_kernel<Cfg<true>, MINB, false>))) return e;
     if ((e = allow_smem(onchip::onchip_hilbert_kernel<Cfg<true>, MINB, true>))) return e;
+    if ((e = allow_smem(onchip::onchip_dct4_kernel<Cfg<true>, MINB>))) return e;
+    if ((e = allow_smem(onchip::onchip_mdct_kernel<Cfg<true>, MINB>))) return e;
     if ((e = cudaFuncSetAttribute(onchip::onchip_csd_kernel<Cfg<true>, minb_csd(false), false>,
                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_csd(false)))) return e;
     if ((e = cudaFuncSetAttribute(onchip::onchip_csd_kernel<Cfg<true>, minb_csd(true), true>,
@@ -186,6 +188,30 @@ struct OnChipImpl {
       return launch(onchip::onchip_hilbert_kernel<Cfg<true>, MINB, true>, a, batch, sms, s);
     return launch(onchip::onchip_hilbert_kernel<Cfg<true>, MINB, false>, a, batch, sms, s);
   }
+  static cudaError_t dct4(const T* in, T* out, const void* twa, const cpx<T>* wq, cpx<T> c, size_t batch, int sms,
+                          cudaStream_t s) {
+    typename onchip::Dct4Body<Cfg<true>>::Args a;
+    static_cast<typename onchip::RealBody<Cfg<true>>::Args&>(a) = {
+        nullptr, nullptr, (const TwPair<T>*)twa, nullptr, (long)batch, (T)1};
+    a.x = in;
+    a.y = out;
+    a.wq = wq;
+    a.c = c;
+    return launch(onchip::onchip_dct4_kernel<Cfg<true>, MINB>, a, batch, sms, s);
+  }
+  static cudaError_t mdct(const T* in, const T* win, T* out, const real::FrameMap& m, size_t nframes, const void* twa,
+                          const cpx<T>* wq, cpx<T> c, int sms, cudaStream_t s) {
+    typename onchip::MdctBody<Cfg<true>>::Args a;
+    static_cast<typename onchip::RealBody<Cfg<true>>::Args&>(a) = {
+        nullptr, nullptr, (const TwPair<T>*)twa, nullptr, (long)nframes, (T)1};
+    a.x = in;
+    a.y = out;
+    a.wq = wq;
+    a.c = c;
+    a.win = win;
+    a.m = m;
+    return launch(onchip::onchip_mdct_kernel<Cfg<true>, MINB>, a, nframes, sms, s);
+  }
   static cudaError_t mel(const T* in, const T* win, const T* filters, const real::Band* bands, size_t n_mels, int power,
                          T* out, const real::FrameMap& m, size_t nframes, const void* twa, const cpx<T>* tab, int sms,
                          cudaStream_t s) {
@@ -257,7 +283,7 @@ struct OnChipImpl {
   }
   static const OnChipOps<T>* ops() {
     static const RealOnChipOps<T> r = {RA, RB, Cfg<true>::C, &real_prepare, &real, &conv, &lconv, &stft, &mel, &mfcc,
-                                      &welch, &dct, &csd, &hilbert};
+                                      &welch, &dct, &csd, &hilbert, &dct4, &mdct};
     static const OnChipOps<T> o = {RA, RB, &prepare, &fft, kHasBluestein ? &bluestein : nullptr, &r};
     return &o;
   }

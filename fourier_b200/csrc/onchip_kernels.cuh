@@ -1060,6 +1060,176 @@ __global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_dct_kernel(const ty
   run_onchip_groups<Cfg, DctBody<Cfg, TYPE>>(a);
 }
 
+// ---- fused type-IV DCT and MDCT of real rows, N = 2L (real::dct4_pre / dct4_post / mdct_fold, DESIGN.md §4.20) -------
+// Dct4Body, on rows of N reals:
+//   * load (phase 0): consecutive lanes of the FFT read consecutive samples of the row and park x[2j] and x[2j+1] as
+//     z[j].x and z[L-1-j].y (reals 2j and N-1-2j), so that the park holds z[n] = (x[2n], x[N-1-2n]);
+//   * pre (phase 1): each lane multiplies the park's positions n = u, u + TP, ... by W^{2n} in place;
+//   * phases 2-5: StftBody's stage A from the park, the scatter, RealBody's gather + stage B and park: the park holds
+//     Z in natural order;
+//   * post (phase 6): each lane forms (y[2k], y[N-1-2k]) of its positions k = u + TP*j from Z[k] into tile register j;
+//   * park (phase 7): those pairs into the park as reals (no lane reads Z any more);
+//   * store (phase 8): consecutive lanes write consecutive complex values (two reals) of the row.
+// The twiddles are applied in passes over the park, with each step's index formed in its own loop iteration, as
+// Dct2Body's pairs are.  Applying them in the stage-A registers and to the stage-B registers instead kept the twiddle
+// indices and table reads live through the FFT phases: ptxas spilled 24-270 bytes at the f32 L = 128, 512 and 1024
+// register caps.
+// A row is read completely into the park before any output is stored, and only its own FFT reads it (a column past the
+// batch transforms zeros and stores nothing), so in == out is safe.
+// MdctBody, on groups of C consecutive frames (real::mdct_map): its load (phase 0) reads the frame's 2N samples as
+// StftBody's does (unmasked inside the row, through FrameMap::Edge at its ends, so no read leaves [0, L)), windows and
+// folds them, and parks the N folded values in Dct4Body's packing; frame q of the launch writes output row q (frame-major,
+// N reals per frame).  The rest is Dct4Body's.
+template <class Cfg> struct Dct4Body {
+  using Stft = StftBody<Cfg>;
+  using Real = RealBody<Cfg>;
+  using Tile = typename Cfg::Tile;   // FWD = true
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  static constexpr int L = Cfg::L, TP = Tile::TP, E = Tile::E;
+  // Real::Args with in = out = nullptr; x, y: rows of N = 2L reals (x == y allowed); wq: W^k, k <= L; c: the post
+  // step's constant (real::dct4_const)
+  struct Args : Real::Args { const T* x; T* y; const V* wq; V c; };
+
+  static FB_HD long row(long grp, int t) { return grp * Cfg::C + Tile::template col_of<true>(t); }
+
+  static FB_HD void load(const Args& a, long grp, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const long b = row(grp, t);
+    T* z = reinterpret_cast<T*>(smem + Real::park(t));
+    if (b >= a.batch) {
+      for (int p = u; p < 2 * L; p += TP) z[p] = (T)0;
+      return;
+    }
+    const T* src = a.x + b * (2 * L);
+    // sample p at real p (even) or N - p (odd) of the park
+#pragma unroll 2
+    for (int p = u; p < 2 * L; p += TP) z[(p & 1) ? 2 * L - p : p] = real::lin_ld(src + p, b);
+  }
+  // z[n] *= W^{2n} at the lane's positions, in place
+  static FB_HD void pre(const Args& a, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    V* z = smem + Real::park(t);
+#pragma unroll 4
+    for (int j = 0; j < E; ++j) {
+      const int n = u + TP * j;
+      const V v = z[n];
+      z[n] = real::dct4_pre(v.x, v.y, a.wq, (long)(2 * L), (long)n);
+    }
+  }
+  // (y[2k], y[N-1-2k]) of the lane's positions k = u + TP*j into tile register j
+  static FB_HD void post(Tile& f, const Args& a, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const V* z = smem + Real::park(t);
+#pragma unroll
+    for (int j = 0; j < E; ++j) {
+      const int k = u + TP * j;
+      f.v[j] = real::dct4_post(z[k], a.c, a.wq, (long)(2 * L), (long)k);
+    }
+  }
+  static FB_HD void park_out(const Tile& f, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    T* y = reinterpret_cast<T*>(smem + Real::park(t));
+#pragma unroll
+    for (int j = 0; j < E; ++j) {
+      const int k = u + TP * j;
+      y[2 * k] = f.v[j].x;
+      y[2 * L - 1 - 2 * k] = f.v[j].y;
+    }
+  }
+  // out: the row's N reals
+  static FB_HD void store(T* out, long g, int t, const V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    const V* y = smem + Real::park(t);
+    V* dst = reinterpret_cast<V*>(out);
+#pragma unroll 2
+    for (int j = u; j < L; j += TP) real::lin_st(dst + j, y[j], g);
+  }
+
+  // phase protocol (tilefft.cuh): load into the park; pre-twiddle in the park; StftBody's stage A and scatter;
+  // RealBody's gather + stage B and park; post into registers, park, store
+  static constexpr int kPhases = 9;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    if constexpr (P == 0) load(a, grp, t, smem);
+    else if constexpr (P == 1) pre(a, t, smem);
+    else if constexpr (P == 2) Stft::load_stage_a(f, t, smem, twa);
+    else if constexpr (P == 3) f.template scatter<true, typename Cfg::Lay>(t, smem);
+    else if constexpr (P == 4) Real::fwd_gather(f, t, smem);
+    else if constexpr (P == 5) Real::fwd_park(f, t, smem);
+    else if constexpr (P == 6) post(f, a, t, smem);
+    else if constexpr (P == 7) park_out(f, t, smem);
+    else {
+      const long b = row(grp, t);
+      if (b < a.batch) store(a.y + b * (2 * L), b, t, smem);
+    }
+  }
+};
+
+template <class Cfg> struct MdctBody {
+  using Dct4 = Dct4Body<Cfg>;
+  using Real = RealBody<Cfg>;
+  using Tile = typename Cfg::Tile;   // FWD = true
+  using V = typename Tile::V;
+  using T = decltype(V::x);
+  static constexpr int L = Cfg::L, TP = Tile::TP;
+  // Dct4::Args with x = the rows, y = the output of frame g0, batch = frames of the launch; plus the window (2N reals)
+  // and the frame map (real::mdct_map)
+  struct Args : Dct4::Args { const T* win; real::FrameMap m; };
+
+  static FB_HD void load(const Args& a, long grp, int t, V* smem) {
+    const int u = Tile::template u_of<true>(t);
+    long q = Dct4::row(grp, t);
+    if (q >= a.batch) q = a.batch - 1;
+    const long g = a.m.g0 + q, b = a.m.row_of(g), t0 = a.m.start(g, b);
+    const T* row = a.x + (b - a.m.r0) * a.m.in_ld;
+    T* z = reinterpret_cast<T*>(smem + Real::park(t));
+    constexpr int N = 2 * L;
+    // folded value n of the frame into the park: n even at n, n odd at N - n (z[j] = (u[2j], u[N-1-2j]))
+    auto put = [&](int n, T f0, T f1) FB_LAMBDA { z[(n & 1) ? N - n : n] = real::mdct_fold(f0, f1, (long)n, (long)N); };
+    if (t0 >= 0 && t0 + 2 * N <= a.m.len) {
+      const T* src = row + t0;
+#pragma unroll 2
+      for (int n = u; n < N; n += TP) {
+        long s0, s1;
+        real::mdct_fold_pos(n, N, s0, s1);
+        put(n, real::lin_ld(src + s0, g) * a.win[s0], real::lin_ld(src + s1, g) * a.win[s1]);
+      }
+    } else {
+      // 32-bit offsets from an anchor sample c of the row (see FrameMap::edge)
+      const real::FrameMap::Edge e = a.m.edge(t0);
+      const T* src = row + e.c;
+#pragma unroll 2
+      for (int n = u; n < N; n += TP) {
+        long s0, s1;
+        real::mdct_fold_pos(n, N, s0, s1);
+        const int d0 = e.map(e.d0 + (int)s0), d1 = e.map(e.d0 + (int)s1);
+        put(n, e.in(d0) ? real::lin_ld(src + d0, g) * a.win[s0] : (T)0,
+            e.in(d1) ? real::lin_ld(src + d1, g) * a.win[s1] : (T)0);
+      }
+    }
+  }
+
+  // phase protocol (tilefft.cuh): the frame folded into the park; Dct4Body's phases 1-7; store
+  static constexpr int kPhases = Dct4::kPhases;
+  template <int P> static FB_HD void phase(Tile& f, const Args& a, long grp, int t, V* smem, const TwPair<T>* twa) {
+    if constexpr (P == 0) load(a, grp, t, smem);
+    else if constexpr (P < kPhases - 1) Dct4::template phase<P>(f, a, grp, t, smem, twa);
+    else {
+      const long q = Dct4::row(grp, t);
+      if (q < a.batch) Dct4::store(a.y + q * (2 * L), a.m.g0 + q, t, smem);
+    }
+  }
+};
+
+template <class Cfg, int MINB>
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_dct4_kernel(const typename Dct4Body<Cfg>::Args a) {
+  run_onchip_groups<Cfg, Dct4Body<Cfg>>(a);
+}
+template <class Cfg, int MINB>
+__global__ void __launch_bounds__(Cfg::THREADS, MINB) onchip_mdct_kernel(const typename MdctBody<Cfg>::Args a) {
+  run_onchip_groups<Cfg, MdctBody<Cfg>>(a);
+}
+
 // ---- fused analytic signal and envelope of real rows, N = 2L (real::hilbert_pair, DESIGN.md §4.19) -----------------
 // ConvBody's phases 0-5 as they are, with the pair step real::hilbert_pair (a fixed multiplier, no spectrum read) in
 // phase 3.  Then:

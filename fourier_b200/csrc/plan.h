@@ -337,6 +337,14 @@ template <typename T> struct RealOnChipOps {
   // into N complex values or N reals per row, out == in allowed for the envelope; h = 1 / (2N)
   cudaError_t (*hilbert)(const T* in, void* out, int output, const void* twa, const cpx<T>* tab, size_t batch, T h,
                          int sms, cudaStream_t);
+  // dct4(): the type-IV DCT (DESIGN.md §4.20) of `batch` rows of N reals, in == out allowed; wq = W^k, k <= L; c from
+  // real::dct4_const
+  cudaError_t (*dct4)(const T* in, T* out, const void* twa, const cpx<T>* wq, cpx<T> c, size_t batch, int sms,
+                      cudaStream_t);
+  // mdct(): the MDCT of frames m.g0 .. m.g0 + nframes - 1 of m (real::mdct_map), frame q of the launch writing its N
+  // coefficients at out + q N
+  cudaError_t (*mdct)(const T* in, const T* win, T* out, const real::FrameMap& m, size_t nframes, const void* twa,
+                      const cpx<T>* wq, cpx<T> c, int sms, cudaStream_t);
 };
 template <typename T> const RealOnChipOps<T>* real_onchip_lookup(size_t l);
 
@@ -461,6 +469,25 @@ class RealPlan {
   // Host pointers: whole rows through stage_rows; the same bits.
   cudaError_t hilbert_host(const T* in, void* out, size_t batch, int output);
 
+  // Type-IV DCT and MDCT (DESIGN.md §4.20), even N only; norm real::kDctNorm*, the other arguments checked by the caller.
+  // dct4: `batch` rows of N reals -> scipy.fft.dct(x, type=4, norm), in == out allowed.  mdct: rows of in_len samples ->
+  // F = mdct_frames(in_len, center) frames of N coefficients per row, frame-major.  imdct: rows of `frames` frames of N
+  // coefficients -> rows of out_len samples, the windowed overlap-add of the inverse.  Device pointers, on `stream`.
+  cudaError_t dct4_device(const T* in, T* out, size_t batch, int norm, cudaStream_t stream);
+  cudaError_t mdct_device(const T* in, size_t in_len, const T* win, bool center, int norm, T* out, size_t batch,
+                          cudaStream_t stream);
+  cudaError_t imdct_device(const T* in, size_t frames, const T* win, bool center, int norm, T* out, size_t out_len,
+                           size_t batch, cudaStream_t stream);
+  // Host pointers: the window once, whole rows through stage_rows; the same bits.
+  cudaError_t dct4_host(const T* in, T* out, size_t batch, int norm);
+  cudaError_t mdct_host(const T* in, size_t in_len, const T* win, bool center, int norm, T* out, size_t batch);
+  cudaError_t imdct_host(const T* in, size_t frames, const T* win, bool center, int norm, T* out, size_t out_len,
+                         size_t batch);
+  // frames of one MDCT row of in_len samples (real::mdct_map)
+  size_t mdct_frames(size_t in_len, bool center) const {
+    return (size_t)real::mdct_map((long)n_, (long)in_len, center).frames;
+  }
+
   unsigned long long launches() const { return launches_; }
   const char* kernel_name() const { return kernel_desc_.c_str(); }
 
@@ -509,6 +536,14 @@ class RealPlan {
   cudaError_t dct_rows(const T* in, T* out, size_t batch, int type, int norm, cudaStream_t s);
   // hilbert_device after its checks: the fused kernel, or chunks of rows through seg_ (half length) or work_ (full)
   cudaError_t hilbert_rows(const T* in, void* out, size_t batch, int output, cudaStream_t s);
+  // dct4_device after its checks: the fused kernel, or chunks of rows through `scratch` (half length)
+  cudaError_t dct4_rows(const T* in, T* out, size_t batch, int norm, DeviceBuffer& scratch, cudaStream_t s);
+  // mdct_device and imdct_device after their checks: the fused kernel or chunks of frames through seg_; runs of frames
+  // (real::istft_runs) through seg_, their DCT-IV by dct4_rows (its scratch work_), then the overlap-add
+  cudaError_t mdct_rows(const T* in, size_t in_len, const T* win, bool center, int norm, T* out, size_t batch,
+                        cudaStream_t s);
+  cudaError_t imdct_rows(const T* in, size_t frames, const T* win, bool center, int norm, T* out, size_t out_len,
+                         size_t batch, cudaStream_t s);
   // the band of every filter row into bands_ (one launch)
   cudaError_t mel_bands(const T* filters, size_t n_mels, cudaStream_t s);
   // mel_device after mel_bands: the fused kernel, or chunks of frames through seg_

@@ -32,6 +32,10 @@
 // Analytic signal and envelope (DESIGN.md §4.19): onchip_hilbert_kernel on the fused path; otherwise per chunk of rows
 // through seg_: Fft of the rows read as M complex values, hilbert_pair_kernel, UnscaledIfft and hilbert_out_kernel at
 // half length; widen_kernel, Fft, hilbert_mul_kernel, UnscaledIfft and hilbert_out_kernel at full length.
+// Type-IV DCT and MDCT (DESIGN.md §4.20), even N only: onchip_dct4_kernel / onchip_mdct_kernel on the fused path;
+// otherwise per chunk of rows or frames through seg_: dct4_pre_kernel or mdct_gather_kernel, the inner Fft in place and
+// dct4_post_kernel.  The IMDCT runs the plan's own DCT-IV over runs of frames into seg_ (real::istft_runs), then
+// imdct_overlap_add_kernel, on every path.
 #include <algorithm>
 #include <string>
 #include <vector>
@@ -419,6 +423,55 @@ dct_unpermute_kernel(const void* __restrict__ seg, T* __restrict__ out, long n, 
   }
 }
 
+// Type-IV DCT and MDCT (real::dct4_pre, dct4_post, mdct_fold_one, imdct_add_one), even N = 2M.  One thread per position
+// k < M of a row or frame, consecutive threads along it.  pre: z[k] of the rows into z (M complex values per row);
+// mdct gather: z[k] of the windowed, folded frames q of the launch (global frame m.g0 + q) into z; post: (y[2k],
+// y[N-1-2k]) from Z[k] in z into the output rows (row b of the launch is row g0 + b, for the emulator's log).
+// overlap-add: one thread per output i0 <= i < i1 of rows b0 .. b0 + nb - 1, as overlap_add_kernel.
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+dct4_pre_kernel(const T* __restrict__ in, cpx<T>* __restrict__ z, const cpx<T>* __restrict__ wq, long n, long batch) {
+  const long m = n / 2, total = m * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / m, k = g - b * m;
+    const T* x = in + b * n;
+    z[g] = real::dct4_pre(real::lin_ld(x + 2 * k, b), real::lin_ld(x + (n - 1 - 2 * k), b), wq, n, k);
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+mdct_gather_kernel(const T* __restrict__ in, const T* __restrict__ win, cpx<T>* __restrict__ z, const real::FrameMap m,
+                   const cpx<T>* __restrict__ wq, long nframes) {
+  const long n = m.hop, half = n / 2, total = half * nframes;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long q = g / half, k = g - q * half;
+    z[g] = real::dct4_pre(real::mdct_fold_one(m, in, win, q, 2 * k), real::mdct_fold_one(m, in, win, q, n - 1 - 2 * k),
+                          wq, n, k);
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+dct4_post_kernel(const cpx<T>* __restrict__ z, T* __restrict__ out, const cpx<T>* __restrict__ wq, cpx<T> c, long n,
+                 long batch, long g0) {
+  const long m = n / 2, total = m * batch;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / m, k = g - b * m;
+    const cpx<T> p = real::dct4_post(z[g], c, wq, n, k);
+    real::lin_st(out + b * n + 2 * k, p.x, g0 + b);
+    real::lin_st(out + b * n + (n - 1 - 2 * k), p.y, g0 + b);
+  }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+imdct_overlap_add_kernel(const T* __restrict__ seg, const T* __restrict__ win, T* __restrict__ out,
+                         const real::FrameMap m, long gs, long b0, long nb, long i0, long i1, long out_ld) {
+  const long cnt = i1 - i0, total = nb * cnt;
+  for (long g = blockIdx.x * (long)blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long r = g / cnt;
+    real::imdct_add_one(m, seg, win, gs, out + r * out_ld, b0 + r, i0 + (g - r * cnt));
+  }
+}
+
 // Analytic signal (real::hilbert_pair, hilbert_bin, hilbert_out_one).  pair: one thread per pair k <= M/2 of a row, in
 // place on z (M complex values per row).  mul: one thread per bin k < N of a row of length-N spectra, in place.  out: one
 // thread per output n of a row, from x[n] and y[n] (seg holds N reals per row at half length, N complex values whose
@@ -455,6 +508,13 @@ __global__ void __launch_bounds__(kThreads)
 real_part_kernel(const cpx<T>* __restrict__ y, T* __restrict__ out, size_t count) {
   for (size_t g = blockIdx.x * (size_t)blockDim.x + threadIdx.x; g < count; g += (size_t)gridDim.x * blockDim.x)
     out[g] = y[g].x;
+}
+
+// the DCT-IV's post-step constant c of a norm (real::dct4_const), rounded once
+template <typename T> cpx<T> dct4_c(int norm, size_t n) {
+  double re, im;
+  real::dct4_const(norm, (long)n, re, im);
+  return mk<T>((T)re, (T)im);
 }
 
 // Items of item_bytes that one chunk of plan scratch holds: as many as fit kScratchTargetBytes, at least 1, at most total.
@@ -1376,6 +1436,152 @@ cudaError_t RealPlan<T>::hilbert_host(const T* in, void* out, size_t batch, int 
   return stage_rows(in, out, batch, n_ * sizeof(T), out_row, [&](const void* din, void* dout, size_t, size_t nb) {
     return hilbert_rows((const T*)din, dout, nb, output, host_stream_);
   });
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::dct4_device(const T* in, T* out, size_t batch, int norm, cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  return dct4_rows(in, out, batch, norm, seg_, s);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::dct4_rows(const T* in, T* out, size_t batch, int norm, DeviceBuffer& scratch, cudaStream_t s) {
+  const C c = dct4_c<T>(norm, n_);
+  const C* wq = (const C*)dct_tab_.data();
+  if (path_ == Path::kRealFused) {
+    FB_CHECK(fused_->dct4(in, out, twa_.data(), wq, c, batch, sm_count_, s));
+    launches_ += 1;
+    return cudaSuccess;
+  }
+  // chunks of rows through scratch, M complex values per row; the pre kernel reads the chunk's rows whole and only the
+  // post kernel writes them, so in == out is safe
+  const size_t chunk = scratch_chunk(batch, n_ * sizeof(T));
+  FB_CHECK(scratch.reserve(chunk * n_ * sizeof(T)));
+  C* z = (C*)scratch.data();
+  for (size_t b0 = 0; b0 < batch; b0 += chunk) {
+    const size_t nb = std::min(chunk, batch - b0);
+    dct4_pre_kernel<T><<<grid_for(nb * m_), kThreads, 0, s>>>(in + b0 * n_, z, wq, (long)n_, (long)nb);
+    FB_CHECK(cudaGetLastError());
+    FB_CHECK(inner_->exec_device(z, z, nb, kFft, s));
+    dct4_post_kernel<T><<<grid_for(nb * m_), kThreads, 0, s>>>(z, out + b0 * n_, wq, c, (long)n_, (long)nb, (long)b0);
+    FB_CHECK(cudaGetLastError());
+    launches_ += 2 + inner_->launches();
+  }
+  return cudaSuccess;
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::dct4_host(const T* in, T* out, size_t batch, int norm) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  return stage_rows(in, out, batch, n_ * sizeof(T), n_ * sizeof(T), [&](const void* din, void* dout, size_t, size_t nb) {
+    return dct4_rows((const T*)din, (T*)dout, nb, norm, seg_, host_stream_);
+  });
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::mdct_device(const T* in, size_t in_len, const T* win, bool center, int norm, T* out,
+                                     size_t batch, cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  return mdct_rows(in, in_len, win, center, norm, out, batch, s);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::mdct_rows(const T* in, size_t in_len, const T* win, bool center, int norm, T* out,
+                                   size_t batch, cudaStream_t s) {
+  const real::FrameMap m = real::mdct_map((long)n_, (long)in_len, center);
+  const size_t total = batch * (size_t)m.frames;
+  const C c = dct4_c<T>(norm, n_);
+  const C* wq = (const C*)dct_tab_.data();
+  if (path_ == Path::kRealFused) {
+    FB_CHECK(fused_->mdct(in, win, out, m, total, twa_.data(), wq, c, sm_count_, s));
+    launches_ += 1;
+    return cudaSuccess;
+  }
+  // chunks of frames through seg_: the gather frames, windows, folds and pre-twiddles them, the inner plan transforms
+  // them in place, and the post kernel writes their coefficients
+  const size_t chunk = scratch_chunk(total, n_ * sizeof(T));
+  FB_CHECK(seg_.reserve(chunk * n_ * sizeof(T)));
+  C* z = (C*)seg_.data();
+  for (size_t q0 = 0; q0 < total; q0 += chunk) {
+    const size_t nq = std::min(chunk, total - q0);
+    real::FrameMap mc = m;
+    mc.g0 = (long)q0;
+    mdct_gather_kernel<T><<<grid_for(nq * m_), kThreads, 0, s>>>(in, win, z, mc, wq, (long)nq);
+    FB_CHECK(cudaGetLastError());
+    FB_CHECK(inner_->exec_device(z, z, nq, kFft, s));
+    dct4_post_kernel<T><<<grid_for(nq * m_), kThreads, 0, s>>>(z, out + q0 * n_, wq, c, (long)n_, (long)nq, (long)q0);
+    FB_CHECK(cudaGetLastError());
+    launches_ += 2 + inner_->launches();
+  }
+  return cudaSuccess;
+}
+
+// Runs of frames through seg_ (real::istft_runs with frames of 2N samples every N): each run's DCT-IV goes into seg_
+// (dct4_rows, its own scratch in work_), then imdct_overlap_add_kernel writes the outputs the run owns.  Every output
+// is written once, by the same sum in the same order wherever the runs are cut.
+template <typename T>
+cudaError_t RealPlan<T>::imdct_device(const T* in, size_t frames, const T* win, bool center, int norm, T* out,
+                                      size_t out_len, size_t batch, cudaStream_t s) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  return imdct_rows(in, frames, win, center, norm, out, out_len, batch, s);
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::imdct_rows(const T* in, size_t frames, const T* win, bool center, int norm, T* out,
+                                    size_t out_len, size_t batch, cudaStream_t s) {
+  real::FrameMap m = real::mdct_map((long)n_, 2 * (long)n_, center);
+  m.frames = (long)frames;
+  m.rcp = 1.0 / (double)frames;
+  const int inv = real::dct_swapped_norm(norm);
+  // cap <= batch * frames: istft_scratch_frames raises the chunk to at most `frames`
+  const size_t cap = real::istft_scratch_frames(scratch_chunk(batch * frames, n_ * sizeof(T)), 2 * n_, n_, frames);
+  FB_CHECK(seg_.reserve(cap * n_ * sizeof(T)));
+  T* seg = (T*)seg_.data();
+  return (cudaError_t)real::istft_runs(2 * n_, n_, (size_t)m.pad, frames, out_len, batch, cap,
+                                       [&](size_t gs, size_t ge, size_t b0, size_t nb, size_t i0, size_t i1) -> int {
+    FB_CHECK(dct4_rows(in + gs * n_, seg, ge - gs, inv, work_, s));
+    imdct_overlap_add_kernel<T><<<grid_for(nb * (i1 - i0)), kThreads, 0, s>>>(
+        seg, win, out + b0 * out_len, m, (long)gs, (long)b0, (long)nb, (long)i0, (long)i1, (long)out_len);
+    FB_CHECK(cudaGetLastError());
+    launches_ += 1;
+    return 0;
+  });
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::mdct_host(const T* in, size_t in_len, const T* win, bool center, int norm, T* out,
+                                   size_t batch) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  const T* dwin;
+  FB_CHECK(stage_consts(win, 2 * n_ * sizeof(T), &dwin));
+  return stage_rows(in, out, batch, in_len * sizeof(T), mdct_frames(in_len, center) * n_ * sizeof(T),
+                    [&](const void* din, void* dout, size_t, size_t nb) {
+                      return mdct_rows((const T*)din, in_len, dwin, center, norm, (T*)dout, nb, host_stream_);
+                    });
+}
+
+template <typename T>
+cudaError_t RealPlan<T>::imdct_host(const T* in, size_t frames, const T* win, bool center, int norm, T* out,
+                                    size_t out_len, size_t batch) {
+  launches_ = 0;
+  if (batch == 0) return cudaSuccess;
+  DeviceGuard g(device_);
+  const T* dwin;
+  FB_CHECK(stage_consts(win, 2 * n_ * sizeof(T), &dwin));
+  return stage_rows(in, out, batch, frames * n_ * sizeof(T), out_len * sizeof(T),
+                    [&](const void* din, void* dout, size_t, size_t nb) {
+                      return imdct_rows((const T*)din, frames, dwin, center, norm, (T*)dout, out_len, nb, host_stream_);
+                    });
 }
 
 template class RealPlan<float>;

@@ -537,6 +537,62 @@ int fourier_b200_hilbert_async_float(struct fourier_b200_rfft_float *plan, const
 int fourier_b200_hilbert_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev, void *out_dev,
                                       size_t batch, int output, void *cuda_stream);
 
+/* ---- type-IV DCT, MDCT and IMDCT of real rows ----
+ * On a real plan of even length N (odd N is refused), h the norm's scale as for the DCT (FOURIER_B200_DCT_NORM_*:
+ * 1, 1 / sqrt(2N) or 1 / (2N); type IV has no bin-0 scale), and h' the scale of the norm with backward and forward
+ * swapped:
+ *   dct4:  y[k] = 2 h sum_{n<N} x[n] cos(pi (2n+1)(2k+1) / (4N)) for `batch` rows of N reals (row b at element b*N),
+ *          scipy.fft.dct(x, type=4, norm); its inverse is dct4 with the swapped norm (scipy.fft.idct(type=4)).  in == out
+ *          transforms in place.
+ *   mdct:  N coefficients per frame of 2N samples every N, times `window` (2N reals):
+ *          X_f[k] = 2 h sum_{s<2N} w[s] x~[fN - pad + s] cos(pi/N (s + 1/2 + N/2)(k + 1/2)), k < N, x~ = 0 outside the
+ *          row.  center != 0: pad = N and F = ceil(in_len / N) + 1 frames, every sample in two frames; center == 0:
+ *          pad = 0 and F = 1 + (in_len - 2N) / N frames (in_len >= 2N), tf.signal.mdct(x, 2N, window_fn,
+ *          pad_end=False).  Rows of in_len reals (row b at element b*in_len) -> F frames of N reals per row
+ *          (row b at element b*F*N, frame-major).
+ *   imdct: y[i] = sum_f w[t - fN] v_f[t - fN], t = i + pad, over the frames f < `frames` with 0 <= t - fN < 2N in
+ *          ascending f, v_f[s] = 2 h' sum_k X_f[k] cos(pi/N (s + 1/2 + N/2)(k + 1/2)); no envelope division.  Rows of
+ *          frames*N reals -> rows of out_len >= 1 reals (0 where no frame covers t).  With center, out_len = in_len and
+ *          a Princen-Bradley window (w[s]^2 + w[s+N]^2 = 1, w symmetric: sine, Vorbis, KBD), imdct(mdct(x)) = x in
+ *          every norm.
+ * Launches: dct4 and mdct 1 on the real_fused path (N = 128 .. 2048 in f32, 128 .. 512 in f64); on real_half (other
+ * even N), per scratch chunk of rows or frames (512 MB), 2 plus those of the inner complex plan of length N/2.  imdct,
+ * per run of frames through the plan's scratch: the dct4 of the run's frames, then 1 overlap-add kernel.
+ * Refused with cudaErrorInvalidValue and a message naming the argument, also when batch == 0 (which otherwise succeeds
+ * and launches nothing): a NULL argument, a norm other than the three macros, in_len == 0, frames == 0 and
+ * out_len == 0.  Also refused: an odd plan length, in_len < 2N without center, an output that overlaps the input or the
+ * window (dct4: in == out is allowed, a partial overlap is not), and a mix of host and device buffers in the
+ * synchronous calls.  Device base pointers must be 16-byte aligned (cudaErrorMisalignedAddress).  Host memory is
+ * staged through the plan's buffers (the window once, whole rows) and gives the same bits as device memory.  The
+ * _async calls take device memory, are enqueued on `cuda_stream` and never synchronise the host. */
+int fourier_b200_dct4_float(struct fourier_b200_rfft_float *plan, const float *in, float *out, size_t batch, int norm);
+int fourier_b200_dct4_double(struct fourier_b200_rfft_double *plan, const double *in, double *out, size_t batch,
+                             int norm);
+int fourier_b200_dct4_async_float(struct fourier_b200_rfft_float *plan, const float *in_dev, float *out_dev,
+                                  size_t batch, int norm, void *cuda_stream);
+int fourier_b200_dct4_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev, double *out_dev,
+                                   size_t batch, int norm, void *cuda_stream);
+int fourier_b200_mdct_float(struct fourier_b200_rfft_float *plan, const float *in, size_t in_len, const float *window,
+                            int center, int norm, float *out, size_t batch);
+int fourier_b200_mdct_double(struct fourier_b200_rfft_double *plan, const double *in, size_t in_len,
+                             const double *window, int center, int norm, double *out, size_t batch);
+int fourier_b200_mdct_async_float(struct fourier_b200_rfft_float *plan, const float *in_dev, size_t in_len,
+                                  const float *window_dev, int center, int norm, float *out_dev, size_t batch,
+                                  void *cuda_stream);
+int fourier_b200_mdct_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev, size_t in_len,
+                                   const double *window_dev, int center, int norm, double *out_dev, size_t batch,
+                                   void *cuda_stream);
+int fourier_b200_imdct_float(struct fourier_b200_rfft_float *plan, const float *in, size_t frames, const float *window,
+                             int center, int norm, float *out, size_t out_len, size_t batch);
+int fourier_b200_imdct_double(struct fourier_b200_rfft_double *plan, const double *in, size_t frames,
+                              const double *window, int center, int norm, double *out, size_t out_len, size_t batch);
+int fourier_b200_imdct_async_float(struct fourier_b200_rfft_float *plan, const float *in_dev, size_t frames,
+                                   const float *window_dev, int center, int norm, float *out_dev, size_t out_len,
+                                   size_t batch, void *cuda_stream);
+int fourier_b200_imdct_async_double(struct fourier_b200_rfft_double *plan, const double *in_dev, size_t frames,
+                                    const double *window_dev, int center, int norm, double *out_dev, size_t out_len,
+                                    size_t batch, void *cuda_stream);
+
 const char *fourier_b200_last_error(void);
 const char *fourier_b200_version(void);
 
